@@ -13,6 +13,8 @@ NCCL all-gather of the per-pair pointmaps the north_star prescribes before align
 `value` is device-timed with inputs resident in HBM; `e2e` goes through the public inference() API with
 pinned HOST inputs and CPU outputs.  Extra key `cloud_opt`: BASELINE configs[2] (8 views -> 28 pairs,
 PointCloudOptimizer, 300 iterations) iterations/s with its own HBM roofline.
+`--dump-outputs DIR` writes what the timed forward returned in its last step (a fixed, seeded sample of it) as
+DIR/<name>.npy, so that two builds can be compared output for output on identical inputs.
 """
 from __future__ import annotations
 
@@ -42,7 +44,8 @@ def peaks():
         p = json.load(open(path))
         return dict(hbm=p['hbm_gbs'], tf_burst=p['bf16_tflops'], tf_sustained=p.get('bf16_tflops_sustained', p['bf16_tflops']),
                     source='measured (MEASURED_PEAKS.json)')
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, source='fallback (B200_PROFILING.md)')
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0,
+                source='NVIDIA H100 SXM data sheet (HBM3 3.35 TB/s, dense BF16 989 TFLOP/s at 700 W); not a measured rate')
 
 
 def host_threads(cap=64):
@@ -168,7 +171,6 @@ def cloud_opt_section(device, pk, steps_iters=300):
     ms = float(np.median(runs))
     by = eng.algorithmic_bytes_per_iter()
     gbs = by / (ms / steps_iters) / 1e6
-    tr = ncu_traffic().get('align_stream' if eng.kernel == 'stream' else 'align_iter')
     # e2e through the public API: host dict in -> global_aligner -> compute_global_alignment -> float loss (median of 3 after
     # one warm-up call: the first call also pays pinned-allocator and lazy-initialisation costs)
     api = []
@@ -229,9 +231,6 @@ def cloud_opt_section(device, pk, steps_iters=300):
                                      '300 iters, lr 0.01 cosine, dist l1, conf log, init=None'),
                 ms_per_iter=ms / steps_iters, runs_ms=[round(r, 3) for r in runs], kernel=eng.kernel, loss_first=float(losses[0]), loss_last=float(losses[-1]),
                 roofline=dict(bound='hbm', achieved=gbs, peak=pk['hbm'], unit='GB/s', frac=gbs / pk['hbm'],
-                              # dram__bytes_read+write per align_iter launch from the committed ncu --set full record
-                              traffic=tr['bytes'] if tr else None,
-                              traffic_source=f"{tr['capture']} @ {tr['commit']}" if tr else None,
                               algorithmic_bytes_per_iter=by, peak_source=pk['source']),
                 e2e=dict(value=steps_iters / t_api, unit='iters/s', includes='H2D of 28 pairs of predictions (pinned host memory, as returned by inference()), packing, 300 iters, loss readback',
                          final_loss=loss, device_resident_inputs=e2e_dev, early_upload=e2e_early))
@@ -270,14 +269,12 @@ def cloud_opt_config5_section(device, pk, n=50, niter=300):
     ms = e0.elapsed_time(e1)
     by = eng.algorithmic_bytes_per_iter()
     gbs = by / (ms / niter) / 1e6
-    tr5 = ncu_traffic().get('align_stream_config5')
     res = dict(metric='cloud_opt iters/sec', value=niter / ms * 1e3, unit='iters/s', ms_per_iter=ms / niter, kernel=eng.kernel,
                config=dict(workload=f'{n} synthetic views -> {E} pairs (symmetrize=False) at 512x384, ModularPointCloudOptimizer, '
                                     f'{niter} iters, lr 0.01 cosine, dist l1, conf log, init=None; predictions resident in HBM'),
                aligner_build_s=round(t_build, 3), loss_first=float(losses[0]), loss_last=float(losses[-1]),
                mem_GB=round(torch.cuda.max_memory_allocated() / 1e9, 1),
                roofline=dict(bound='hbm', achieved=gbs, peak=pk['hbm'], unit='GB/s', frac=gbs / pk['hbm'],
-                             traffic=tr5['bytes'] if tr5 else None, traffic_source=f"{tr5['capture']} @ {tr5['commit']}" if tr5 else None,
                              algorithmic_bytes_per_iter=by, peak_source=pk['source']))
     del net, eng, out
     torch.cuda.empty_cache()
@@ -441,16 +438,21 @@ def run_reference_arm(args):
     print(json.dumps(line), flush=True)
 
 
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernels, as recorded from `ncu --set full`
-    captures in profiles/ncu_traffic.json (each entry names its capture file and the commit it was taken at).  The bench
-    cannot run under ncu, so these are read from the committed record rather than measured in the timed run; an entry
-    that is missing yields traffic = null."""
-    path = os.path.join(ROOT, 'profiles', 'ncu_traffic.json')
-    try:
-        return json.load(open(path))
-    except (OSError, ValueError):
-        return {}
+DUMP_SAMPLE = 1 << 20   # elements kept per output array: 4 arrays x 4 MB in float32
+
+
+def dump_outputs(out_dir, result):
+    """The forward's outputs of one step ({pts3d, conf} for both views of every pair) as DIR/<view>_<key>.npy.  Arrays
+    larger than DUMP_SAMPLE elements are sampled at fixed positions (numpy seed 0, sorted flat indices), so that the
+    dump stays far below 64 MB and two runs with the same arguments store the same positions."""
+    os.makedirs(out_dir, exist_ok=True)
+    for view, r in zip(('view1', 'view2'), result):
+        for key, t in sorted(r.items()):
+            flat = t.detach().float().reshape(-1)
+            if flat.numel() > DUMP_SAMPLE:
+                pos = np.sort(np.random.default_rng(0).choice(flat.numel(), DUMP_SAMPLE, replace=False))
+                flat = flat[torch.from_numpy(pos).to(flat.device)]
+            np.save(os.path.join(out_dir, f'{view}_{key}.npy'), flat.cpu().numpy().astype(np.float32))
 
 
 def build_roofline(prof, pk, value, world):
@@ -460,18 +462,15 @@ def build_roofline(prof, pk, value, world):
     name, dom = max(prof.items(), key=lambda kv: kv[1]['ms'])
     dom_tflops = dom['flops'] / dom['ms'] / 1e9 if dom['flops'] and dom['ms'] else 0.0
     alg_tflops = value * GFLOP_PER_PAIR / 1e3
-    traffic = ncu_traffic().get(name)
     return dict(bound='tensor', kernel=name, achieved=dom_tflops, peak=pk['tf_sustained'], unit='TFLOP/s',
-                frac=dom_tflops / pk['tf_sustained'], traffic=traffic['bytes'] if traffic else None,
-                traffic_note=(f"{traffic['shape']}; algorithmic {traffic['algorithmic_bytes'] / 1e6:.1f} MB; "
-                              f"{traffic['capture']} @ {traffic['commit']}") if traffic else None,
-                what='dominant kernel class of the step: algorithmic FLOP of its launches / their CUDA-event time, vs the measured '
-                     'cuBLAS bf16 peak sustained inside a long step (burst peak: frac_of_burst_peak)',
+                frac=dom_tflops / pk['tf_sustained'],
+                what='dominant kernel class of the step: algorithmic FLOP of its launches / their CUDA-event time, vs the bf16 peak '
+                     'of peak_source (burst peak: frac_of_burst_peak)',
                 peak_source=pk['source'], launches=dom['count'], share_of_step=dom['ms'] / tot_ms,
                 frac_of_burst_peak=dom_tflops / pk['tf_burst'],
                 whole_step=dict(achieved=alg_tflops, peak=pk['tf_sustained'] * world, unit='TFLOP/s',
                                 frac=alg_tflops / (pk['tf_sustained'] * world),
-                                what='pairs/s x 1856.8 GFLOP/pair (SURVEY §8d) vs measured cuBLAS bf16 sustained peak'))
+                                what='pairs/s x 1856.8 GFLOP/pair (SURVEY §8d) vs the bf16 peak of peak_source'))
 
 
 def main():
@@ -483,6 +482,8 @@ def main():
     ap.add_argument('--pairs', type=int, default=PAIRS_PER_GPU, help='pairs per GPU per step')
     ap.add_argument('--skip-cpu-baseline', action='store_true')
     ap.add_argument('--skip-cloud-opt', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='write the outputs of the last timed step (fixed seeded sample, float32) as DIR/<name>.npy')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 0)
     if args.impl == 'reference':
@@ -492,7 +493,7 @@ def main():
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local = int(os.environ.get('LOCAL_RANK', '0'))
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py (our arm) needs a CUDA B200; there is no CPU fallback')
+        raise SystemExit('bench.py (our arm) needs a CUDA H100; there is no CPU fallback')
     torch.cuda.set_device(local)
     device = torch.device('cuda', local)
     import torch.distributed as dist
@@ -530,6 +531,7 @@ def main():
     for _ in range(W_):
         step()
     drain()
+    last = None
     torch.cuda.synchronize()
     if world > 1:
         dist.barrier()
@@ -539,11 +541,13 @@ def main():
         torch.cuda.synchronize()
         e0.record()
         for _ in range(args.steps):
-            step()
+            last = step()
         drain()
         e1.record()
         torch.cuda.synchronize()
     launches = _lib.launch_count()
+    if args.dump_outputs and rank == 0 and last is not None:
+        dump_outputs(args.dump_outputs, last)
     ms = torch.tensor([e0.elapsed_time(e1)], device=device)
     if world > 1:
         dist.barrier()
@@ -612,7 +616,7 @@ def main():
                                      'ViTLarge_BaseDecoder_512_dpt forward only, not symmetrised (encoder sees 2 images/pair)'
                                      + (', + the single NCCL all-gather of pointmaps of inference_sharded (PairOutputGather, async, overlapped with the next step)' if world > 1 else ''),
                             weights='random init (synthetic, seed 0)', compute='bf16 operands / fp32 accumulate / fp32 residual stream',
-                            l2='activations per step (>5 GB) exceed the 126 MB L2; no explicit flush needed',
+                            l2='activations per step (>5 GB) exceed the 50 MB L2; no explicit flush needed',
                             parallelism=f'dp{world}'),
                 clocks=clocks, e2e=e2e, gpu_launches=int(launches),
                 roofline=build_roofline(prof, pk, value, world),

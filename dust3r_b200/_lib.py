@@ -1,7 +1,7 @@
 """ctypes binding of libdust3r_b200.so (the C ABI declared in include/dust3r_b200.h).
 
-There is deliberately NO fallback: if the shared library is missing or the device is not a B200
-(sm_100), every compute entry point raises.  Build with `python -m dust3r_b200.build`.
+There is deliberately NO fallback: if the shared library is missing or the device is not an H100
+(sm_90), every compute entry point raises.  Build with `python -m dust3r_b200.build`.
 """
 from __future__ import annotations
 
@@ -113,11 +113,11 @@ def check(rc: int):
 
 
 def require_cuda_device(device):
-    """The product path only exists on a B200; fail loudly anywhere else."""
+    """The product path only exists on an H100 (sm_90); fail loudly anywhere else."""
     import torch
     dev = torch.device(device)
     if dev.type != 'cuda':
-        raise D3RError(f'dust3r_b200 computes on CUDA sm_100a only (got device {dev}); there is no CPU fallback')
+        raise D3RError(f'dust3r_b200 computes on CUDA sm_90a only (got device {dev}); there is no CPU fallback')
     if not torch.cuda.is_available():
         raise D3RError('CUDA is not available: dust3r_b200 has no CPU fallback')
     with torch.cuda.device(dev):

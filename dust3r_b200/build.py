@@ -1,4 +1,4 @@
-"""Builds libdust3r_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Builds libdust3r_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
 Usage:  python -m dust3r_b200.build [--force]
 """
@@ -16,7 +16,7 @@ OUT = os.path.join(HERE, 'libdust3r_b200.so')
 OBJ_DIR = os.path.join(CSRC, 'build')
 
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-ARCH = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 CFLAGS = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr',
           '-Xptxas', '-v', '-Xcudafe', '--diag_suppress=177']
 
@@ -56,19 +56,7 @@ def _compile(src, log):
     return obj
 
 
-def generate_sources():
-    """csrc/gemm2_tcgen05.cuh (the CTA-pair GEMM kernel) is a mechanical derivation of csrc/gemm_tcgen05.cuh: it is generated
-    here (scripts/gen_gemm2.py) and not kept under version control, so an epilogue exists in exactly one source."""
-    gen = os.path.join(HERE, '..', 'scripts', 'gen_gemm2.py')
-    src, dst = os.path.join(CSRC, 'gemm_tcgen05.cuh'), os.path.join(CSRC, 'gemm2_tcgen05.cuh')
-    if not os.path.exists(dst) or os.path.getmtime(dst) < max(os.path.getmtime(src), os.path.getmtime(gen)):
-        r = subprocess.run([sys.executable, gen], capture_output=True, text=True)
-        if r.returncode != 0:
-            raise RuntimeError(f'gen_gemm2.py failed:\n{r.stdout}\n{r.stderr}')
-
-
 def build(force=False, verbose=False):
-    generate_sources()
     os.makedirs(OBJ_DIR, exist_ok=True)
     if force:
         for f in os.listdir(OBJ_DIR):

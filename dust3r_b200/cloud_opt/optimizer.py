@@ -182,7 +182,7 @@ class PointCloudOptimizer(BasePCOptimizer):
         return [row[:h * w].view(h, w) for row, (h, w) in zip(stack, self.imshapes)]
 
     def depth_to_pts3d(self):
-        """(n, max_area, 3) world-frame pointmaps.  On a B200 this is one launch of the engine's
+        """(n, max_area, 3) world-frame pointmaps.  On the GPU this is one launch of the engine's
         unprojection kernel; before `.to(cuda)` it is evaluated with torch ops (host glue, not timed)."""
         if self.device.type == 'cuda':
             eng = self._get_engine()

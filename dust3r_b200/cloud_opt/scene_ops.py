@@ -1,5 +1,5 @@
 """CUDA versions of the scene-level operators either side of the alignment loop (SURVEY §8f): thin host wrappers over
-csrc/scene_ops.cu.  Each takes CUDA fp32 tensors on a B200 and mirrors the host port it accelerates:
+csrc/scene_ops.cu.  Each takes CUDA fp32 tensors on an H100 and mirrors the host port it accelerates:
 
   clean_pointcloud      cloud_opt/pointcloud_filter.py   (dust3r/cloud_opt/base_opt.py:369-405)
   rigid_registration    cloud_opt/commons.py             (roma.rigid_points_registration as used by init_im_poses.py)

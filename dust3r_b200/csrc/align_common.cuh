@@ -66,7 +66,7 @@ __device__ __forceinline__ void fix_add(long long* dst, float x, int* overflow_f
   const long long q = __double2ll_rn(double(x) * kFixScale);
   atomicAdd(reinterpret_cast<unsigned long long*>(dst), static_cast<unsigned long long>(q));
 }
-// 2^-40 * q without FP64 (int64 -> double conversions are multi-pass on sm_100 and sit on the small step's critical path):
+// 2^-40 * q without FP64 (int64 -> double conversions are multi-pass on sm_90 and sit on the small step's critical path):
 // q = hi * 2^32 + lo; hi * 2^-8 carries the value, lo * 2^-40 < 2^-8 the fraction below.
 // `bad` collects the range check in a register: a conditional STORE per value would order the 26 accumulator loads of a thread
 // behind one another (measured: +3.6 us on the small step); the caller reports once with fix_report.

@@ -1,4 +1,4 @@
-// Fused global-alignment step for B200 (sm_100a): one launch per Adam iteration.
+// Fused global-alignment step for H100 (sm_90a): one launch per Adam iteration.
 //
 // Replaces, per iteration, the ~dozens of elementwise/bmm/gather kernels + autograd + foreach-Adam
 // of the reference loop (dust3r/cloud_opt/base_opt.py:352-366 driving optimizer.py:188-201 or

@@ -1,4 +1,4 @@
-// Streaming variant of the fused global-alignment step (sm_100a): persistent grid, every WARP is an independent
+// Streaming variant of the fused global-alignment step (sm_90a): persistent grid, every WARP is an independent
 // pipeline over its own list of work items.
 //
 // Same mathematics and the same HBM traffic as csrc/align_step.cu (32*E*P + 24*n*P bytes per iteration, SURVEY §8d;
@@ -13,8 +13,8 @@
 //        MV  the image's transform row + log-depth, exp_avg, exp_avg_sq slices for the in-place Adam update;
 //     no warp ever waits for another warp: the ring is refilled by the warp that drained it, across item boundaries;
 //   * observations are stored slot-interleaved as pixel PAIRS, [32 x (xA,xB,yA,yB)] [32 x (zA,zB,wA,wB)] per slot, so
-//     two LDS.128 hand the thread two pixels as packed f32x2 operands and the whole residual / gradient algebra runs
-//     on FFMA2 / FADD2 / FMUL2 (half the issue slots; the scalar transform coefficients ride as broadcast operands);
+//     two LDS.128 hand the thread two pixels as packed pairs and the whole residual / gradient algebra runs on
+//     pixel pairs (two independent dependency chains per thread);
 //   * the 13 per-entry sums are reduced across the warp through a transpose in the just-drained stage buffer
 //     (13 STS + 4 LDS.128 + 16 FADD instead of a 16-shuffle butterfly), accumulated per warp in shared memory over
 //     all of the warp's items of an image, and leave the SM once per (warp, image) as 2^44 fixed-point integer
@@ -36,12 +36,26 @@ constexpr int kScrStride = 36;      // floats per row of the transpose scratch (
 static_assert(sizeof(d3r_align_item) == 64, "d3r_align_item must be 64 bytes");
 
 typedef unsigned long long f2;      // two packed fp32 (lo = pixel A, hi = pixel B)
-__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) { f2 d; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c)); return d; }
-__device__ __forceinline__ f2 add2(f2 a, f2 b) { f2 d; asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
-__device__ __forceinline__ f2 mul2(f2 a, f2 b) { f2 d; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b)); return d; }
 __device__ __forceinline__ f2 pack2(float lo, float hi) { f2 d; asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(lo), "f"(hi)); return d; }
-__device__ __forceinline__ f2 bc2(float x) { return pack2(x, x); }   // ptxas folds this into a scalar (.F32) FFMA2 operand
+__device__ __forceinline__ f2 bc2(float x) { return pack2(x, x); }
 __device__ __forceinline__ void unpack2(f2 v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
+// Hopper has no packed fp32 arithmetic: each pair operation is two scalar round-to-nearest operations, which gives
+// the same bits per lane as a packed one
+__device__ __forceinline__ f2 fma2(f2 a, f2 b, f2 c) {
+  float a0, a1, b0, b1, c0, c1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1); unpack2(c, c0, c1);
+  return pack2(__fmaf_rn(a0, b0, c0), __fmaf_rn(a1, b1, c1));
+}
+__device__ __forceinline__ f2 add2(f2 a, f2 b) {
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(__fadd_rn(a0, b0), __fadd_rn(a1, b1));
+}
+__device__ __forceinline__ f2 mul2(f2 a, f2 b) {
+  float a0, a1, b0, b1;
+  unpack2(a, a0, a1); unpack2(b, b0, b1);
+  return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
+}
 __device__ __forceinline__ float rsqrt_approx(float x) { float y; asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float sqrt_approx(float x) { float y; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }

@@ -1,4 +1,4 @@
-// Attention entry points: kernel selection and the C ABI (the kernels live in attention_tc3.cu / attention_tc2.cu).
+// Attention entry points: kernel selection and the C ABI (the kernel lives in attention_wgmma.cu).
 //   O[b, i, h*64 + d] = softmax_j(scale * q[b,i,h,:] . k[b,j,h,:]) v[b,j,h,d]      head dim 64 (all DUSt3R heads), bf16 in/out
 // replaces the materialised (B,H,N,N) fp32 attention matrix of croco/models/blocks.py:105-109 / :161-165.
 #include "d3r_common.cuh"
@@ -7,36 +7,19 @@
 namespace d3r {
 namespace attn {
 
-// 3 (default): tcgen05 split-row kernel with P in tensor memory (attention_tc3.cu); 2: the same dataflow with P through shared
-// memory (attention_tc2.cu), kept as the A/B reference -- both produce the same bits on aligned shapes.
+// 3 (default): P V with P in registers; 2: the same dataflow with P through shared memory, kept as the A/B reference --
+// both produce the same bits.
 static int g_impl = 3;
-void set_tc2_ablation(int a);
-void set_tc3_ablation(int a);
-int attention_tc2_set_debug(void* dev_buf);
-int attention_tc3_set_debug(void* dev_buf);
 
-// impl 3 / 2, + 10 k: timing ablations of that kernel (debug; results are wrong)
-void set_impl(int impl) {
-  g_impl = (impl % 10 == 2) ? 2 : 3;
-  set_tc2_ablation(g_impl == 2 ? impl / 10 : 0);
-  set_tc3_ablation(g_impl == 3 ? impl / 10 : 0);
-}
+void set_impl(int impl) { g_impl = (impl == 2) ? 2 : 3; }
 
 int attention_hd64(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* out,
                    long long ldo, int B, int heads, int Nq, int Nk, float scale, cudaStream_t st) {
-  if (g_impl == 2) return attention_hd64_tc2(q, ldq, k, ldk, v, ldv, out, ldo, B, heads, Nq, Nk, scale, st);
-  return attention_hd64_tc3(q, ldq, k, ldk, v, ldv, out, ldo, B, heads, Nq, Nk, scale, st);
-}
-
-int attention_set_debug(void* dev_buf) {
-  if (int rc = attention_tc2_set_debug(dev_buf)) return rc;
-  return attention_tc3_set_debug(dev_buf);
+  return attention_hd64_wgmma(q, ldq, k, ldk, v, ldv, out, ldo, B, heads, Nq, Nk, scale, g_impl == 2, st);
 }
 
 }  // namespace attn
 }  // namespace d3r
-
-extern "C" int d3r_attention_set_debug(void* dev_buf) { return d3r::attn::attention_set_debug(dev_buf); }
 
 extern "C" void d3r_set_attention_impl(int32_t impl) { d3r::attn::set_impl(impl); }
 

@@ -19,7 +19,7 @@ int num_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    if (sms <= 0) sms = 148;
+    if (sms <= 0) sms = 132;
   }
   return sms;
 }
@@ -36,8 +36,8 @@ extern "C" int d3r_check_device(void) {
   int major = 0, minor = 0;
   D3R_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
   D3R_CUDA(cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev));
-  if (major != 10) {
-    d3r::set_error("dust3r_b200 is built for sm_100a only; device %d is sm_%d%d", dev, major, minor);
+  if (major != 9 || minor != 0) {
+    d3r::set_error("dust3r_b200 is built for sm_90a only; device %d is sm_%d%d", dev, major, minor);
     return D3R_ERR_UNSUPPORTED_DEVICE;
   }
   return D3R_OK;

@@ -1,4 +1,4 @@
-// Shared helpers of the dust3r_b200 CUDA library (sm_100a only).
+// Shared helpers of the dust3r_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>

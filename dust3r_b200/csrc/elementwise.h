@@ -19,10 +19,9 @@ namespace attn {
 // q rows: (b*Nq + i)*ldq + h*64 ; k/v rows: (b*Nk + j)*ldk(v) + h*64.
 int attention_hd64(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* out,
                    long long ldo, int B, int heads, int Nq, int Nk, float scale, cudaStream_t st);
-int attention_hd64_tc3(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* out,
-                      long long ldo, int B, int heads, int Nq, int Nk, float scale, cudaStream_t st);
-int attention_hd64_tc2(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* out,
-                      long long ldo, int B, int heads, int Nq, int Nk, float scale, cudaStream_t st);
+// p_smem: P V with P through shared memory instead of registers (same bits; the A/B reference of the register path)
+int attention_hd64_wgmma(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* out,
+                         long long ldo, int B, int heads, int Nq, int Nk, float scale, bool p_smem, cudaStream_t st);
 void set_impl(int impl);
 }  // namespace attn
 }  // namespace d3r

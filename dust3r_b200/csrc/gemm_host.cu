@@ -1,6 +1,5 @@
-// Host side of the tcgen05 GEMM / conv kernels: tensor-map construction, tile-shape selection, launch.
-#include "gemm_tcgen05.cuh"
-#include "gemm2_tcgen05.cuh"
+// Host side of the wgmma GEMM / conv kernels: tensor-map construction, tile-shape selection, launch.
+#include "gemm_wgmma.cuh"
 #include "gemm_host.h"
 #include "prof.h"
 #include <mutex>
@@ -47,98 +46,65 @@ static int encode(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* d
 bool use_pair(int bn, int num_kb);
 
 int pick_block_n(int N, uint32_t flags) {
-  if (flags & F_HEAD_FINAL) return 128;
-  if (N % 256 == 0) return 256;
+  if (flags & F_HEAD_FINAL) return 128;   // the head tail needs a whole 128-channel row in one tile
   if (N % 128 == 0) return 128;
-  if (N % 64 == 0) return (N >= 512) ? 256 : 64;
-  return (N > 128) ? 256 : 128;
+  if (N % 64 == 0) return 64;
+  return (N > 128) ? 128 : 64;            // N % 32 == 0: the last tile is partly empty
 }
 
-template <int BN, int EPI>
-static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const Params& p, int total_tiles, cudaStream_t st) {
-  static unsigned long long attr_devices = 0;
-  if (first_launch_on_this_device(attr_devices))
-    D3R_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN, EPI>::kSmemBytes));
-  int grid = total_tiles < num_sms() ? total_tiles : num_sms();
-  const char* tag = (p.mode == 1) ? ((p.flags & F_HEAD_FINAL) ? "conv3x3_head_tail" : "conv3x3_tcgen05")
-                                  : (BN == 256 ? "gemm_tcgen05_bn256" : (BN == 128 ? "gemm_tcgen05_bn128" : "gemm_tcgen05_bn64"));
-  char detail[96];
-  snprintf(detail, sizeof(detail), "M=%d N=%d K=%d flags=0x%x mode=%d epi=%d", p.M, p.N, p.K, (unsigned)p.flags, p.mode, EPI);
-  prof::Scope scope(tag, st, 2.0 * double(p.M) * double(p.N) * double(p.K), 0.0, 1, detail);
-  D3R_CUDA(pdl::launch(gemm_kernel<BN, EPI>, dim3(grid), dim3(kNumThreads), size_t(Cfg<BN, EPI>::kSmemBytes), st, ta, tb, to, p));
-  D3R_LAUNCH_CHECK();
-  return D3R_OK;
-}
-
-// 0: 1-CTA kernels, 1: CTA-pair (cta_group::2) kernels whenever BLOCK_N >= 128, 2 (default): pair kernels from
-// g_pair_min_kb k-blocks of 64 on, 1-CTA kernels for the shortest reductions (K = 96 / 192 of the DPT re-assembly).
-// Round 1 drew the line at 16 k-blocks from isolated-GEMM timings; interleaved A/B runs of the WHOLE forward step
-// (scripts/gemm_policy_ab.py, round 2) put >= 4 ahead by 1 %: 67.5-67.7 ms against 68.3 ms at >= 16.
+// 0: 1-CTA kernels, 1: CTA-pair kernels (cluster of two, B tile multicast) whenever BLOCK_N == 128, 2 (default): pair
+// kernels from g_pair_min_kb k-blocks of 64 on, 1-CTA kernels for the shortest reductions (K = 96 / 192 of the DPT
+// re-assembly), whose time goes to the epilogue rather than to operand traffic.
 static int g_impl = 2;
 static int g_pair_min_kb = 4;
 void set_impl(int impl) { g_impl = impl; }
 void set_pair_min_kb(int kb) { g_pair_min_kb = kb; }
 bool use_pair(int bn, int num_kb) { return bn >= 128 && (g_impl == 1 || (g_impl == 2 && num_kb >= g_pair_min_kb)); }
 
-template <int BN, int EPI>
-static int launch2(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const Params& p, int m_tiles, int n_tiles,
-                   cudaStream_t st) {
+template <int BN, int EPI, bool PAIR>
+static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int m_tiles, int n_tiles, cudaStream_t st) {
   static unsigned long long attr_devices = 0;
   if (first_launch_on_this_device(attr_devices))
-    D3R_CUDA(cudaFuncSetAttribute(gemm2_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg2<BN, EPI>::kSmemBytes));
-  const int cluster_tiles = ((m_tiles + 1) / 2) * n_tiles;
-  const int max_clusters = num_sms() / 2;
-  const int clusters = cluster_tiles < max_clusters ? cluster_tiles : max_clusters;
-  const char* tag = (p.mode == 1) ? ((p.flags & F_HEAD_FINAL) ? "conv3x3_head_tail_2cta" : "conv3x3_tcgen05_2cta")
-                                  : (BN == 256 ? (p.K >= 1024 ? "gemm_tcgen05_2cta_bn256" : "gemm_tcgen05_2cta_bn256_shortk")
-                                               : "gemm_tcgen05_2cta_bn128");   // short-K projections (decoder K = 768, DPT K = 256)
-                                                                               // are epilogue-bound: a class of their own in the breakdown
+    D3R_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, EPI, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::kSmemBytes));
+  int grid;
+  if (PAIR) {
+    const int items = ((m_tiles + 1) / 2) * n_tiles;
+    const int max_clusters = num_sms() / 2;
+    grid = 2 * (items < max_clusters ? items : max_clusters);
+  } else {
+    const int items = m_tiles * n_tiles;
+    grid = items < num_sms() ? items : num_sms();
+  }
+  const char* tag = (p.mode == 1) ? ((p.flags & F_HEAD_FINAL) ? (PAIR ? "conv3x3_head_tail_2cta" : "conv3x3_head_tail")
+                                                              : (PAIR ? "conv3x3_wgmma_2cta" : "conv3x3_wgmma"))
+                                  : (PAIR ? "gemm_wgmma_2cta_bn128" : (BN == 128 ? "gemm_wgmma_bn128" : "gemm_wgmma_bn64"));
   char detail[96];
   snprintf(detail, sizeof(detail), "M=%d N=%d K=%d flags=0x%x mode=%d epi=%d", p.M, p.N, p.K, (unsigned)p.flags, p.mode, EPI);
   prof::Scope scope(tag, st, 2.0 * double(p.M) * double(p.N) * double(p.K), 0.0, 1, detail);
-  D3R_CUDA(pdl::launch(gemm2_kernel<BN, EPI>, dim3(2 * clusters), dim3(kNumThreads), size_t(Cfg2<BN, EPI>::kSmemBytes), st, ta, tb, to, p));
+  D3R_CUDA(pdl::launch_clustered(gemm_kernel<BN, EPI, PAIR>, dim3(grid), dim3(kNumThreads), size_t(Cfg<BN>::kSmemBytes), st, PAIR ? 2 : 1, ta, tb, p));
   D3R_LAUNCH_CHECK();
   return D3R_OK;
 }
 
-static int dispatch(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int total_tiles, cudaStream_t st) {
-  // epilogue specialisation (BLOCK_N = 256 only: every hot projection of the two ViTs has N % 256 == 0)
-  int epi = (bn == 256) ? pick_epi(p.mode, p.flags) : EPI_GENERIC;
-  CUtensorMap to = ta;   // placeholder unless the epilogue stores through TMA
-  if (epi == EPI_RESID) {
-    if ((reinterpret_cast<uintptr_t>(p.out) & 15) != 0 || p.ldo % 4 != 0) {
-      epi = EPI_GENERIC;   // TMA needs 16-byte aligned rows; the register epilogue has no such requirement
-    } else {
-      cuuint64_t dims[2] = {(cuuint64_t)p.N, (cuuint64_t)p.M};
-      cuuint64_t str[1] = {(cuuint64_t)p.ldo * 4};
-      cuuint32_t box[2] = {32, 32};
-      int rc = encode(&to, p.out, 2, dims, str, box, CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
-      if (rc) return rc;
-    }
+template <bool PAIR>
+static int dispatch_bn128(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int m_tiles, int n_tiles, cudaStream_t st) {
+  switch (epi) {
+    case EPI_RESID: return launch<128, EPI_RESID, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
+    case EPI_ACT: return launch<128, EPI_ACT, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
+    case EPI_ROPE: return launch<128, EPI_ROPE, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
+    default: return launch<128, EPI_GENERIC, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
   }
-  if (use_pair(bn, p.num_kb)) {
-    const int n_tiles = (p.N + bn - 1) / bn;
-    const int m_tiles = total_tiles / n_tiles;
-    if (bn == 256) {
-      switch (epi) {
-        case EPI_RESID: return launch2<256, EPI_RESID>(ta, tb, to, p, m_tiles, n_tiles, st);
-        case EPI_ACT: return launch2<256, EPI_ACT>(ta, tb, to, p, m_tiles, n_tiles, st);
-        case EPI_ROPE: return launch2<256, EPI_ROPE>(ta, tb, to, p, m_tiles, n_tiles, st);
-        default: return launch2<256, EPI_GENERIC>(ta, tb, to, p, m_tiles, n_tiles, st);
-      }
-    }
-    return launch2<128, EPI_GENERIC>(ta, tb, to, p, m_tiles, n_tiles, st);
-  }
+}
+
+static int dispatch(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int m_tiles, cudaStream_t st) {
+  const int n_tiles = (p.N + bn - 1) / bn;
+  // epilogue specialisation (BLOCK_N = 128 only: every hot projection of the two ViTs has N % 128 == 0)
+  const int epi = (bn == 128) ? pick_epi(p.mode, p.flags) : EPI_GENERIC;
   switch (bn) {
-    case 256:
-      switch (epi) {
-        case EPI_RESID: return launch<256, EPI_RESID>(ta, tb, to, p, total_tiles, st);
-        case EPI_ACT: return launch<256, EPI_ACT>(ta, tb, to, p, total_tiles, st);
-        case EPI_ROPE: return launch<256, EPI_ROPE>(ta, tb, to, p, total_tiles, st);
-        default: return launch<256, EPI_GENERIC>(ta, tb, to, p, total_tiles, st);
-      }
-    case 128: return launch<128, EPI_GENERIC>(ta, tb, to, p, total_tiles, st);
-    case 64: return launch<64, EPI_GENERIC>(ta, tb, to, p, total_tiles, st);
+    case 128:
+      if (use_pair(bn, p.num_kb)) return dispatch_bn128<true>(epi, ta, tb, p, m_tiles, n_tiles, st);
+      return dispatch_bn128<false>(epi, ta, tb, p, m_tiles, n_tiles, st);
+    case 64: return launch<64, EPI_GENERIC, false>(ta, tb, p, m_tiles, n_tiles, st);
   }
   set_error("unsupported BLOCK_N %d", bn);
   return D3R_ERR_INVALID;
@@ -171,8 +137,7 @@ int gemm_bf16(const void* A, long long lda, const void* B, Params p, cudaStream_
   }
   int rc = make_tmap_b(&tb, B, p.N, 1, p.K, bn, p.num_kb);
   if (rc) return rc;
-  const int total = ((p.M + BLOCK_M - 1) / BLOCK_M) * ((p.N + bn - 1) / bn);
-  return dispatch(bn, ta, tb, p, total, st);
+  return dispatch(bn, ta, tb, p, (p.M + BLOCK_M - 1) / BLOCK_M, st);
 }
 
 int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, int Cin, int Cout, Params p, cudaStream_t st) {
@@ -203,8 +168,7 @@ int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, 
   }
   int rc = make_tmap_b(&tb, w_packed, Cout, 9, Cin, bn, p.num_kb);
   if (rc) return rc;
-  const int total = B * p.tiles_x * p.tiles_y * ((p.N + bn - 1) / bn);
-  return dispatch(bn, ta, tb, p, total, st);
+  return dispatch(bn, ta, tb, p, B * p.tiles_x * p.tiles_y, st);
 }
 
 }  // namespace gemm

@@ -1,6 +1,6 @@
-// Internal host API of the tcgen05 GEMM (C++ side; the C ABI wrappers live in gemm_host.cu).
+// Internal host API of the wgmma GEMM (C++ side; the C ABI wrappers live in gemm_host.cu).
 #pragma once
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 
 namespace d3r {
 namespace gemm {

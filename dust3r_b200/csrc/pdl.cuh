@@ -1,6 +1,6 @@
 // Programmatic dependent launch (PDL) for the forward's kernel chain: every launch carries
 // cudaLaunchAttributeProgrammaticStreamSerialization, every kernel does its launch-independent set-up (barrier
-// init, TMEM allocation, tensor-map prefetch) first and then calls pdl::sync_with_predecessor() BEFORE it touches
+// init, tensor-map prefetch) first and then calls pdl::sync_with_predecessor() BEFORE it touches
 // any global memory another kernel may have produced or may still be reading.  The next kernel's CTAs are therefore
 // scheduled onto SMs as soon as the current kernel's CTAs retire from them, with their prologue already done when the
 // predecessor finishes.  A kernel launched without the attribute sees both instructions as no-ops.
@@ -30,19 +30,37 @@ __device__ __forceinline__ void sync_with_predecessor() {
   asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
 }
 
+// cluster_x > 1: the grid is launched as clusters of cluster_x consecutive CTAs
 template <class... KArgs, class... Args>
-inline cudaError_t launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+inline cudaError_t launch_clustered(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, int cluster_x,
+                                    Args&&... args) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute at[2];
+  int n = 0;
+  if (enabled()) {
+    at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    at[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
+  if (cluster_x > 1) {
+    at[n].id = cudaLaunchAttributeClusterDimension;
+    at[n].val.clusterDim.x = cluster_x;
+    at[n].val.clusterDim.y = 1;
+    at[n].val.clusterDim.z = 1;
+    ++n;
+  }
   cfg.attrs = at;
-  cfg.numAttrs = enabled() ? 1 : 0;
+  cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kernel, std::forward<Args>(args)...);
+}
+
+template <class... KArgs, class... Args>
+inline cudaError_t launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  return launch_clustered(kernel, grid, block, smem, st, 1, std::forward<Args>(args)...);
 }
 
 }  // namespace pdl

@@ -1,4 +1,4 @@
-// Scene-level kernels either side of the alignment loop (SURVEY §8f "next" rows), sm_100a:
+// Scene-level kernels either side of the alignment loop (SURVEY §8f "next" rows), sm_90a:
 //   * clean_pointcloud          cross-view consistency filter                 dust3r/cloud_opt/base_opt.py:369-405
 //   * weighted Procrustes sums  moments of weighted Umeyama / Kabsch          roma.rigid_points_registration as called by
 //                                                                             dust3r/cloud_opt/init_im_poses.py:66-110, 253-262

@@ -1,11 +1,11 @@
-"""AsymmetricCroCo3DStereo — drop-in for dust3r/model.py:46-211 whose forward runs on the B200-native CUDA
+"""AsymmetricCroCo3DStereo — drop-in for dust3r/model.py:46-211 whose forward runs on the H100-native CUDA
 path (csrc/forward.cu) through the C ABI.
 
 The module owns fp32 `nn.Parameter`s under the reference's state-dict names (config.state_dict_spec), so
 `load_state_dict` / `from_pretrained` accept real DUSt3R checkpoints.  Before the first forward (and after
 any weight change) the parameters are repacked once into the kernels' operand layout (bf16 K-major GEMM
 weights, tap-major 3x3 filters, fused k|v projection, fp32 biases / LayerNorm parameters, RoPE tables).
-There is no torch / CPU fallback: forward() requires a CUDA sm_100 device and the built extension.
+There is no torch / CPU fallback: forward() requires a CUDA sm_90 device and the built extension.
 """
 from __future__ import annotations
 

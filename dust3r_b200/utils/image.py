@@ -6,7 +6,7 @@ are those of dust3r/utils/image.py:74-128.
 `load_images(..., device=None)` is the reference's host path (PIL resize + crop on a CPU core, float image to be uploaded by
 inference()).  `load_images(..., device='cuda')` (SURVEY §8f rank 4) only DECODES on the host: the 8-bit RGB pixels go up once
 and the resize (Pillow's two-pass fixed-point resampling, restated as two integer kernels), the crop and ImgNorm run on the
-B200 (`d3r_image_resize_crop_normalize`, csrc/image_ops.cu) -- bit-identical to the host path, the normalised image is born
+H100 (`d3r_image_resize_crop_normalize`, csrc/image_ops.cu) -- bit-identical to the host path, the normalised image is born
 in HBM and inference() uses it in place."""
 from __future__ import annotations
 
@@ -92,7 +92,7 @@ def _host_view(pil, size, square_ok, patch_size):
 def load_images(folder_or_list, size, square_ok=False, verbose=True, patch_size=16, device=None, workers=None):
     """Folder name or list of file names -> list of dict(img (1,3,H,W) in [-1,1], true_shape int32 [[H,W]], idx,
     instance) ready for make_pairs / inference.  Files that are not .jpg/.jpeg/.png are skipped.
-    device=None: the reference's host pipeline, `img` is a CPU tensor.  device=<a B200>: decode on the host, resize / crop /
+    device=None: the reference's host pipeline, `img` is a CPU tensor.  device=<an H100>: decode on the host, resize / crop /
     normalise on that GPU (same bits), `img` is resident there.
     Files are decoded (device=None: decoded, resized and normalised) by `workers` threads -- PIL releases the GIL in its codecs
     and resampling loops -- while the results are consumed in file order, so idx / instance / verbose output are those of the

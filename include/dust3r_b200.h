@@ -1,5 +1,5 @@
 /*
- * dust3r_b200 — C ABI of the B200-native DUSt3R hot paths (sm_100a).
+ * dust3r_b200 — C ABI of the H100-native DUSt3R hot paths (sm_90a).
  *
  * The reference (naver/dust3r) has no FFI/plugin registry; its only native entry point is the
  * pybind function `curope.rope_2d` (croco/models/curope/curope.cpp:49-69).  Everything else on
@@ -33,7 +33,7 @@ extern "C" {
 const char* d3r_last_error(void);
 /* ABI version of this header; bumped on any signature change. */
 int d3r_abi_version(void);
-/* 0 when the current device is sm_100 (B200); D3R_ERR_UNSUPPORTED_DEVICE otherwise. */
+/* 0 when the current device is sm_90 (H100); D3R_ERR_UNSUPPORTED_DEVICE otherwise. */
 int d3r_check_device(void);
 
 /* Launch accounting / profiling aid: number of kernels this library launched since the last reset;
@@ -222,7 +222,7 @@ int d3r_align_pack_entries(const d3r_pack_entry* table_dev, int32_t n_entries, i
 #define D3R_F_ROPE          (1u << 8)   /* 2D RoPE on columns < rope_cols; replaces curope.rope_2d        */
 #define D3R_F_OUT2_BF16     (1u << 11)
 
-/* out[M,N] = epilogue(A[M,K] * B[N,K]^T); A, B bf16 row-major (nn.Linear weight layout), tcgen05.
+/* out[M,N] = epilogue(A[M,K] * B[N,K]^T); A, B bf16 row-major (nn.Linear weight layout), wgmma.
  * N % 32 == 0, K % 8 == 0.  With D3R_F_ROPE: rope_cos/sin are [max_pos][16] fp32 tables
  * (angle = pos * base^(-k/16), croco/models/curope/kernels.cu:41-52), rows are tokens of images of
  * `tokens_per_img` tokens laid out row-major on a grid `grid_w` wide. */
@@ -231,7 +231,7 @@ int d3r_gemm_bf16(const void* A_dev, const void* B_dev, void* out_dev, const flo
                   const float* rope_cos_dev, const float* rope_sin_dev, int32_t rope_cols, int32_t tokens_per_img,
                   int32_t grid_w, void* stream);
 
-/* 3x3 stride-1 pad-1 convolution as implicit GEMM on tcgen05.  x: (B,H,W,Cin) bf16 NHWC;
+/* 3x3 stride-1 pad-1 convolution as implicit GEMM on wgmma.  x: (B,H,W,Cin) bf16 NHWC;
  * w_packed: [Cout][ky*3+kx][Cin] bf16; out/add0/add1/out2: (B,H,W,Cout) bf16 NHWC.
  * (croco/models/dpt_block.py ResidualConvUnit_custom / layer_rn / head convs) */
 int d3r_conv3x3_bf16(const void* x_nhwc_dev, const void* w_packed_dev, void* out_dev, const float* bias_dev,
@@ -244,17 +244,15 @@ int d3r_attention_hd64(const void* q_dev, int64_t ldq, const void* k_dev, int64_
                        void* out_dev, int64_t ldo, int32_t B, int32_t heads, int32_t Nq, int32_t Nk, float scale,
                        void* stream);
 
-/* Selects the GEMM / conv kernel family: 0 = 1-CTA tcgen05 kernels, 1 = CTA-pair (cta_group::2) kernels,
- * 2 (default) = CTA-pair kernels from 4 k-blocks of 64 on (K >= 256), 1-CTA for shorter reductions. */
+/* Selects the GEMM / conv kernel family: 0 = 1-CTA kernels, 1 = CTA-pair kernels (a cluster of two CTAs on two
+ * M tiles sharing one multicast B tile), 2 (default) = CTA-pair kernels from 4 k-blocks of 64 on (K >= 256), 1-CTA
+ * for shorter reductions. */
 void d3r_set_gemm_impl(int32_t impl);
 /* Tuning aid for impl 2: minimum number of 64-wide k-blocks for which the CTA-pair kernel is used (default 4). */
 void d3r_set_gemm_pair_min_kblocks(int32_t kblocks);
 
-/* Debug aid: per-image timeline stamps (64 x uint64 %globaltimer per traced CTA) of the tcgen05 attention. */
-int d3r_attention_set_debug(void* dev_buf);
-
-/* Selects the attention kernel: 3 (default) = tcgen05/TMEM split-row kernel (two warps per 32 query rows, 128-key blocks) with P
- * kept in tensor memory (A-from-TMEM tcgen05.mma); 2 = the same dataflow with P through shared memory (A/B reference). */
+/* Selects the attention kernel: 3 (default) = wgmma kernel (64 query rows per warpgroup, 128-key blocks) with P kept in
+ * registers (A-from-registers wgmma); 2 = the same dataflow with P through shared memory (A/B reference). */
 void d3r_set_attention_impl(int32_t impl);
 
 /* ------------------------------------------------------------------------------------------

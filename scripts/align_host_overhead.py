@@ -1,6 +1,6 @@
 """Host-side overhead of the alignment e2e call (global_aligner + compute_global_alignment, BASELINE configs[2]) measured
 WITHOUT a GPU: the C library and the torch.cuda entry points the engine uses are replaced by no-ops and everything runs on CPU
-tensors, so what is timed is exactly the Python / numpy / torch-CPU work that surrounds the kernel launches on a B200.
+tensors, so what is timed is exactly the Python / numpy / torch-CPU work that surrounds the kernel launches on an H100.
 
     python -O scripts/align_host_overhead.py        # -O: the engine asserts that its buffers are CUDA tensors
 
@@ -32,7 +32,7 @@ class FakeStream:
     cuda_stream = 0
     def synchronize(self): pass
 torch.cuda.current_stream = lambda d=None: FakeStream()
-torch.cuda.get_device_properties = lambda d: types.SimpleNamespace(multi_processor_count=148)
+torch.cuda.get_device_properties = lambda d: types.SimpleNamespace(multi_processor_count=132)
 torch.cuda.synchronize = lambda *a: None
 
 from dust3r_b200.utils.synth import synth_pair_predictions

@@ -1,4 +1,4 @@
-"""Epilogue-cost sweep of the tcgen05 GEMM: same shape, different fused epilogues (iteration aid)."""
+"""Epilogue-cost sweep of the wgmma GEMM: same shape, different fused epilogues (iteration aid)."""
 import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

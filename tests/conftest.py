@@ -8,15 +8,17 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 GOLDEN = os.path.join(ROOT, 'tests', 'golden')
-REFERENCE = '/root/reference'
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA B200 device (run on the GPU box with -m gpu)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA H100 device (select with -m gpu)')
 
 
-def has_reference():
-    return os.path.isdir(os.path.join(REFERENCE, 'dust3r'))
+def reference_golden():
+    """Outputs of the unmodified reference (naver/dust3r) for the tests that compare with it, stored by
+    tests/golden/make_reference_golden.py."""
+    import numpy as np
+    return np.load(os.path.join(GOLDEN, 'reference_live.npz'))
 
 
 @pytest.fixture(scope='session')

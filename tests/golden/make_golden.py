@@ -1,6 +1,6 @@
-"""Generates tests/golden/*.npz by running the UNMODIFIED reference (/root/reference) on CPU fp32.
+"""Generates tests/golden/*.npz by running the UNMODIFIED reference (naver/dust3r) on CPU fp32.
 
-    python tests/golden/make_golden.py            # in the build container (reference mounted)
+    DUST3R_REFERENCE=<path to a naver/dust3r checkout> python tests/golden/make_golden.py
 
 Forward goldens come from the pure reference.  Alignment goldens are "reference cloud_opt + local roma
 restatement" (oracle/roma_stub) because `roma` is not installable offline (SURVEY §8c).
@@ -17,7 +17,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, os.path.join(ROOT, 'oracle', 'roma_stub'))
-sys.path.insert(0, '/root/reference')
+sys.path.insert(0, os.environ['DUST3R_REFERENCE'])
 sys.path.insert(0, ROOT)
 
 from dust3r_b200.config import ModelConfig, vitl_512_dpt, vitl_224_linear  # noqa: E402

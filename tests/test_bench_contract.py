@@ -43,23 +43,26 @@ def test_reference_arm_other_ranks_exit_quietly():
 
 
 def test_build_roofline_on_a_recorded_breakdown():
-    """The `roofline` object is assembled by a pure function: feed it the per-kernel breakdown of a recorded run."""
+    """The `roofline` object is assembled by a pure function: feed it a per-kernel breakdown in the format of the bench's
+    `kernels` record (a fixed, made-up one: the function is checked, not a GPU)."""
     sys.path.insert(0, ROOT)
     import bench
-    rec = json.loads(open(os.path.join(ROOT, 'profiles', 'r01_bench_v13.json')).read().strip().splitlines()[-1])
+    rec = dict(value=300.0, kernels={
+        'gemm_wgmma_2cta_bn128': dict(launches=600, ms=60.0, tflops=700.0, gbs=None),
+        'attention_wgmma': dict(launches=120, ms=20.0, tflops=400.0, gbs=None),
+        'layernorm': dict(launches=200, ms=5.0, tflops=None, gbs=2500.0)})
     prof = {k: dict(count=v['launches'], ms=v['ms'], flops=(v['tflops'] or 0.0) * v['ms'] * 1e9, bytes=(v['gbs'] or 0.0) * v['ms'] * 1e6)
             for k, v in rec['kernels'].items()}
-    pk = dict(hbm=6556.2, tf_burst=1683.2, tf_sustained=1439.4, source='test')
+    pk = dict(hbm=3350.0, tf_burst=989.0, tf_sustained=900.0, source='test')
     for world in (1, 8):
         r = bench.build_roofline(prof, pk, rec['value'] * world, world)
         json.dumps(r)                                     # serialisable
-        assert r['bound'] == 'tensor' and r['unit'] == 'TFLOP/s' and r['kernel'] == 'gemm_tcgen05_2cta_bn256'
+        assert r['bound'] == 'tensor' and r['unit'] == 'TFLOP/s' and r['kernel'] == 'gemm_wgmma_2cta_bn128'
         assert abs(r['frac'] - r['achieved'] / r['peak']) < 1e-12 and 0.5 < r['frac'] < 1.0
         assert r['peak'] == pk['tf_sustained'] and 0 < r['frac_of_burst_peak'] < r['frac']
-        assert r['traffic'] and r['traffic'] < 1.2 * bench.ncu_traffic()[r['kernel']]['algorithmic_bytes']
+        assert r['launches'] == 600 and abs(r['share_of_step'] - 60.0 / 85.0) < 1e-12
         ws = r['whole_step']
         assert abs(ws['achieved'] - rec['value'] * world * bench.GFLOP_PER_PAIR / 1e3) < 1e-6
         assert abs(ws['frac'] - ws['achieved'] / (pk['tf_sustained'] * world)) < 1e-12
-    # a class the table has no capture for: traffic stays null
     odd = bench.build_roofline({'some_kernel': dict(count=1, ms=1.0, flops=1e12, bytes=0.0)}, pk, 1.0, 1)
-    assert odd['traffic'] is None and odd['traffic_note'] is None and odd['achieved'] == 1000.0
+    assert odd['achieved'] == 1000.0

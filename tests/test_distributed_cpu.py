@@ -1,4 +1,4 @@
-"""world_size-2 gloo test of the pair sharding + all-gather plumbing (the forward itself needs a B200, so a
+"""world_size-2 gloo test of the pair sharding + all-gather plumbing (the forward itself needs an H100, so a
 deterministic stand-in model produces the per-pair outputs)."""
 import os
 import sys

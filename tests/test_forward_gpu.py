@@ -1,4 +1,4 @@
-"""Pairwise forward on the B200 path vs the CPU fp32 oracle / the reference's golden outputs.
+"""Pairwise forward on the H100 path vs the CPU fp32 oracle / the reference's golden outputs.
 
 Numerics: GEMM operands are bf16 (8-bit mantissa), accumulation and the residual stream are fp32; the
 reference computes in fp32 (TF32 on GPU).  Stated tolerances (calibrated on the synthetic-weight models):

@@ -1,5 +1,5 @@
-"""tcgen05 GEMM / implicit-GEMM conv kernels through the C ABI vs plain torch fp32 on the same
-bf16-rounded operands.  Tolerance: the kernel accumulates in fp32 (TMEM) exactly like the torch
+"""wgmma GEMM / implicit-GEMM conv kernels through the C ABI vs plain torch fp32 on the same
+bf16-rounded operands.  Tolerance: the kernel accumulates in fp32 (registers) exactly like the torch
 reference up to summation order; outputs stored as bf16 carry one rounding (rel 2^-8)."""
 import ctypes as C
 import math
@@ -16,7 +16,7 @@ from dust3r_b200._lib_fwd import (F_BIAS, F_GELU, F_RELU, F_OUT_F32, F_RESID_INP
 
 @pytest.fixture(params=[0, 1], ids=['cta1', 'cta_pair'], autouse=True)
 def gemm_impl(request):
-    """every test runs on both kernel families: 1-CTA tcgen05 and CTA-pair (cta_group::2)"""
+    """every test runs on both kernel families: 1-CTA and CTA-pair (a cluster of two sharing a multicast B tile)"""
     lib = _lib.get_lib()
     lib.d3r_set_gemm_impl(request.param)
     yield request.param
@@ -96,8 +96,8 @@ def test_gemm_epilogues(cuda_device):
 @pytest.mark.timeout(300)
 @pytest.mark.parametrize('M,N,K', [(777, 512, 320), (1000, 768, 1024), (130, 256, 64), (4100, 1024, 4096)])
 def test_gemm_specialised_epilogues(cuda_device, M, N, K):
-    """The compile-time epilogue specialisations (N % 256 == 0): residual update through TMA reduce-add (rows past M
-    are clipped by the tensor map), bias/GELU -> bf16, bias/ReLU -> bf16, with and without bias."""
+    """The compile-time epilogue specialisations (N % 128 == 0): in-place residual update (rows past M
+    are left untouched), bias/GELU -> bf16, bias/ReLU -> bf16, with and without bias."""
     A = _rand((M, K), cuda_device, seed=21).bfloat16()
     B = _rand((N, K), cuda_device, scale=K ** -0.5, seed=22).bfloat16()
     bias = _rand((N,), cuda_device, seed=23)

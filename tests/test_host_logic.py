@@ -6,7 +6,7 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN, has_reference
+from conftest import GOLDEN, reference_golden
 from dust3r_b200.config import vitl_512_dpt, vitl_224_linear, state_dict_spec
 from dust3r_b200.image_pairs import make_pairs
 
@@ -57,7 +57,7 @@ def test_rotation_helpers_roundtrip():
 
 def test_optimizer_host_objects_on_cpu():
     """Construction, parametrisation and getters work without a GPU; the optimisation itself must
-    refuse to run anywhere but on a B200 (no CPU fallback)."""
+    refuse to run anywhere but on an H100 (no CPU fallback)."""
     from dust3r_b200.cloud_opt import global_aligner, GlobalAlignerMode
     from dust3r_b200.utils.synth import synth_pair_predictions
     from dust3r_b200._lib import D3RError
@@ -84,76 +84,66 @@ def test_optimizer_host_objects_on_cpu():
     assert out['pred1']['pts3d'].device.type == 'cpu'
 
 
-@pytest.mark.skipif(not has_reference(), reason='reference not mounted')
 def test_optimizer_init_matches_reference_draws():
-    """Same torch seed -> same initial parameters as the reference constructor (optimizer.py:29-33)."""
-    import sys
-    sys.path.insert(0, os.path.join(os.path.dirname(GOLDEN), '..', 'oracle', 'roma_stub'))
-    sys.path.insert(0, '/root/reference')
+    """Same torch seed -> same initial parameters as the reference constructor (optimizer.py:29-33); the reference's
+    values are stored in tests/golden/reference_live.npz (tests/golden/make_reference_golden.py)."""
     import copy
-    from dust3r.cloud_opt import global_aligner as ref_aligner, GlobalAlignerMode as RefMode
     from dust3r_b200.cloud_opt import global_aligner, GlobalAlignerMode
     from dust3r_b200.utils.synth import synth_pair_predictions
+    gold = reference_golden()
     n, H, W = 3, 16, 32
     edges = [(i, j) for i in range(n) for j in range(i)]
     out = synth_pair_predictions(n, edges, H, W, seed=2)
     torch.manual_seed(123)
-    ref = ref_aligner(copy.deepcopy(out), 'cpu', mode=RefMode.PointCloudOptimizer, verbose=False)
-    torch.manual_seed(123)
     net = global_aligner(copy.deepcopy(out), 'cpu', mode=GlobalAlignerMode.PointCloudOptimizer, verbose=False)
     for k in ('pw_poses', 'im_depthmaps', 'im_poses', 'im_focals', 'im_pp'):
-        assert torch.equal(getattr(ref, k).data, getattr(net, k).data), k
-    for a, b in zip(ref.get_pts3d(), net.get_pts3d()):
-        assert torch.allclose(a, b, atol=1e-5, rtol=1e-5)
-    assert torch.allclose(ref.get_pw_poses(), net.get_pw_poses(), atol=1e-6)
+        assert torch.equal(torch.from_numpy(gold[f'optinit|{k}']), getattr(net, k).data), k
+    pts = net.get_pts3d()
+    assert len(pts) == len([f for f in gold.files if f.startswith('optinit|pts3d|')])
+    for i, b in enumerate(pts):
+        assert torch.allclose(torch.from_numpy(gold[f'optinit|pts3d|{i}']), b, atol=1e-5, rtol=1e-5)
+    assert torch.allclose(torch.from_numpy(gold['optinit|pw']), net.get_pw_poses(), atol=1e-6)
 
 
 def test_geometry_helpers_match_live_reference():
     """xy_grid / geotrf / inv / depthmap_to_pts3d / depthmap_to_(absolute_)camera_coordinates against the reference's
-    dust3r/utils/geometry.py on random inputs (CPU), every calling convention the two hot paths use."""
-    import pytest
-    from conftest import has_reference
-    if not has_reference():
-        pytest.skip('reference not mounted')
-    import sys
+    dust3r/utils/geometry.py on random inputs (CPU), every calling convention the two hot paths use; the reference's
+    results are stored in tests/golden/reference_live.npz."""
     import numpy as np
     import torch
-    sys.path.insert(0, '/root/reference')
-    import dust3r.utils.geometry as ref
     import dust3r_b200.utils.geometry as mine
+    gold = reference_golden()
+    T_ = torch.from_numpy
     g = torch.Generator().manual_seed(0)
-    for kw in (dict(), dict(origin=(2, 3)), dict(homogeneous=True), dict(unsqueeze=0), dict(cat_dim=0)):
-        a, b = mine.xy_grid(7, 5, device='cpu', **kw), ref.xy_grid(7, 5, device='cpu', **kw)
-        assert type(a) is type(b) and torch.equal(a, b), kw
+    for c, kw in enumerate((dict(), dict(origin=(2, 3)), dict(homogeneous=True), dict(unsqueeze=0), dict(cat_dim=0))):
+        a = mine.xy_grid(7, 5, device='cpu', **kw)
+        assert torch.is_tensor(a) and torch.equal(a, T_(gold[f'geo|xy_t|{c}'])), kw
         if 'unsqueeze' not in kw:      # (the reference's numpy branch cannot unsqueeze)
-            a, b = mine.xy_grid(7, 5, **kw), ref.xy_grid(7, 5, **kw)          # device=None -> numpy
-            assert type(a) is type(b) and np.array_equal(a, b), kw
+            a = mine.xy_grid(7, 5, **kw)          # device=None -> numpy
+            assert isinstance(a, np.ndarray) and np.array_equal(a, gold[f'geo|xy_n|{c}']), kw
     T = torch.randn((3, 4, 4), generator=g)
     T[:, 3] = torch.tensor([0., 0, 0, 1])
     P = torch.randn((3, 6, 5, 3), generator=g)
-    assert torch.equal(mine.geotrf(T, P), ref.geotrf(T, P))
-    assert torch.equal(mine.geotrf(T[0], P[0]), ref.geotrf(T[0], P[0]))
+    assert torch.equal(mine.geotrf(T, P), T_(gold['geo|geotrf']))
+    assert torch.equal(mine.geotrf(T[0], P[0]), T_(gold['geo|geotrf0']))
     K = torch.tensor([[30., 0, 16], [0, 31, 12], [0, 0, 1]])
-    assert torch.equal(mine.geotrf(K, P[0], norm=1, ncol=2), ref.geotrf(K, P[0], norm=1, ncol=2))
-    assert np.allclose(mine.geotrf(T[0].numpy(), P[0].numpy()), ref.geotrf(T[0].numpy(), P[0].numpy()))
-    assert torch.equal(mine.inv(T), ref.inv(T)) and np.array_equal(mine.inv(T[0].numpy()), ref.inv(T[0].numpy()))
+    assert torch.equal(mine.geotrf(K, P[0], norm=1, ncol=2), T_(gold['geo|geotrf_k']))
+    assert np.allclose(mine.geotrf(T[0].numpy(), P[0].numpy()), gold['geo|geotrf_np'])
+    assert torch.equal(mine.inv(T), T_(gold['geo|inv'])) and np.array_equal(mine.inv(T[0].numpy()), gold['geo|inv_np'])
     depth = torch.rand((2, 6, 5), generator=g) + 0.5
-    for focal in (torch.rand((2, 1, 6, 5), generator=g) + 20, torch.rand((2, 2, 6, 5), generator=g) + 20):
+    for c, focal in enumerate((torch.rand((2, 1, 6, 5), generator=g) + 20, torch.rand((2, 2, 6, 5), generator=g) + 20)):
         pp = torch.tensor([[2.5, 3.0], [2.0, 3.5]])
-        assert torch.equal(mine.depthmap_to_pts3d(depth, focal, pp=pp), ref.depthmap_to_pts3d(depth, focal, pp=pp))
-        assert torch.equal(mine.depthmap_to_pts3d(depth, focal), ref.depthmap_to_pts3d(depth, focal))
+        assert torch.equal(mine.depthmap_to_pts3d(depth, focal, pp=pp), T_(gold[f'geo|d2p_pp|{c}']))
+        assert torch.equal(mine.depthmap_to_pts3d(depth, focal), T_(gold[f'geo|d2p|{c}']))
     d = depth[0].numpy()
     d[0, 0] = 0
-    for fn in ('depthmap_to_camera_coordinates',):
-        xa, ma = getattr(mine, fn)(d, K.numpy())
-        xb, mb = getattr(ref, fn)(d, K.numpy())
-        assert np.array_equal(xa, xb) and np.array_equal(ma, mb)
+    xa, ma = mine.depthmap_to_camera_coordinates(d, K.numpy())
+    assert np.array_equal(xa, gold['geo|cam_x']) and np.array_equal(ma, gold['geo|cam_m'])
     pose = np.eye(4, dtype=np.float32)
     pose[:3, :3] = np.float32([[0, -1, 0], [1, 0, 0], [0, 0, 1]])
     pose[:3, 3] = (1, 2, 3)
     xa, ma = mine.depthmap_to_absolute_camera_coordinates(d, K.numpy(), pose)
-    xb, mb = ref.depthmap_to_absolute_camera_coordinates(d, K.numpy(), pose)
-    assert np.allclose(xa, xb, atol=1e-6) and np.array_equal(ma, mb)
+    assert np.allclose(xa, gold['geo|abs_x'], atol=1e-6) and np.array_equal(ma, gold['geo|abs_m'])
 
 
 def test_stream_work_items_cover_every_slot_once_and_balance():
@@ -199,30 +189,19 @@ def test_find_reciprocal_matches_host_path_matches_live_reference():
     """utils/geometry.py:345-361 (scipy cKDTree on the CPU, like the reference); the CUDA path is checked against this one in
     tests/test_scene_ops_gpu.py."""
     import numpy as np
-    from conftest import has_reference
-    if not has_reference():
-        pytest.skip('reference not mounted')
-    import sys
-    sys.path.insert(0, '/root/reference')
-    from dust3r.utils.geometry import find_reciprocal_matches as ref
     from dust3r_b200.utils.geometry import find_reciprocal_matches as mine
+    gold = reference_golden()
     rng = np.random.default_rng(0)
     P1 = rng.standard_normal((700, 3)).astype(np.float32)
     P2 = np.concatenate((P1[:400] + 0.01 * rng.standard_normal((400, 3)).astype(np.float32), rng.standard_normal((150, 3)).astype(np.float32)))
-    a, b = ref(P1, P2), mine(P1, P2)
-    assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1]) and int(a[2]) == int(b[2]) > 300
+    b = mine(P1, P2)
+    assert np.array_equal(gold['recip|0'], b[0]) and np.array_equal(gold['recip|1'], b[1]) and int(gold['recip|2']) == int(b[2]) > 300
 
 
-def test_load_model_and_from_pretrained_on_a_reference_format_checkpoint(tmp_path):
-    """dust3r/model.py:27-43, 76-85: a checkpoint is {'args': Namespace(model="AsymmetricCroCo3DStereo(...)"), 'model': state
-    dict}; load_model rebuilds the network from the constructor string (ManyAR_PatchEmbed -> PatchEmbedDust3R,
-    landscape_only forced to False) and loads the weights; from_pretrained(path) of an existing file does the same.  No real
-    checkpoint is available offline: a small synthetic one is written in that format (and read back by the live reference's
-    own load_model when it is mounted)."""
+def synthetic_checkpoint(path):
+    """A small synthetic checkpoint in the released format; returns its full state dict."""
     import argparse
-    from conftest import has_reference
     from dust3r_b200.config import ModelConfig
-    from dust3r_b200.model import AsymmetricCroCo3DStereo, load_model
     from dust3r_b200.utils.synth import synth_state_dict
     cfg = ModelConfig(img_size=(96, 96), enc_embed_dim=192, enc_depth=3, enc_num_heads=3, dec_embed_dim=128, dec_depth=2,
                       dec_num_heads=2, head_type='linear', landscape_only=False)
@@ -230,10 +209,22 @@ def test_load_model_and_from_pretrained_on_a_reference_format_checkpoint(tmp_pat
     ctor = ("AsymmetricCroCo3DStereo(pos_embed='RoPE100', patch_embed_cls='ManyAR_PatchEmbed', img_size=(96, 96), head_type='linear', "
             "output_mode='pts3d', depth_mode=('exp', -inf, inf), conf_mode=('exp', 1, inf), enc_embed_dim=192, enc_depth=3, "
             "enc_num_heads=3, dec_embed_dim=128, dec_depth=2, dec_num_heads=2)")
-    path = str(tmp_path / 'synthetic_checkpoint.pth')
     # released checkpoints predate dec_blocks2 in some cases: drop them so that the duplication rule (model.py:91-98) is exercised
     stored = {k: v for k, v in sd.items() if not k.startswith('dec_blocks2')}
     torch.save({'args': argparse.Namespace(model=ctor), 'model': stored}, path)
+    return sd
+
+
+def test_load_model_and_from_pretrained_on_a_reference_format_checkpoint(tmp_path):
+    """dust3r/model.py:27-43, 76-85: a checkpoint is {'args': Namespace(model="AsymmetricCroCo3DStereo(...)"), 'model': state
+    dict}; load_model rebuilds the network from the constructor string (ManyAR_PatchEmbed -> PatchEmbedDust3R,
+    landscape_only forced to False) and loads the weights; from_pretrained(path) of an existing file does the same.  No real
+    checkpoint is available offline: a small synthetic one is written in that format; what the reference's own load_model
+    rebuilds from it (key set + sha256 of every tensor) is stored in tests/golden/reference_live.npz."""
+    import hashlib
+    from dust3r_b200.model import AsymmetricCroCo3DStereo, load_model
+    path = str(tmp_path / 'synthetic_checkpoint.pth')
+    sd = synthetic_checkpoint(path)
     net = load_model(path, 'cpu', verbose=False)
     assert isinstance(net, AsymmetricCroCo3DStereo) and net.landscape_only is False
     got = net.state_dict()
@@ -243,17 +234,11 @@ def test_load_model_and_from_pretrained_on_a_reference_format_checkpoint(tmp_pat
         assert torch.equal(got[k], src), k
     net2 = AsymmetricCroCo3DStereo.from_pretrained(path)
     assert all(torch.equal(a, b) for a, b in zip(net2.state_dict().values(), got.values()))
-    if has_reference():
-        import sys
-        sys.path.insert(0, '/root/reference')
-        from dust3r.model import load_model as ref_load_model
-        # torch >= 2.6 defaults torch.load to weights_only=True, which rejects the Namespace every DUSt3R checkpoint stores:
-        # allow it for the reference's own (unmodified) loader
-        with torch.serialization.safe_globals([argparse.Namespace]):
-            ref = ref_load_model(path, 'cpu', verbose=False)
-        rsd = ref.state_dict()
-        assert set(rsd) == set(got)
-        assert all(torch.equal(rsd[k], got[k]) for k in got)
+    gold = reference_golden()
+    keys = [str(k) for k in gold['loadmodel|keys']]
+    assert set(keys) == set(got)
+    sha = lambda t: hashlib.sha256(t.detach().cpu().contiguous().numpy().tobytes()).hexdigest()
+    assert all(sha(got[k]) == str(h) for k, h in zip(keys, gold['loadmodel|sha']))
 
 
 @pytest.mark.parametrize('imshapes,n_edges', [([(384, 512)] * 8, 28), ([(32, 48), (48, 32), (16, 64), (64, 64)], 5), ([(8, 8), (24, 40)], 1)])

@@ -1,7 +1,7 @@
 """load_images preprocessing (SURVEY §8f rank 4; dust3r/utils/image.py:62-128), CPU side:
 
   * oracle/image_oracle.py (integer restatement of Pillow's resize + crop + torchvision ImgNorm) is pinned bit-exactly against
-    Pillow / torchvision themselves, the unmodified reference's load_images (when /root/reference is mounted) and the
+    Pillow / torchvision themselves, the unmodified reference's load_images (stored outputs, tests/golden/reference_live.npz) and the
     committed golden fixture tests/golden/load_images.npz (reference outputs);
   * the product's host-side tables (dust3r_b200/utils/image.py) equal the oracle's;
   * the per-thread bodies of the CUDA kernels (dust3r_b200/csrc/resample_core.h) are compiled for the HOST
@@ -18,7 +18,7 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN, REFERENCE, ROOT, has_reference
+from conftest import GOLDEN, ROOT, reference_golden
 from dust3r_b200.utils import image as img_mod
 from dust3r_b200.utils.synth import synth_photo
 from oracle import image_oracle as io
@@ -28,6 +28,12 @@ CASES = [  # (H, W, size, square_ok)
     (300, 170, 224, False), (480, 640, 512, False), (640, 480, 512, False), (90, 70, 160, False), (384, 512, 512, False),
     (97, 1003, 512, False), (601, 397, 224, False), (224, 224, 224, False),
 ]
+
+
+def _digest(img):
+    """(shape, sha256 of the fp32 bytes): how tests/golden/reference_live.npz stores the reference's images."""
+    import hashlib
+    return tuple(img.shape), hashlib.sha256(img.detach().cpu().contiguous().numpy().tobytes()).hexdigest()
 
 
 def _write_png(tmp_path, arr, name):
@@ -92,21 +98,18 @@ def test_oracle_equals_golden_reference_outputs():
         assert out.shape == ref.shape and np.array_equal(out, ref), k
 
 
-@pytest.mark.skipif(not has_reference(), reason='reference tree not mounted')
 def test_oracle_and_host_port_equal_live_reference_load_images(tmp_path):
-    sys.path.insert(0, REFERENCE)
-    try:
-        from dust3r.utils.image import load_images as ref_load_images
-    finally:
-        sys.path.remove(REFERENCE)
+    """The reference's load_images on the same PNG files (its outputs stored in tests/golden/reference_live.npz)."""
+    gold = reference_golden()
     for k, (h, w, size, sq) in enumerate(CASES):
         photo = synth_photo(h, w, seed=10 + k)
         path = _write_png(tmp_path, photo, f'{k}.png')
-        ref = ref_load_images([path], size=size, square_ok=sq, verbose=False)[0]
+        ref = dict(true_shape=gold[f'loadimg|{k}|true_shape'], idx=int(gold[f'loadimg|{k}|idx']), instance=str(gold[f'loadimg|{k}|instance']))
+        ref_img = (tuple(gold[f'loadimg|{k}|img_shape'].tolist()), str(gold[f'loadimg|{k}|img_sha']))
         ours = img_mod.load_images([path], size=size, square_ok=sq, verbose=False)[0]
         out, true_shape = io.load_image_oracle(photo, size, sq)
-        assert torch.equal(ours['img'], ref['img']) and np.array_equal(ours['true_shape'], ref['true_shape'])
-        assert np.array_equal(out, ref['img'].numpy()) and np.array_equal(true_shape, ref['true_shape']), (h, w, size, sq)
+        assert _digest(ours['img']) == ref_img and np.array_equal(ours['true_shape'], ref['true_shape'])
+        assert _digest(torch.from_numpy(np.asarray(out, dtype=np.float32))) == ref_img and np.array_equal(true_shape, ref['true_shape']), (h, w, size, sq)
         assert ours['idx'] == ref['idx'] and ours['instance'] == ref['instance']
 
 
@@ -190,15 +193,10 @@ def test_load_images_folder_threads_keep_the_sequential_contract(tmp_path, capsy
             assert torch.equal(a['img'], b['img']) and np.array_equal(a['true_shape'], b['true_shape'])
             assert a['idx'] == b['idx'] and a['instance'] == b['instance']
     assert [v['idx'] for v in seq] == list(range(len(shapes))) and lines_seq.count(' - adding im') == len(shapes)
-    if has_reference():
-        sys.path.insert(0, REFERENCE)
-        try:
-            from dust3r.utils.image import load_images as ref_load_images
-        finally:
-            sys.path.remove(REFERENCE)
-        ref = ref_load_images(str(tmp_path), size=64, verbose=False)
-        assert len(ref) == len(seq)
-        for a, b in zip(seq, ref):
-            assert torch.equal(a['img'], b['img']) and np.array_equal(a['true_shape'], b['true_shape']) and a['instance'] == b['instance']
+    gold = reference_golden()     # the reference's load_images on the same folder
+    assert int(gold['folder|n']) == len(seq)
+    for k, a in enumerate(seq):
+        assert _digest(a['img']) == (tuple(gold[f'folder|{k}|img_shape'].tolist()), str(gold[f'folder|{k}|img_sha']))
+        assert np.array_equal(a['true_shape'], gold[f'folder|{k}|true_shape']) and a['instance'] == str(gold[f'folder|{k}|instance'])
     with pytest.raises(AssertionError):
         img_mod.load_images([os.path.join(str(tmp_path), 'readme.txt')], size=64, verbose=False)
