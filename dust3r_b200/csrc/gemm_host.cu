@@ -45,14 +45,16 @@ static int encode(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* d
 
 bool use_pair(int bn, int num_kb);
 
-int pick_block_n(int N, uint32_t flags) {
+int pick_block_n(int N, int mode, uint32_t flags) {
   if (flags & F_HEAD_FINAL) return 128;   // the head tail needs a whole 128-channel row in one tile
+  // 128x256 tiles for the specialised epilogues (every ViT projection): half the A traffic per FLOP of 128x128
+  if (N % 256 == 0 && pick_epi(mode, flags) != EPI_GENERIC) return 256;
   if (N % 128 == 0) return 128;
   if (N % 64 == 0) return 64;
   return (N > 128) ? 128 : 64;            // N % 32 == 0: the last tile is partly empty
 }
 
-// 0: 1-CTA kernels, 1: CTA-pair kernels (cluster of two, B tile multicast) whenever BLOCK_N == 128, 2 (default): pair
+// 0: 1-CTA kernels, 1: CTA-pair kernels (cluster of two, B tile multicast) whenever BLOCK_N >= 128, 2 (default): pair
 // kernels from g_pair_min_kb k-blocks of 64 on, 1-CTA kernels for the shortest reductions (K = 96 / 192 of the DPT
 // re-assembly), whose time goes to the epilogue rather than to operand traffic.
 static int g_impl = 2;
@@ -77,7 +79,8 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p,
   }
   const char* tag = (p.mode == 1) ? ((p.flags & F_HEAD_FINAL) ? (PAIR ? "conv3x3_head_tail_2cta" : "conv3x3_head_tail")
                                                               : (PAIR ? "conv3x3_wgmma_2cta" : "conv3x3_wgmma"))
-                                  : (PAIR ? "gemm_wgmma_2cta_bn128" : (BN == 128 ? "gemm_wgmma_bn128" : "gemm_wgmma_bn64"));
+                                  : (BN == 256 ? (PAIR ? "gemm_wgmma_2cta_bn256" : "gemm_wgmma_bn256")
+                                               : (PAIR ? "gemm_wgmma_2cta_bn128" : (BN == 128 ? "gemm_wgmma_bn128" : "gemm_wgmma_bn64")));
   char detail[96];
   snprintf(detail, sizeof(detail), "M=%d N=%d K=%d flags=0x%x mode=%d epi=%d", p.M, p.N, p.K, (unsigned)p.flags, p.mode, EPI);
   prof::Scope scope(tag, st, 2.0 * double(p.M) * double(p.N) * double(p.K), 0.0, 1, detail);
@@ -86,24 +89,26 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p,
   return D3R_OK;
 }
 
-template <bool PAIR>
-static int dispatch_bn128(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int m_tiles, int n_tiles, cudaStream_t st) {
+template <int BN, bool PAIR>
+static int dispatch_epi(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int m_tiles, int n_tiles, cudaStream_t st) {
   switch (epi) {
-    case EPI_RESID: return launch<128, EPI_RESID, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
-    case EPI_ACT: return launch<128, EPI_ACT, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
-    case EPI_ROPE: return launch<128, EPI_ROPE, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
-    default: return launch<128, EPI_GENERIC, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
+    case EPI_RESID: return launch<BN, EPI_RESID, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
+    case EPI_ACT: return launch<BN, EPI_ACT, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
+    case EPI_ROPE: return launch<BN, EPI_ROPE, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
   }
+  if constexpr (BN == 128) return launch<128, EPI_GENERIC, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
+  set_error("no BLOCK_N %d kernel for the generic epilogue", BN);
+  return D3R_ERR_INVALID;
 }
 
 static int dispatch(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int m_tiles, cudaStream_t st) {
   const int n_tiles = (p.N + bn - 1) / bn;
-  // epilogue specialisation (BLOCK_N = 128 only: every hot projection of the two ViTs has N % 128 == 0)
-  const int epi = (bn == 128) ? pick_epi(p.mode, p.flags) : EPI_GENERIC;
+  // epilogue specialisations exist for BLOCK_N 128 and 256 (every hot projection of the two ViTs has N % 256 == 0)
+  const int epi = (bn >= 128) ? pick_epi(p.mode, p.flags) : EPI_GENERIC;
+  const bool pair = use_pair(bn, p.num_kb);
   switch (bn) {
-    case 128:
-      if (use_pair(bn, p.num_kb)) return dispatch_bn128<true>(epi, ta, tb, p, m_tiles, n_tiles, st);
-      return dispatch_bn128<false>(epi, ta, tb, p, m_tiles, n_tiles, st);
+    case 256: return pair ? dispatch_epi<256, true>(epi, ta, tb, p, m_tiles, n_tiles, st) : dispatch_epi<256, false>(epi, ta, tb, p, m_tiles, n_tiles, st);
+    case 128: return pair ? dispatch_epi<128, true>(epi, ta, tb, p, m_tiles, n_tiles, st) : dispatch_epi<128, false>(epi, ta, tb, p, m_tiles, n_tiles, st);
     case 64: return launch<64, EPI_GENERIC, false>(ta, tb, p, m_tiles, n_tiles, st);
   }
   set_error("unsupported BLOCK_N %d", bn);
@@ -126,7 +131,7 @@ int gemm_bf16(const void* A, long long lda, const void* B, Params p, cudaStream_
   D3R_CHECK_ARG((reinterpret_cast<uintptr_t>(A) & 15) == 0 && (reinterpret_cast<uintptr_t>(B) & 15) == 0, "gemm: operands must be 16-byte aligned");
   p.mode = 0;
   p.num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
-  const int bn = pick_block_n(p.N, p.flags);
+  const int bn = pick_block_n(p.N, p.mode, p.flags);
   CUtensorMap ta, tb;
   {
     cuuint64_t dims[2] = {(cuuint64_t)p.K, (cuuint64_t)p.M};
@@ -157,7 +162,7 @@ int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, 
   p.tiles_x = (W + p.tile_w - 1) / p.tile_w;
   p.tiles_y = (H + p.tile_h - 1) / p.tile_h;
   p.ldo = Cout;
-  const int bn = pick_block_n(p.N, p.flags);
+  const int bn = pick_block_n(p.N, p.mode, p.flags);
   CUtensorMap ta, tb;
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};

@@ -4,7 +4,7 @@
 
 namespace d3r {
 namespace gemm {
-int pick_block_n(int N, uint32_t flags);
+int pick_block_n(int N, int mode, uint32_t flags);
 void set_impl(int impl);
 void set_pair_min_kb(int kb);
 // A: [M][lda] bf16 row-major (K valid columns), B: [N][K] bf16.  p.{M,N,K,flags,out,...} filled by the caller.

@@ -101,7 +101,7 @@ template <int BLOCK_N>
 struct Cfg {
   static constexpr int kStageA = BLOCK_M * BLOCK_K * 2;
   static constexpr int kStageB = BLOCK_N * BLOCK_K * 2;
-  static constexpr int kStages = (BLOCK_N >= 128) ? 6 : 8;
+  static constexpr int kStages = (BLOCK_N == 256) ? 4 : (BLOCK_N == 128) ? 6 : 8;
   static constexpr int kSmemBytes = kStages * (kStageA + kStageB) + 1024 /*align*/ + 256 /*barriers*/ + (4 * 128 + 16) * 4 /*head*/;
   static_assert(kSmemBytes <= 227 * 1024, "shared memory of one CTA");
 };
@@ -251,7 +251,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
         for (int k = 0; k < BLOCK_K / WGMMA_K; ++k) {
           // advance 32 B (= 16 bf16 of K) inside the 128 B swizzle row: +2 in 16-byte units
-          if constexpr (BLOCK_N == 128) ptx::wgmma_m64n128k16_ss(acc, da + uint64_t(2 * k), db + uint64_t(2 * k), (kb | k) != 0 ? 1u : 0u);
+          if constexpr (BLOCK_N == 256) ptx::wgmma_m64n256k16_ss(acc, da + uint64_t(2 * k), db + uint64_t(2 * k), (kb | k) != 0 ? 1u : 0u);
+          else if constexpr (BLOCK_N == 128) ptx::wgmma_m64n128k16_ss(acc, da + uint64_t(2 * k), db + uint64_t(2 * k), (kb | k) != 0 ? 1u : 0u);
           else ptx::wgmma_m64n64k16_ss(acc, da + uint64_t(2 * k), db + uint64_t(2 * k), (kb | k) != 0 ? 1u : 0u);
         }
         ptx::wgmma_commit();
