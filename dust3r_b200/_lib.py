@@ -56,7 +56,7 @@ def _declare(lib):
     lib.d3r_prof_dump.argtypes = [C.c_char_p, C.c_int]
     lib.d3r_sizeof_align_desc.restype = C.c_int
     lib.d3r_align_workspace_floats.restype = i64
-    lib.d3r_align_workspace_floats.argtypes = [i32, i32, i32, i32]
+    lib.d3r_align_workspace_floats.argtypes = [i32, i32]
     for name in ('d3r_align_prepare',):
         getattr(lib, name).restype = C.c_int
         getattr(lib, name).argtypes = [C.POINTER(AlignDesc), vp]
@@ -66,8 +66,6 @@ def _declare(lib):
     lib.d3r_align_overflow_flag.argtypes = [C.POINTER(AlignDesc), C.POINTER(C.c_int32), vp]
     lib.d3r_align_pts3d.restype = C.c_int
     lib.d3r_align_pts3d.argtypes = [C.POINTER(AlignDesc), vp, vp]
-    lib.d3r_align_pack_obs.restype = C.c_int
-    lib.d3r_align_pack_obs.argtypes = [vp, vp, vp, i64, i64, vp]
     lib.d3r_align_pack_entries.restype = C.c_int
     lib.d3r_align_pack_entries.argtypes = [vp, i32, i32, i32, i32, vp, vp]
     lib.d3r_clean_pointcloud.restype = C.c_int

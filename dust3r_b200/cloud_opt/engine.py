@@ -1,5 +1,5 @@
-"""Host driver of the fused alignment kernel (csrc/align_step.cu) — builds the HBM layout the kernel
-streams and launches `d3r_align_run` through the C ABI.
+"""Host driver of the fused alignment kernels (csrc/align_stream.cu when every image has P % 4 == 0, csrc/align_step.cu
+for any shape) — builds the HBM layout the kernels stream and launches `d3r_align_run` through the C ABI.
 
 HBM layout (all fp32, owned by torch):
   obs        float4[ sum over entries P_img ]   (pred.x, pred.y, pred.z, conf_trf(conf)) per pixel;
@@ -195,7 +195,7 @@ class AlignEngine:
             torch.cuda.current_stream(dev).synchronize()     # the staged copies may be freed after this point
         del keep, table_dev
         self._build_items(ent_ptr, ent_obs_off, slots) if stream else self._no_items()
-        nws = self.lib.d3r_align_workspace_floats(n, E, self.n_chunks, self.max_chunks)
+        nws = self.lib.d3r_align_workspace_floats(n, E)
         self.workspace = torch.zeros((nws,), dtype=torch.float32, device=dev)
         self.counters = torch.zeros((n + 2,), dtype=torch.int32, device=dev)
         self.n_small = 11 * n + 10 * E

@@ -1,9 +1,11 @@
-// Shared device code of the alignment kernels (csrc/align_step.cu: general CTA-per-chunk kernel; csrc/align_stream.cu:
+// Shared code of the alignment kernels (csrc/align_step.cu: general CTA-per-chunk kernel; csrc/align_stream.cu:
 // persistent warp-streaming kernel): workspace carving, fixed-point accumulation, quaternion / Adam math, the
-// derived-transform refresh and the small-parameter step run by the last CTA of every iteration.
+// derived-transform refresh, the small-parameter step run by the last CTA of every iteration, and the iteration launch.
 #pragma once
 #include "d3r_common.cuh"
+#include "pdl.cuh"
 #include "prof.h"
+#include "sm90_ptx.cuh"
 
 namespace d3r {
 namespace align {
@@ -20,10 +22,9 @@ constexpr int kImgT = 16;                  // R (9) T (3) 1/fx 1/fy cx cy
 struct Workspace {
   float* edgeT;          // [E][12]
   float* imgT;           // [n][16]
-  long long* ent_acc;    // [2E][13]  fixed-point (2^44) accumulators, zero between launches
+  long long* ent_acc;    // [2E][13]  fixed-point (2^40) accumulators, zero between launches
   long long* img_acc;    // [n][12]
-  float* g_edge;         // [E][10]   small-step scratch: pairwise-pose / adaptor gradients
-  float* g_img;          // [n][11]   pose (7) / focal (2) / pp (2) gradients
+  float* grad;           // [11n + 10E] multi-pass small-step scratch: raw gradients in the flat parameter layout
   int* flags;            // [4]       [0] = fixed-point overflow seen
   float* entT;           // [2E][12]  streaming kernel: -M (9), -t (3) of the entry's edge, indexed by entry (no indirection)
   float* geomE;          // [E][24]   cache for the next small step: R (9) ad (3) s T (3) qhat (4) |q| sg^2 exp|t| (3)
@@ -40,8 +41,7 @@ __host__ __device__ inline Workspace carve(float* ws, int n, int E) {
   w.imgT = ws + o;     o += align4(int64_t(n) * kImgT);
   w.ent_acc = reinterpret_cast<long long*>(ws + o); o += align4(int64_t(2) * E * kEntVals * 2);
   w.img_acc = reinterpret_cast<long long*>(ws + o); o += align4(int64_t(n) * kImgVals * 2);
-  w.g_edge = ws + o;   o += align4(int64_t(E) * 10);
-  w.g_img = ws + o;    o += align4(int64_t(n) * 11);
+  w.grad = ws + o;     o += align4(int64_t(n) * 11 + int64_t(E) * 10);
   w.flags = reinterpret_cast<int*>(ws + o); o += 4;
   w.entT = ws + o;     o += align4(int64_t(2) * E * kEdgeT);
   w.geomE = ws + o;    o += align4(int64_t(E) * 24);
@@ -51,7 +51,7 @@ __host__ __device__ inline Workspace carve(float* ws, int n, int E) {
 
 inline int64_t workspace_floats(int n, int E) {
   return align4(int64_t(E) * kEdgeT) + align4(int64_t(n) * kImgT) + align4(int64_t(2) * E * kEntVals * 2) +
-         align4(int64_t(n) * kImgVals * 2) + align4(int64_t(E) * 10) + align4(int64_t(n) * 11) + 4 +
+         align4(int64_t(n) * kImgVals * 2) + align4(int64_t(n) * 11 + int64_t(E) * 10) + 4 +
          align4(int64_t(2) * E * kEdgeT) + align4(int64_t(E) * 24) + align4(int64_t(n) * 20);
 }
 
@@ -161,42 +161,58 @@ __device__ __forceinline__ float block_sum8(float v, float* slot /* 8 floats */)
   return t;
 }
 
-struct EdgeGeom {
-  float R[9], T[3], ad[3], s, qh[4], qn;
-};
-__device__ __forceinline__ void edge_geom(const float* p8, float a0, float a1, const d3r_align_desc& D, float mean_sigma,
-                                          float log_base, EdgeGeom& g) {
-  quat_to_R(p8, g.R, g.qh, &g.qn);
-  g.s = expf(p8[7]);
-  if (D.norm_pw_scale) g.s *= expf(log_base - mean_sigma);
-  g.ad[0] = a0; g.ad[1] = a0; g.ad[2] = a1;
-  if (D.norm_pw_scale) {
-    const float mu = (a0 + a0 + a1) / 3.f;
-    g.ad[0] -= mu; g.ad[1] -= mu; g.ad[2] -= mu;
-  }
+template <int N>
+__device__ __forceinline__ void load_row(const float* __restrict__ src, float (&c)[N]) {
+  const float4* c4 = reinterpret_cast<const float4*>(src);
 #pragma unroll
-  for (int b = 0; b < 3; ++b) g.ad[b] = expf(g.ad[b] / D.pw_break);
-#pragma unroll
-  for (int a = 0; a < 3; ++a) g.T[a] = signed_expm1f(p8[4 + a]);
+  for (int k = 0; k < N / 4; ++k) { const float4 t = c4[k]; c[4 * k] = t.x; c[4 * k + 1] = t.y; c[4 * k + 2] = t.z; c[4 * k + 3] = t.w; }
 }
 
-// what the next small step needs of an edge's / image's geometry (recomputing it there sits on the critical path)
-__device__ __forceinline__ void store_geom_edge(float* __restrict__ c, const EdgeGeom& g, const float* p8) {
+// Derived transforms of edge e from its pairwise pose p8 and adaptors a0, a1: the edgeT row M = s*R*diag(adapt) (9),
+// s*T (3); for the streaming kernel the same row negated once per entry in entT (both sides of the edge see the same
+// transform, read without indirection); and the geometry cache the next small step reads instead of recomputing it.
+__device__ __forceinline__ void edge_refresh(const d3r_align_desc& D, const Workspace& ws, int e, const float* p8, float a0, float a1,
+                                             float mean_sigma, float log_base) {
+  float c[kGeomE];   // R (9) ad (3) s T (3) qhat (4) |q| sg^2 exp|t| (3)
+  float* R = c; float* ad = c + 9; float* T = c + 13;
+  quat_to_R(p8, R, c + 16, c + 20);
+  float s = expf(p8[7]);
+  if (D.norm_pw_scale) s *= expf(log_base - mean_sigma);   // base_opt.py:178-184
+  c[12] = s;
+  // adaptors (base_opt.py:143-148): adapt3 = exp((cat(a0,a0,a1) - mean)/pw_break)
+  ad[0] = a0; ad[1] = a0; ad[2] = a1;
+  if (D.norm_pw_scale) {
+    const float mu = (a0 + a0 + a1) / 3.f;
+    ad[0] -= mu; ad[1] -= mu; ad[2] -= mu;
+  }
 #pragma unroll
-  for (int k = 0; k < 9; ++k) c[k] = g.R[k];
+  for (int b = 0; b < 3; ++b) ad[b] = expf(ad[b] / D.pw_break);
 #pragma unroll
-  for (int k = 0; k < 3; ++k) { c[9 + k] = g.ad[k]; c[13 + k] = g.T[k]; }
-  c[12] = g.s;
+  for (int a = 0; a < 3; ++a) T[a] = signed_expm1f(p8[4 + a]);
+  float o[kEdgeT];
 #pragma unroll
-  for (int k = 0; k < 4; ++k) c[16 + k] = g.qh[k];
-  c[20] = g.qn;
+  for (int a = 0; a < 3; ++a)
+#pragma unroll
+    for (int b = 0; b < 3; ++b) o[a * 3 + b] = s * R[a * 3 + b] * ad[b];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) o[9 + a] = s * T[a];
+#pragma unroll
+  for (int k = 0; k < kEdgeT; ++k) ws.edgeT[e * kEdgeT + k] = o[k];
+  if (D.stream_kernel) {
+    const int ei = D.edge_ent[e * 2 + 0], ej = D.edge_ent[e * 2 + 1];
+#pragma unroll
+    for (int k = 0; k < kEdgeT; ++k) { ws.entT[int64_t(ei) * kEdgeT + k] = -o[k]; ws.entT[int64_t(ej) * kEdgeT + k] = -o[k]; }
+  }
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
     const float t = p8[4 + a];
     const float sg = (t > 0.f) - (t < 0.f);
     c[21 + a] = sg * sg * expf(fabsf(t));
   }
+#pragma unroll
+  for (int k = 0; k < kGeomE; ++k) ws.geomE[int64_t(e) * kGeomE + k] = c[k];
 }
+
 __device__ __forceinline__ void image_transform_row(const d3r_align_desc& D, const float* q7, float f0, float f1, float pp0, float pp1,
                                                     int Hh, int Ww, float* __restrict__ o, float* __restrict__ c) {
   float R[9], qh[4], qn;
@@ -221,6 +237,97 @@ __device__ __forceinline__ void image_transform_row(const d3r_align_desc& D, con
   o[15] = 0.5f * float(Hh) + 10.f * pp1;
 }
 
+// Raw gradients of edge e -- pairwise pose (quaternion 4, translation 3, log-scale 1) and adaptors (2) -- from the sums
+// of its two entries (si, sj: sum g (x) q (9), sum g (3)) and its cached geometry c (geomE row), written to `grad` in the
+// flat parameter layout.  Returns dL/dlog-scale, whose mean over the edges (the coupling of the normalised scales) the
+// Adam step subtracts.
+__device__ __forceinline__ float edge_grad(const d3r_align_desc& D, const SmallLayout& L, int e, const float* si, const float* sj,
+                                           const float* c, float* grad) {
+  const float* R = c; const float* ad = c + 9; const float sc = c[12]; const float* T = c + 13; const float* qh = c + 16;
+  float dM[9], dt[3];
+#pragma unroll
+  for (int k = 0; k < 9; ++k) dM[k] = -(si[k] + sj[k]);   // dL/dM_ab = -sum g_a q_b
+#pragma unroll
+  for (int a = 0; a < 3; ++a) dt[a] = -(si[9 + a] + sj[9 + a]);
+  float dLds = 0.f, dR[9], dad[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+#pragma unroll
+    for (int b = 0; b < 3; ++b) {
+      dLds += dM[a * 3 + b] * R[a * 3 + b] * ad[b];
+      dR[a * 3 + b] = dM[a * 3 + b] * sc * ad[b];
+      dad[b] += dM[a * 3 + b] * sc * R[a * 3 + b];
+    }
+    dLds += dt[a] * T[a];
+  }
+  float ge[10];
+  quat_backward(dR, qh, c[20], ge);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) ge[4 + a] = dt[a] * sc * c[21 + a];
+  ge[7] = dLds * sc;
+  float gad[3];
+#pragma unroll
+  for (int b = 0; b < 3; ++b) gad[b] = dad[b] * ad[b] / D.pw_break;
+  if (D.norm_pw_scale) { const float mu = (gad[0] + gad[1] + gad[2]) / 3.f; gad[0] -= mu; gad[1] -= mu; gad[2] -= mu; }
+  ge[8] = gad[0] + gad[1];
+  ge[9] = gad[2];
+#pragma unroll
+  for (int k = 0; k < 8; ++k) grad[L.pw + e * 8 + k] = ge[k];
+  grad[L.adapt + e * 2 + 0] = ge[8];
+  grad[L.adapt + e * 2 + 1] = ge[9];
+  return dLds * sc;
+}
+
+// Raw gradients of image i -- pose (quaternion 4, translation 3), focals (2), principal point (2) -- from its sums
+// S (sum G (x) c (9), sum G (3); overwritten) and its cached geometry c (geomI row), written to `grad` in the flat
+// parameter layout.
+__device__ __forceinline__ void image_grad(const d3r_align_desc& D, const SmallLayout& L, int i, float (&S)[kImgVals], const float* c,
+                                           float* grad) {
+  const float* R = c;
+  if (D.stream_kernel) {   // the streaming kernel accumulates sum G (x) Y, Y = R c: sum G (x) c = (sum G (x) Y) R
+    float Sc[9];
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+#pragma unroll
+      for (int b = 0; b < 3; ++b) Sc[a * 3 + b] = S[a * 3 + 0] * R[0 * 3 + b] + S[a * 3 + 1] * R[1 * 3 + b] + S[a * 3 + 2] * R[2 * 3 + b];
+#pragma unroll
+    for (int k = 0; k < 9; ++k) S[k] = Sc[k];
+  }
+  float gi[11];
+  quat_backward(S, c + 9, c[13], gi);
+#pragma unroll
+  for (int a = 0; a < 3; ++a) gi[4 + a] = S[9 + a] * c[14 + a];
+  // focals: c_x = d (u-cx)/fx, fx = exp(phi/focal_break);  pp: cx = W/2 + 10 pp_x
+  float gfx = 0.f, gfy = 0.f, gpx = 0.f, gpy = 0.f;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    gfx += R[a * 3 + 0] * S[a * 3 + 0];
+    gfy += R[a * 3 + 1] * S[a * 3 + 1];
+    gpx += R[a * 3 + 0] * S[a * 3 + 2];
+    gpy += R[a * 3 + 1] * S[a * 3 + 2];
+  }
+  gfx = -gfx / D.focal_break;
+  gfy = -gfy / D.focal_break;
+  gi[7] = D.tied_focal ? gfx + gfy : gfx;     // one shared focal: both slots get the summed gradient and evolve identically
+  gi[8] = D.tied_focal ? gfx + gfy : gfy;
+  gi[9] = -10.f * gpx / c[17];
+  gi[10] = -10.f * gpy / c[18];
+#pragma unroll
+  for (int k = 0; k < 7; ++k) grad[L.poses + i * 7 + k] = gi[k];
+  grad[L.focals + i * 2 + 0] = gi[7]; grad[L.focals + i * 2 + 1] = gi[8];
+  grad[L.pp + i * 2 + 0] = gi[9]; grad[L.pp + i * 2 + 1] = gi[10];
+}
+
+__device__ __forceinline__ bool is_log_scale(const SmallLayout& L, int idx) { return idx >= L.pw && idx < L.adapt && ((idx - L.pw) & 7) == 7; }
+
+// Adam step of the trainable flat parameter idx with raw gradient g: returns the new value and updates the moments m, v.
+// With norm_pw_scale the log-scales see the mean-coupling term of the normalisation.
+__device__ __forceinline__ float adam_param(const d3r_align_desc& D, const SmallLayout& L, int idx, float p, float& m, float& v, float g,
+                                            float coupling, float step_size, float bc2s) {
+  if (is_log_scale(L, idx) && D.norm_pw_scale) g -= coupling;
+  return adam_update(p, g, m, v, D.beta1, D.beta2, step_size, bc2s, D.adam_eps);
+}
+
 // image i is handled by thread (blockDim-1-i) so that images and edges land on different warps
 __device__ __forceinline__ int img_of_thread(int it) { return int(blockDim.x) - 1 - int(threadIdx.x) + it * int(blockDim.x); }
 
@@ -236,25 +343,7 @@ static __device__ void compute_transforms(const d3r_align_desc& D, const Workspa
     float p8[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) p8[k] = sm[L.pw + e * 8 + k];
-    const float a0 = sm[L.adapt + e * 2 + 0], a1 = sm[L.adapt + e * 2 + 1];
-    EdgeGeom g;
-    edge_geom(p8, a0, a1, D, mean_sigma, log_base, g);
-    float* o = ws.edgeT + e * kEdgeT;
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-#pragma unroll
-      for (int b = 0; b < 3; ++b) o[a * 3 + b] = g.s * g.R[a * 3 + b] * g.ad[b];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) o[9 + a] = g.s * g.T[a];
-    if (D.stream_kernel) {   // the streaming kernel reads -M, -t per ENTRY (both sides of the edge see the same transform)
-#pragma unroll
-      for (int side = 0; side < 2; ++side) {
-        float* oe = ws.entT + int64_t(D.edge_ent[e * 2 + side]) * kEdgeT;
-#pragma unroll
-        for (int k = 0; k < kEdgeT; ++k) oe[k] = -o[k];
-      }
-    }
-    store_geom_edge(ws.geomE + int64_t(e) * kGeomE, g, p8);
+    edge_refresh(D, ws, e, p8, sm[L.adapt + e * 2 + 0], sm[L.adapt + e * 2 + 1], mean_sigma, log_base);
   }
   for (int r = 0, i = img_of_thread(0); i < n; i = img_of_thread(++r)) {
     float p7[7];
@@ -267,7 +356,10 @@ static __device__ void compute_transforms(const d3r_align_desc& D, const Workspa
   }
 }
 
-// backward through the small parameters + Adam; run by the last CTA of the grid
+// Multi-pass small-parameter step: backward through the small parameters + Adam, run by the last CTA of the grid for any
+// graph size and for eval_only.  Strided loops over edges / images / parameters, gradients through global scratch, the
+// loss summed over the entries in order.  The geometry of every edge and image is read from the cache that
+// prepare_kernel and every step's refresh keep current.
 static __device__ __noinline__ void small_param_step(const d3r_align_desc& D, const Workspace& ws, int it, float* s_red) {
   const int n = D.n_imgs, E = D.n_edges;
   const SmallLayout L(n, E);
@@ -276,119 +368,32 @@ static __device__ __noinline__ void small_param_step(const d3r_align_desc& D, co
   float* __restrict__ av = D.small_v;
   const uint8_t* __restrict__ tr = D.small_trainable;
   const float step_size = D.sched[it * 4 + 1], bc2s = D.sched[it * 4 + 2];
-  const float b1 = D.beta1, b2 = D.beta2, eps = D.adam_eps;
 
-  // phase 0: loss (fixed order over entries) and mean log-scale, one barrier
-  float lpart = 0.f, spart = 0.f;
+  // phase 0: loss (fixed order over entries), one barrier
+  float lpart = 0.f;
   int bad = 0;
   for (int k = threadIdx.x; k < 2 * E; k += blockDim.x) lpart += fix_get(ws.ent_acc + k * kEntVals + 12, bad);
-  for (int e = threadIdx.x; e < E; e += blockDim.x) spart += sm[L.pw + e * 8 + 7];
-  lpart = warp_sum(lpart);
-  spart = warp_sum(spart);
-  if ((threadIdx.x & 31) == 0) { s_red[threadIdx.x >> 5] = lpart; s_red[8 + (threadIdx.x >> 5)] = spart; }
-  __syncthreads();
-  float loss = 0.f, mean_sigma = 0.f;
-#pragma unroll
-  for (int w = 0; w < kWarps; ++w) { loss += s_red[w]; mean_sigma += s_red[8 + w]; }
-  mean_sigma /= float(E);
+  const float loss = block_sum8(lpart, s_red);
   if (threadIdx.x == 0) D.loss_out[it] = loss;
-  const float log_base = logf(D.base_scale);
   D3R_TSTAMP(0);
 
-  // phase 1: gradients -> scratch.  edges on low thread ids, images on high thread ids (different warps).
+  // phase 1: gradients -> ws.grad.  edges on low thread ids, images on high thread ids (different warps).
   float coupl = 0.f;
   if (!D.eval_only) {
     for (int e = threadIdx.x; e < E; e += blockDim.x) {
-      float p8[8], si[12], sj[12];
       const int ei = D.edge_ent[e * 2 + 0], ej = D.edge_ent[e * 2 + 1];
-#pragma unroll
-      for (int k = 0; k < 8; ++k) p8[k] = sm[L.pw + e * 8 + k];
-      const float a0 = sm[L.adapt + e * 2 + 0], a1 = sm[L.adapt + e * 2 + 1];
+      float si[12], sj[12], c[kGeomE];
 #pragma unroll
       for (int k = 0; k < 12; ++k) { si[k] = fix_get(ws.ent_acc + ei * kEntVals + k, bad); sj[k] = fix_get(ws.ent_acc + ej * kEntVals + k, bad); }
-      EdgeGeom g;
-      edge_geom(p8, a0, a1, D, mean_sigma, log_base, g);
-      float dM[9], dt[3];
-#pragma unroll
-      for (int k = 0; k < 9; ++k) dM[k] = -(si[k] + sj[k]);   // dL/dM_ab = -sum g_a q_b
-#pragma unroll
-      for (int a = 0; a < 3; ++a) dt[a] = -(si[9 + a] + sj[9 + a]);
-      float dLds = 0.f, dR[9], dad[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-#pragma unroll
-        for (int b = 0; b < 3; ++b) {
-          dLds += dM[a * 3 + b] * g.R[a * 3 + b] * g.ad[b];
-          dR[a * 3 + b] = dM[a * 3 + b] * g.s * g.ad[b];
-          dad[b] += dM[a * 3 + b] * g.s * g.R[a * 3 + b];
-        }
-        dLds += dt[a] * g.T[a];
-      }
-      float gr[10];
-      quat_backward(dR, g.qh, g.qn, gr);
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        const float t = p8[4 + a];
-        const float sg = (t > 0.f) - (t < 0.f);
-        gr[4 + a] = dt[a] * g.s * sg * sg * expf(fabsf(t));
-      }
-      gr[7] = dLds * g.s;             // the mean-coupling term is subtracted in phase 2
-      coupl += dLds * g.s;
-      // adaptors (base_opt.py:143-148): adapt3 = exp((cat(a0,a0,a1) - mean)/pw_break)
-      float gad[3];
-#pragma unroll
-      for (int b = 0; b < 3; ++b) gad[b] = dad[b] * g.ad[b] / D.pw_break;
-      if (D.norm_pw_scale) { const float mu = (gad[0] + gad[1] + gad[2]) / 3.f; gad[0] -= mu; gad[1] -= mu; gad[2] -= mu; }
-      gr[8] = gad[0] + gad[1];
-      gr[9] = gad[2];
-#pragma unroll
-      for (int k = 0; k < 10; ++k) ws.g_edge[e * 10 + k] = gr[k];
+      load_row(ws.geomE + int64_t(e) * kGeomE, c);
+      coupl += edge_grad(D, L, e, si, sj, c, ws.grad);
     }
     for (int r = 0, i = img_of_thread(0); i < n; i = img_of_thread(++r)) {
-      float q7[7], S[12];
+      float S[kImgVals], c[kGeomI];
 #pragma unroll
-      for (int k = 0; k < 7; ++k) q7[k] = sm[L.poses + i * 7 + k];
-      const float f0 = sm[L.focals + i * 2 + 0], f1 = sm[L.focals + i * 2 + 1];
-#pragma unroll
-      for (int k = 0; k < 12; ++k) S[k] = fix_get(ws.img_acc + i * kImgVals + k, bad);   // S[a*3+b] = sum G_a c_b ; S[9+a] = sum G_a
-      float R[9], qh[4], qn;
-      quat_to_R(q7, R, qh, &qn);
-      if (D.stream_kernel) {
-        // the streaming kernel accumulates sum G (x) Y with Y = X - T = R c (world frame): sum G (x) c = (sum G (x) Y) R
-        float Sc[9];
-#pragma unroll
-        for (int a = 0; a < 3; ++a)
-#pragma unroll
-          for (int b = 0; b < 3; ++b) Sc[a * 3 + b] = S[a * 3 + 0] * R[0 * 3 + b] + S[a * 3 + 1] * R[1 * 3 + b] + S[a * 3 + 2] * R[2 * 3 + b];
-#pragma unroll
-        for (int k = 0; k < 9; ++k) S[k] = Sc[k];
-      }
-      float gr[11];
-      quat_backward(S, qh, qn, gr);
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        const float t = q7[4 + a];
-        const float sg = (t > 0.f) - (t < 0.f);
-        gr[4 + a] = S[9 + a] * sg * sg * expf(fabsf(t));
-      }
-      // focals: c_x = d (u-cx)/fx, fx = exp(phi/focal_break);  pp: cx = W/2 + 10 pp_x
-      float gfx = 0.f, gfy = 0.f, gpx = 0.f, gpy = 0.f;
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        gfx += R[a * 3 + 0] * S[a * 3 + 0];
-        gfy += R[a * 3 + 1] * S[a * 3 + 1];
-        gpx += R[a * 3 + 0] * S[a * 3 + 2];
-        gpy += R[a * 3 + 1] * S[a * 3 + 2];
-      }
-      gfx = -gfx / D.focal_break;
-      gfy = -gfy / D.focal_break;
-      // one shared focal: both slots get the summed gradient and evolve identically
-      gr[7] = D.tied_focal ? gfx + gfy : gfx;
-      gr[8] = D.tied_focal ? gfx + gfy : gfy;
-      gr[9] = -10.f * gpx / expf(f0 / D.focal_break);
-      gr[10] = -10.f * gpy / expf(f1 / D.focal_break);
-#pragma unroll
-      for (int k = 0; k < 11; ++k) ws.g_img[i * 11 + k] = gr[k];
+      for (int k = 0; k < kImgVals; ++k) S[k] = fix_get(ws.img_acc + i * kImgVals + k, bad);
+      load_row(ws.geomI + int64_t(i) * kGeomI, c);
+      image_grad(D, L, i, S, c, ws.grad);
     }
   }
   fix_report(bad, ws.flags);
@@ -400,29 +405,11 @@ static __device__ __noinline__ void small_param_step(const d3r_align_desc& D, co
   if (D.eval_only) return;
   D3R_TSTAMP(2);
 
-  // phase 2: Adam over the flat parameter vector  [poses 7n | focals 2n | pp 2n | pw 8E | adapt 2E]
+  // phase 2: Adam over the flat parameter vector
   for (int idx = threadIdx.x; idx < L.total; idx += blockDim.x) {
     if (!tr[idx]) continue;
-    float g;
-    if (idx < L.focals) {
-      const int i = idx / 7;
-      g = ws.g_img[i * 11 + (idx - i * 7)];
-    } else if (idx < L.pp) {
-      const int r = idx - L.focals;
-      g = ws.g_img[(r >> 1) * 11 + 7 + (r & 1)];
-    } else if (idx < L.pw) {
-      const int r = idx - L.pp;
-      g = ws.g_img[(r >> 1) * 11 + 9 + (r & 1)];
-    } else if (idx < L.adapt) {
-      const int r = idx - L.pw;
-      g = ws.g_edge[(r >> 3) * 10 + (r & 7)];
-      if ((r & 7) == 7 && D.norm_pw_scale) g -= coupling;
-    } else {
-      const int r = idx - L.adapt;
-      g = ws.g_edge[(r >> 1) * 10 + 8 + (r & 1)];
-    }
     float m = am[idx], v = av[idx];
-    sm[idx] = adam_update(sm[idx], g, m, v, b1, b2, step_size, bc2s, eps);
+    sm[idx] = adam_param(D, L, idx, sm[idx], m, v, ws.grad[idx], coupling, step_size, bc2s);
     am[idx] = m;
     av[idx] = v;
   }
@@ -434,11 +421,10 @@ static __device__ __noinline__ void small_param_step(const d3r_align_desc& D, co
 
 
 // ---- latency-optimised small-parameter step for graphs with one thread per edge / per image (E, n <= blockDim) ----
-// Same mathematics as small_param_step.  The tail of a 60-microsecond iteration is bound by the dependent instruction
-// chain of whichever thread does the most, so the work is cut three ways:
-//   A  one thread per edge / per image: accumulators + the geometry CACHED by the previous refresh (ws.geomE / geomI:
-//      rotation, normalised quaternion, scale, adaptors ... -- nothing is recomputed) -> raw gradients, written to
-//      shared memory in the flat parameter layout;
+// The tail of a 60-microsecond iteration is bound by the dependent instruction chain of whichever thread does the most,
+// so the work is cut three ways:
+//   A  one thread per edge / per image: accumulators + the cached geometry -> raw gradients, written to shared memory
+//      in the flat parameter layout;
 //   B  one thread per PARAMETER: Adam (parameter, moments and flag were requested before stage A, so their latency is
 //      hidden behind it), refreshed value to global and shared memory;
 //   C  one thread per edge / per image again: derived transforms + geometry cache of the refreshed parameters.
@@ -453,7 +439,6 @@ static __device__ __forceinline__ void small_param_step_fast(const d3r_align_des
   float* __restrict__ av = D.small_v;
   const uint8_t* __restrict__ tr = D.small_trainable;
   const float step_size = D.sched[it * 4 + 1], bc2s = D.sched[it * 4 + 2];
-  const float b1 = D.beta1, b2 = D.beta2, eps = D.adam_eps;
   float* g_s = scr;               // [L.total] raw gradients
   float* p_s = scr + L.total;     // [L.total] refreshed parameters
   const int tid = threadIdx.x, nthr = blockDim.x;
@@ -476,91 +461,24 @@ static __device__ __forceinline__ void small_param_step_fast(const d3r_align_des
   if (has_e) {
     const int ei = D.edge_ent[e * 2 + 0], ej = D.edge_ent[e * 2 + 1];
     float c[kGeomE];
-    const float4* c4 = reinterpret_cast<const float4*>(ws.geomE + int64_t(e) * kGeomE);
-#pragma unroll
-    for (int k = 0; k < kGeomE / 4; ++k) { const float4 t = c4[k]; c[4 * k] = t.x; c[4 * k + 1] = t.y; c[4 * k + 2] = t.z; c[4 * k + 3] = t.w; }
+    load_row(ws.geomE + int64_t(e) * kGeomE, c);
     float si[13], sj[13];
 #pragma unroll
     for (int k = 0; k < 13; ++k) { si[k] = fix_get(ws.ent_acc + ei * kEntVals + k, bad); sj[k] = fix_get(ws.ent_acc + ej * kEntVals + k, bad); }
 #pragma unroll
     for (int k = 0; k < kEntVals; ++k) { ws.ent_acc[ei * kEntVals + k] = 0; ws.ent_acc[ej * kEntVals + k] = 0; }   // read: clear for the next launch
     lpart = si[12] + sj[12];
-    const float* R = c; const float* ad = c + 9; const float sc = c[12]; const float* T = c + 13; const float* qh = c + 16;
-    float dM[9], dt[3];
-#pragma unroll
-    for (int k = 0; k < 9; ++k) dM[k] = -(si[k] + sj[k]);
-#pragma unroll
-    for (int a = 0; a < 3; ++a) dt[a] = -(si[9 + a] + sj[9 + a]);
-    float dLds = 0.f, dR[9], dad[3] = {0.f, 0.f, 0.f};
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-#pragma unroll
-      for (int b = 0; b < 3; ++b) {
-        dLds += dM[a * 3 + b] * R[a * 3 + b] * ad[b];
-        dR[a * 3 + b] = dM[a * 3 + b] * sc * ad[b];
-        dad[b] += dM[a * 3 + b] * sc * R[a * 3 + b];
-      }
-      dLds += dt[a] * T[a];
-    }
-    float ge[10];
-    quat_backward(dR, qh, c[20], ge);
-#pragma unroll
-    for (int a = 0; a < 3; ++a) ge[4 + a] = dt[a] * sc * c[21 + a];
-    ge[7] = dLds * sc;             // the mean-coupling term is subtracted in stage B
-    coupl = dLds * sc;
-    float gad[3];
-#pragma unroll
-    for (int b = 0; b < 3; ++b) gad[b] = dad[b] * ad[b] / D.pw_break;
-    if (D.norm_pw_scale) { const float mu = (gad[0] + gad[1] + gad[2]) / 3.f; gad[0] -= mu; gad[1] -= mu; gad[2] -= mu; }
-    ge[8] = gad[0] + gad[1];
-    ge[9] = gad[2];
-#pragma unroll
-    for (int k = 0; k < 8; ++k) g_s[L.pw + e * 8 + k] = ge[k];
-    g_s[L.adapt + e * 2 + 0] = ge[8];
-    g_s[L.adapt + e * 2 + 1] = ge[9];
+    coupl = edge_grad(D, L, e, si, sj, c, g_s);
   }
   if (has_i) {
     float c[kGeomI];
-    const float4* c4 = reinterpret_cast<const float4*>(ws.geomI + int64_t(i) * kGeomI);
+    load_row(ws.geomI + int64_t(i) * kGeomI, c);
+    float S[kImgVals];
 #pragma unroll
-    for (int k = 0; k < kGeomI / 4; ++k) { const float4 t = c4[k]; c[4 * k] = t.x; c[4 * k + 1] = t.y; c[4 * k + 2] = t.z; c[4 * k + 3] = t.w; }
-    float S[12];
-#pragma unroll
-    for (int k = 0; k < 12; ++k) S[k] = fix_get(ws.img_acc + i * kImgVals + k, bad);   // S[a*3+b] = sum G_a c_b ; S[9+a] = sum G_a
+    for (int k = 0; k < kImgVals; ++k) S[k] = fix_get(ws.img_acc + i * kImgVals + k, bad);   // S[a*3+b] = sum G_a c_b ; S[9+a] = sum G_a
 #pragma unroll
     for (int k = 0; k < kImgVals; ++k) ws.img_acc[i * kImgVals + k] = 0;
-    const float* R = c;
-    if (D.stream_kernel) {   // the streaming kernel accumulates sum G (x) Y, Y = R c: sum G (x) c = (sum G (x) Y) R
-      float Sc[9];
-#pragma unroll
-      for (int a = 0; a < 3; ++a)
-#pragma unroll
-        for (int b = 0; b < 3; ++b) Sc[a * 3 + b] = S[a * 3 + 0] * R[0 * 3 + b] + S[a * 3 + 1] * R[1 * 3 + b] + S[a * 3 + 2] * R[2 * 3 + b];
-#pragma unroll
-      for (int k = 0; k < 9; ++k) S[k] = Sc[k];
-    }
-    float gi[11];
-    quat_backward(S, c + 9, c[13], gi);
-#pragma unroll
-    for (int a = 0; a < 3; ++a) gi[4 + a] = S[9 + a] * c[14 + a];
-    float gfx = 0.f, gfy = 0.f, gpx = 0.f, gpy = 0.f;
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-      gfx += R[a * 3 + 0] * S[a * 3 + 0];
-      gfy += R[a * 3 + 1] * S[a * 3 + 1];
-      gpx += R[a * 3 + 0] * S[a * 3 + 2];
-      gpy += R[a * 3 + 1] * S[a * 3 + 2];
-    }
-    gfx = -gfx / D.focal_break;
-    gfy = -gfy / D.focal_break;
-    gi[7] = D.tied_focal ? gfx + gfy : gfx;     // one shared focal: both slots get the summed gradient
-    gi[8] = D.tied_focal ? gfx + gfy : gfy;
-    gi[9] = -10.f * gpx / c[17];
-    gi[10] = -10.f * gpy / c[18];
-#pragma unroll
-    for (int k = 0; k < 7; ++k) g_s[L.poses + i * 7 + k] = gi[k];
-    g_s[L.focals + i * 2 + 0] = gi[7]; g_s[L.focals + i * 2 + 1] = gi[8];
-    g_s[L.pp + i * 2 + 0] = gi[9]; g_s[L.pp + i * 2 + 1] = gi[10];
+    image_grad(D, L, i, S, c, g_s);
   }
   fix_report(bad, ws.flags);
   lpart = warp_sum(lpart);
@@ -582,15 +500,12 @@ static __device__ __forceinline__ void small_param_step_fast(const d3r_align_des
     uint8_t t;
     if (r < 2) { p = pp_[r & 1]; m = pm_[r & 1]; v = pv_[r & 1]; t = pt_[r & 1]; }
     else { p = sm[idx]; m = am[idx]; v = av[idx]; t = tr[idx]; }
-    const bool is_sigma = idx >= L.pw && idx < L.adapt && ((idx - L.pw) & 7) == 7;
     if (t) {
-      float g = g_s[idx];
-      if (is_sigma && D.norm_pw_scale) g -= coupling;
-      p = adam_update(p, g, m, v, b1, b2, step_size, bc2s, eps);
+      p = adam_param(D, L, idx, p, m, v, g_s[idx], coupling, step_size, bc2s);
       sm[idx] = p; am[idx] = m; av[idx] = v;
     }
     p_s[idx] = p;
-    if (is_sigma) snew += p;
+    if (is_log_scale(L, idx)) snew += p;
   }
   snew = warp_sum(snew);
   if ((tid & 31) == 0) s_red[16 + (tid >> 5)] = snew;
@@ -608,23 +523,7 @@ static __device__ __forceinline__ void small_param_step_fast(const d3r_align_des
     float p8[8];
 #pragma unroll
     for (int k = 0; k < 8; ++k) p8[k] = p_s[L.pw + e * 8 + k];
-    EdgeGeom g;
-    edge_geom(p8, p_s[L.adapt + e * 2 + 0], p_s[L.adapt + e * 2 + 1], D, mean_sigma, log_base, g);
-    float o[kEdgeT];
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-#pragma unroll
-      for (int b = 0; b < 3; ++b) o[a * 3 + b] = g.s * g.R[a * 3 + b] * g.ad[b];
-#pragma unroll
-    for (int a = 0; a < 3; ++a) o[9 + a] = g.s * g.T[a];
-#pragma unroll
-    for (int k = 0; k < kEdgeT; ++k) ws.edgeT[e * kEdgeT + k] = o[k];
-    if (D.stream_kernel) {
-      const int ei = D.edge_ent[e * 2 + 0], ej = D.edge_ent[e * 2 + 1];
-#pragma unroll
-      for (int k = 0; k < kEdgeT; ++k) { ws.entT[int64_t(ei) * kEdgeT + k] = -o[k]; ws.entT[int64_t(ej) * kEdgeT + k] = -o[k]; }
-    }
-    store_geom_edge(ws.geomE + int64_t(e) * kGeomE, g, p8);
+    edge_refresh(D, ws, e, p8, p_s[L.adapt + e * 2 + 0], p_s[L.adapt + e * 2 + 1], mean_sigma, log_base);
   }
   if (has_i) {
     float q7[7];
@@ -673,6 +572,30 @@ static __device__ __forceinline__ void small_step(const d3r_align_desc& D, const
     small_param_step_fast(D, it, s_red, scr);
   else
     small_param_step(D, ws, it, s_red);
+}
+
+// Launches iterations [it_begin, it_end) of an iteration kernel, `grid` CTAs of `threads` each.  Every launch allows
+// programmatic stream serialisation, so that its CTAs run their launch-independent prologue while the previous iteration's
+// last CTA is still in its small-parameter step; the kernels call pdl::sync_with_predecessor() before they read what that
+// step wrote.  The shared-memory opt-in is a per-device function attribute (a process may drive several GPUs), so it is
+// set on every call; two CTAs per SM need the maximum carve-out.
+static int launch_iterations(void (*kernel)(d3r_align_desc, int), const d3r_align_desc* desc, int grid, int threads, size_t smem,
+                             int it_begin, int it_end, cudaStream_t st) {
+  D3R_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  D3R_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3((unsigned)grid);
+  cfg.blockDim = dim3((unsigned)threads);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = st;
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  for (int it = it_begin; it < it_end; ++it) D3R_CUDA(cudaLaunchKernelEx(&cfg, kernel, *desc, it));
+  D3R_LAUNCH_CHECK();
+  return D3R_OK;
 }
 
 }  // namespace align

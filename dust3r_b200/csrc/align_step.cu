@@ -37,29 +37,7 @@ __global__ void __launch_bounds__(kThreads) prepare_kernel(const __grid_constant
 constexpr int kStages = 3;
 constexpr int kEntTile = 16;               // entries whose per-warp partial sums are staged in smem at a time
 constexpr int kRedVals = 16;               // 13 padded to 16 for the halving butterfly
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
+using ptx::smem_u32;
 
 // Sum 16 per-lane values across the warp with 16 shuffles (instead of 16 x 5): at every halving step a lane
 // keeps one half of its values and trades the other half with its partner.  On return lane l holds the
@@ -132,10 +110,10 @@ align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
 
   if (tid == 0) {
     for (int s = 0; s < kStages; ++s) {
-      mbar_init(smem_u32(&s_full[s]), 1);
-      mbar_init(smem_u32(&s_empty[s]), kWarps);
+      ptx::mbar_init(smem_u32(&s_full[s]), 1);
+      ptx::mbar_init(smem_u32(&s_empty[s]), kWarps);
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    ptx::fence_barrier_init();
   }
   // slots past the chunk are never written by the bulk copies: zero them once (weight 0 -> no contribution)
   for (int s = 0; s < kStages; ++s)
@@ -145,9 +123,9 @@ align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
   const uint32_t stage_bytes = uint32_t(npx) * 16u;
   auto produce = [&](int k) {   // called by one thread
     const int s = k % kStages;
-    mbar_wait(smem_u32(&s_empty[s]), ((k / kStages) & 1) ^ 1);
-    mbar_expect_tx(smem_u32(&s_full[s]), stage_bytes);
-    bulk_g2s(smem_u32(s_obs + s * kSlots), obs_base + D.ent_obs_off[e0 + k] + pbase, stage_bytes, smem_u32(&s_full[s]));
+    ptx::mbar_wait(smem_u32(&s_empty[s]), ((k / kStages) & 1) ^ 1);
+    ptx::mbar_arrive_expect_tx(smem_u32(&s_full[s]), stage_bytes);
+    ptx::bulk_g2s(smem_u32(s_obs + s * kSlots), obs_base + D.ent_obs_off[e0 + k] + pbase, stage_bytes, smem_u32(&s_full[s]));
   };
   if (tid == 0)
     for (int k = 0; k < min(kStages, deg); ++k) produce(k);
@@ -155,11 +133,10 @@ align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
   // Programmatic dependent launch: everything above touches only per-problem constants (index tables, the
   // observation slabs) -- this iteration's CTAs were allowed to start it while the previous iteration's last CTA
   // was still in its small-parameter step.  Everything below reads what that step (and the previous depth update)
-  // wrote, so wait here for the previous grid to complete and flush.
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  // ... and allow the NEXT iteration's CTAs to be scheduled as soon as every CTA of this grid has got this far: they
-  // take the slots of this grid's last wave as its CTAs retire, and block at their own griddepcontrol.wait
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  // wrote, so wait here for the previous grid to complete and flush, and allow the NEXT iteration's CTAs to be
+  // scheduled as soon as every CTA of this grid has got this far: they take the slots of this grid's last wave as its
+  // CTAs retire, and block at their own wait.
+  pdl::sync_with_predecessor();
   const float* iT = ws.imgT + img * kImgT;
   float R[9], T[3];
 #pragma unroll
@@ -204,7 +181,7 @@ align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
       const float M[9] = {t0.x, t0.y, t0.z, t0.w, t1.x, t1.y, t1.z, t1.w, t2.x};
       const float t[3] = {t2.y, t2.z, t2.w};
       const int s = stage;
-      mbar_wait(smem_u32(&s_full[s]), stage_phase);
+      ptx::mbar_wait(smem_u32(&s_full[s]), stage_phase);
       if (++stage == kStages) { stage = 0; stage_phase ^= 1; }
       const float4* so = s_obs + s * kSlots;
       float acc[kRedVals];
@@ -239,7 +216,7 @@ align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
       }
       // this warp is done with the stage: hand it back, and (thread 0) refill it with entry kk + kStages
       __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&s_empty[s]));
+      if (lane == 0) ptx::mbar_arrive(smem_u32(&s_empty[s]));
       if (tid == 0 && kk + kStages < deg) produce(kk + kStages);
       const float tot = butterfly16(acc, lane);
       const int vi = (lane >> 1) & 15;
@@ -336,12 +313,6 @@ __global__ void __launch_bounds__(kThreads) pts3d_kernel(const __grid_constant__
   }
 }
 
-__global__ void pack_obs_kernel(const float* __restrict__ pts, const float* __restrict__ w, float4* __restrict__ obs,
-                                int64_t n) {
-  int64_t i = int64_t(blockIdx.x) * blockDim.x + threadIdx.x;
-  if (i < n) obs[i] = make_float4(pts[i * 3 + 0], pts[i * 3 + 1], pts[i * 3 + 2], w[i]);
-}
-
 }  // namespace align
 }  // namespace d3r
 
@@ -362,10 +333,7 @@ extern "C" int d3r_align_set_debug(void* dev_buf) {
 extern "C" int d3r_align_chunk_pixels(void) { return kChunk; }
 extern "C" int d3r_sizeof_align_desc(void) { return (int)sizeof(d3r_align_desc); }
 
-extern "C" int64_t d3r_align_workspace_floats(int32_t n_imgs, int32_t n_edges, int32_t n_chunks, int32_t max_chunks) {
-  (void)n_chunks; (void)max_chunks;   // kept in the signature for ABI stability; accumulators are per entry now
-  return workspace_floats(n_imgs, n_edges);
-}
+extern "C" int64_t d3r_align_workspace_floats(int32_t n_imgs, int32_t n_edges) { return workspace_floats(n_imgs, n_edges); }
 
 static int validate(const d3r_align_desc* d) {
   D3R_CHECK_ARG(d != nullptr, "d3r_align: null descriptor");
@@ -389,24 +357,7 @@ extern "C" int d3r_align_prepare(const d3r_align_desc* desc, void* stream) {
 template <bool kL2, int PPT>
 static int launch_iters(const d3r_align_desc* desc, int it_begin, int it_end, cudaStream_t st) {
   const size_t smem = size_t(kStages) * PPT * kThreads * sizeof(float4) + size_t(kEntTile) * kWarps * kEntVals * sizeof(float);
-  // function attributes are per device / context: set them on every launch batch (cheap) so that a process driving
-  // several GPUs gets the opt-in on each of them
-  D3R_CUDA(cudaFuncSetAttribute(align_iter_kernel<kL2, PPT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  // two CTAs per SM need the maximum shared-memory carve-out
-  D3R_CUDA(cudaFuncSetAttribute(align_iter_kernel<kL2, PPT>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)desc->n_chunks);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;   // overlap a launch's prologue with its predecessor's tail
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  for (int it = it_begin; it < it_end; ++it) D3R_CUDA(cudaLaunchKernelEx(&cfg, align_iter_kernel<kL2, PPT>, *desc, it));
-  D3R_LAUNCH_CHECK();
-  return D3R_OK;
+  return launch_iterations(align_iter_kernel<kL2, PPT>, desc, desc->n_chunks, kThreads, smem, it_begin, it_end, st);
 }
 
 template <bool kL2>
@@ -448,18 +399,6 @@ extern "C" int d3r_align_pts3d(const d3r_align_desc* desc, float* out_dev, void*
   if (rc) return rc;
   D3R_CHECK_ARG(out_dev != nullptr, "d3r_align_pts3d: null output");
   pts3d_kernel<<<desc->n_chunks, kThreads, 0, (cudaStream_t)stream>>>(*desc, out_dev);
-  D3R_LAUNCH_CHECK();
-  return D3R_OK;
-}
-
-extern "C" int d3r_align_pack_obs(const float* pts_dev, const float* weight_dev, void* obs_dev, int64_t obs_off,
-                                  int64_t n_pix, void* stream) {
-  D3R_CHECK_ARG(pts_dev && weight_dev && obs_dev && n_pix >= 0, "d3r_align_pack_obs: bad arguments");
-  if (n_pix == 0) return D3R_OK;
-  const int threads = 256;
-  const int64_t blocks = (n_pix + threads - 1) / threads;
-  pack_obs_kernel<<<(unsigned)blocks, threads, 0, (cudaStream_t)stream>>>(pts_dev, weight_dev,
-                                                                        reinterpret_cast<float4*>(obs_dev) + obs_off, n_pix);
   D3R_LAUNCH_CHECK();
   return D3R_OK;
 }

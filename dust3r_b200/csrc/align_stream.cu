@@ -17,7 +17,7 @@
 //     pixel pairs (two independent dependency chains per thread);
 //   * the 13 per-entry sums are reduced across the warp through a transpose in the just-drained stage buffer
 //     (13 STS + 4 LDS.128 + 16 FADD instead of a 16-shuffle butterfly), accumulated per warp in shared memory over
-//     all of the warp's items of an image, and leave the SM once per (warp, image) as 2^44 fixed-point integer
+//     all of the warp's items of an image, and leave the SM once per (warp, image) as 2^40 fixed-point integer
 //     atomics (order independent -> bit-reproducible), exactly like the general kernel;
 //   * sqrt / reciprocal / exp of the per-pixel Adam update and unprojection use the MUFU approximations (<= 2 ulp).
 //
@@ -60,43 +60,7 @@ __device__ __forceinline__ float rsqrt_approx(float x) { float y; asm("rsqrt.app
 __device__ __forceinline__ float sqrt_approx(float x) { float y; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
-__device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void sb_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void sb_expect_tx(uint32_t bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void sb_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  uint32_t spins = 0;
-  do {
-    asm volatile(
-        "{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}\n"
-        : "=r"(done) : "r"(bar), "r"(parity) : "memory");
-    // a stage that never lands is a bug (byte count mismatch): fail the launch instead of hanging the GPU
-    if (!done && ++spins > (1u << 22)) __trap();
-  } while (!done);
-}
-__device__ __forceinline__ void sb_bulk(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
-}
-
-// Streamed data (observations, log-depths, Adam moments) is loaded with the L2 evict_first policy: it is dead after one use
-// within an iteration, and at default priority 200+ MB of it per iteration push everything else out of the 126 MB L2 --
-// including the instructions and inputs of the small-parameter step, which one CTA then re-fetches from DRAM on the critical
-// path.  Among themselves evict_first lines still age in order, so the reversed traversal of odd iterations keeps finding the
-// tail of the previous pass.
-__device__ __forceinline__ uint64_t policy_evict_first() {
-  uint64_t pol;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-  return pol;
-}
-__device__ __forceinline__ void sb_bulk_stream(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t pol) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
-               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(pol) : "memory");
-}
+using ptx::smem_u32;
 
 struct ProdState {          // per warp, touched by lane 0 only
   int item, item_end;
@@ -129,6 +93,11 @@ __device__ __forceinline__ float warp_transpose_sum(const float (&a)[NV], float*
 }
 
 // Issues the next stage of this warp's sequence into its ring slot (lane 0 only).
+// Streamed data (observations, log-depths, Adam moments) is loaded with the L2 evict_first policy: it is dead after one use
+// within an iteration, and at default priority 200+ MB of it per iteration push everything else out of the 126 MB L2 --
+// including the instructions and inputs of the small-parameter step, which one CTA then re-fetches from DRAM on the critical
+// path.  Among themselves evict_first lines still age in order, so the reversed traversal of odd iterations keeps finding the
+// tail of the previous pass.
 template <int PPT, int NST>
 __device__ __forceinline__ void produce_next(const d3r_align_desc& D, const Workspace& ws, const d3r_align_item* item_tab,
                                              ProdState* ps, uint8_t* ring, uint64_t* full) {
@@ -136,20 +105,20 @@ __device__ __forceinline__ void produce_next(const d3r_align_desc& D, const Work
   const int item = ps->item;
   if (item >= ps->item_end) return;
   const int s = ps->slot;
-  const uint32_t dst = s_u32(ring + s * kStage);
-  const uint32_t bar = s_u32(&full[s]);
+  const uint32_t dst = smem_u32(ring + s * kStage);
+  const uint32_t bar = smem_u32(&full[s]);
   const int phase = ps->phase;
-  const uint64_t pol = policy_evict_first();
+  const uint64_t pol = ptx::policy_evict_first();
   ps->slot = (s + 1 == NST) ? 0 : s + 1;
   if (phase == 0) {                                  // L: header | image row | log-depth slice
     const d3r_align_item* gh = item_tab + item;
     const d3r_align_item h = *gh;
     const uint32_t px_bytes = uint32_t(h.npx) * 4u;
     const float* irow = ws.imgT + int64_t(h.img) * kImgT;
-    sb_expect_tx(bar, 64u + 64u + px_bytes);
-    sb_bulk(dst, gh, 64u, bar);
-    sb_bulk(dst + 64u, irow, 64u, bar);
-    sb_bulk_stream(dst + kHdrBytes, D.logd + h.pix0, px_bytes, bar, pol);
+    ptx::mbar_arrive_expect_tx(bar, 64u + 64u + px_bytes);
+    ptx::bulk_g2s(dst, gh, 64u, bar);
+    ptx::bulk_g2s(dst + 64u, irow, 64u, bar);
+    ptx::bulk_g2s_hint(dst + kHdrBytes, D.logd + h.pix0, px_bytes, bar, pol);
     ps->deg = h.deg; ps->px_bytes = px_bytes; ps->pay_bytes = uint32_t(h.nslots) * kSlotBytes; ps->slab_units = h.slab_units;
     ps->row = ws.entT + int64_t(h.e0) * kEdgeT;
     ps->obs = reinterpret_cast<const uint4*>(D.obs) + h.obs0;
@@ -159,20 +128,20 @@ __device__ __forceinline__ void produce_next(const d3r_align_desc& D, const Work
     const float* row = ps->row;
     const uint4* obs = ps->obs;
     const uint32_t pay = ps->pay_bytes;
-    sb_expect_tx(bar, 48u + pay);
-    sb_bulk(dst, row, 48u, bar);
-    sb_bulk_stream(dst + kHdrBytes, obs, pay, bar, pol);
+    ptx::mbar_arrive_expect_tx(bar, 48u + pay);
+    ptx::bulk_g2s(dst, row, 48u, bar);
+    ptx::bulk_g2s_hint(dst + kHdrBytes, obs, pay, bar, pol);
     ps->row = row + kEdgeT;
     ps->obs = obs + ps->slab_units;
     ps->phase = phase + 1;
   } else {                                           // MV: image row | log-depth | exp_avg | exp_avg_sq
     const uint32_t px_bytes = ps->px_bytes;
     const int64_t pix0 = ps->pix0;
-    sb_expect_tx(bar, 64u + 3u * px_bytes);
-    sb_bulk(dst, ps->irow, 64u, bar);
-    sb_bulk_stream(dst + kHdrBytes, D.logd + pix0, px_bytes, bar, pol);
-    sb_bulk_stream(dst + kHdrBytes + PPT * 256, D.logd_m + pix0, px_bytes, bar, pol);
-    sb_bulk_stream(dst + kHdrBytes + 2 * PPT * 256, D.logd_v + pix0, px_bytes, bar, pol);
+    ptx::mbar_arrive_expect_tx(bar, 64u + 3u * px_bytes);
+    ptx::bulk_g2s(dst, ps->irow, 64u, bar);
+    ptx::bulk_g2s_hint(dst + kHdrBytes, D.logd + pix0, px_bytes, bar, pol);
+    ptx::bulk_g2s_hint(dst + kHdrBytes + PPT * 256, D.logd_m + pix0, px_bytes, bar, pol);
+    ptx::bulk_g2s_hint(dst + kHdrBytes + 2 * PPT * 256, D.logd_v + pix0, px_bytes, bar, pol);
     ps->item = item + 1;
     ps->phase = 0;
   }
@@ -329,16 +298,15 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
   unsigned long long* dbg = g_align_dbg ? g_align_dbg + 4 * size_t(gw) : nullptr;   // per-warp timeline (debug aid)
   if (dbg && lane == 0) dbg[0] = gtime();
   if (lane == 0) {
-    for (int s = 0; s < NST; ++s) sb_init(s_u32(&full[s]), 1);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    for (int s = 0; s < NST; ++s) ptx::mbar_init(smem_u32(&full[s]), 1);
+    ptx::fence_barrier_init();
     ps->item = ib; ps->item_end = ie; ps->phase = 0; ps->slot = 0;
   }
   for (int i = lane; i < Wn * kEntVals + 16; i += 32) s_acc[i] = 0.f;
   __syncwarp();
 
   // everything below reads what the previous iteration wrote (transforms, log-depths, Adam moments)
-  asm volatile("griddepcontrol.wait;" ::: "memory");
-  asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
+  pdl::sync_with_predecessor();
   if (dbg && lane == 0) dbg[1] = gtime();
   if (lane == 0)
     for (int s = 0; s < NST; ++s) produce_next<PPT, NST>(D, ws, item_tab, ps, ring, full);
@@ -377,7 +345,7 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
   for (int item = ib; item < ie; ++item) {
     // ------------------------------------------------------------------ L stage: unproject this item's pixels
     uint8_t* slot = ring + si * kStage;
-    sb_wait(s_u32(&full[si]), par);
+    ptx::mbar_wait_bounded(smem_u32(&full[si]), par);
     const d3r_align_item* h = reinterpret_cast<const d3r_align_item*>(slot);
     const int img = h->img, nslots = h->nslots, npx = h->npx, e0 = h->e0, deg = h->deg;
     const int64_t pix0 = h->pix0;
@@ -404,7 +372,7 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
         acc_e0 = e0 + k; acc_cnt = min(Wn, deg - k); kin = 0;
       }
       slot = ring + si * kStage;
-      sb_wait(s_u32(&full[si]), par);
+      ptx::mbar_wait_bounded(smem_u32(&full[si]), par);
       float a13[kEntVals];
       if (nslots == 3) entry_slots<kL2, 3, PPT>(slot, lane, X, G, a13);
       else if (nslots == 2) entry_slots<kL2, 2, PPT>(slot, lane, X, G, a13);
@@ -412,7 +380,7 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
       __syncwarp();                               // every lane is done reading the observations of this stage
       const float tot = warp_transpose_sum<kEntVals>(a13, reinterpret_cast<float*>(slot + kHdrBytes), lane);
       if (!(lane & 1) && lane < 2 * kEntVals) s_acc[kin * kEntVals + (lane >> 1)] += tot;
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      ptx::fence_proxy_async();
       __syncwarp();
       if (lane == 0) produce_next<PPT, NST>(D, ws, item_tab, ps, ring, full);
       advance();
@@ -420,7 +388,7 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
 
     // ------------------------------------------------------------------ MV stage: depth gradient + Adam in place
     slot = ring + si * kStage;
-    sb_wait(s_u32(&full[si]), par);
+    ptx::mbar_wait_bounded(smem_u32(&full[si]), par);
     if (train) {
       float s12[kImgVals];
       if (nslots == 3) adam_slots<3, PPT>(D, slot, lane, npx, pix0, step_size, inv_bc2s, X, G, s12);
@@ -429,7 +397,7 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
       __syncwarp();
       const float tot = warp_transpose_sum<kImgVals>(s12, reinterpret_cast<float*>(slot + kHdrBytes), lane);
       if (!(lane & 1) && lane < 2 * kImgVals) s_img[lane >> 1] += tot;
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      ptx::fence_proxy_async();
     }
     __syncwarp();
     if (lane == 0) produce_next<PPT, NST>(D, ws, item_tab, ps, ring, full);
@@ -494,29 +462,6 @@ __global__ void __launch_bounds__(256) pack_entries_kernel(const d3r_pack_entry*
 
 // world points for the streaming layout's owners are produced by the general pts3d kernel (layout independent)
 
-template <bool kL2, int PPT, int NST>
-static int launch_stream_t(const d3r_align_desc* desc, int it_begin, int it_end, cudaStream_t st) {
-  constexpr int kStage = kHdrBytes + PPT * kSlotBytes;
-  const int acc_floats = (desc->stream_window * kEntVals + 16 + 31) & ~31;
-  const size_t smem = size_t(kSWarps) * (size_t(NST) * kStage + size_t(acc_floats) * 4);
-  // per device: the opt-in is a per-context function attribute (a process may drive several GPUs)
-  D3R_CUDA(cudaFuncSetAttribute(align_stream_kernel<kL2, PPT, NST>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  D3R_CUDA(cudaFuncSetAttribute(align_stream_kernel<kL2, PPT, NST>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3((unsigned)desc->stream_grid);
-  cfg.blockDim = dim3(kSThreads);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
-  cfg.numAttrs = 1;
-  for (int it = it_begin; it < it_end; ++it) D3R_CUDA(cudaLaunchKernelEx(&cfg, align_stream_kernel<kL2, PPT, NST>, *desc, it));
-  D3R_LAUNCH_CHECK();
-  return D3R_OK;
-}
-
 int stream_set_debug(unsigned long long* p) {   // this translation unit's copy of the timeline pointer
   D3R_CUDA(cudaMemcpyToSymbol(g_align_dbg, &p, sizeof(p)));
   return D3R_OK;
@@ -537,8 +482,10 @@ int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, cudaStre
   const bool deep = stream_smem_bytes(3, 4, desc->stream_window) <= budget;
   D3R_CHECK_ARG(deep || stream_smem_bytes(3, 3, desc->stream_window) <= budget, "d3r_align_run: stream_window=%d does not fit shared memory",
                 desc->stream_window);
-  if (desc->dist_l2) return deep ? launch_stream_t<true, 3, 4>(desc, it_begin, it_end, st) : launch_stream_t<true, 3, 3>(desc, it_begin, it_end, st);
-  return deep ? launch_stream_t<false, 3, 4>(desc, it_begin, it_end, st) : launch_stream_t<false, 3, 3>(desc, it_begin, it_end, st);
+  void (*kernel)(d3r_align_desc, int) = desc->dist_l2 ? (deep ? align_stream_kernel<true, 3, 4> : align_stream_kernel<true, 3, 3>)
+                                                      : (deep ? align_stream_kernel<false, 3, 4> : align_stream_kernel<false, 3, 3>);
+  return launch_iterations(kernel, desc, desc->stream_grid, kSThreads, stream_smem_bytes(3, deep ? 4 : 3, desc->stream_window),
+                           it_begin, it_end, st);
 }
 
 }  // namespace align

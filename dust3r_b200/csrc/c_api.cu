@@ -28,7 +28,7 @@ int num_sms() {
 
 extern "C" const char* d3r_last_error(void) { return d3r::g_err; }
 
-extern "C" int d3r_abi_version(void) { return 3; }
+extern "C" int d3r_abi_version(void) { return 4; }
 
 extern "C" int d3r_check_device(void) {
   int dev = 0;

@@ -6,7 +6,7 @@
 // predecessor finishes.  A kernel launched without the attribute sees both instructions as no-ops.
 // Measured on the 567-launch forward step: no gain (75.5 ms without vs 76.2 ms with, power-capped box) -- the step is
 // not launch-gap bound -- so the attribute is OFF by default and D3R_PDL=1 in the environment enables it.  (The
-// alignment loop, whose ~10 us serial tail per 77 us iteration does benefit, always uses PDL: align_step.cu.)
+// alignment loop, whose ~10 us serial tail per 77 us iteration does benefit, always uses PDL: launch_iterations in align_common.cuh.)
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdlib>

@@ -1,5 +1,6 @@
 // Thin inline-PTX wrappers for the Hopper (sm_90a) primitives used by the dust3r_b200 kernels:
-// mbarrier, TMA (cp.async.bulk.tensor, with cluster multicast), clusters, wgmma (fence / mma / commit / wait).
+// mbarrier, bulk copies (cp.async.bulk), TMA (cp.async.bulk.tensor, with cluster multicast), clusters, wgmma (fence / mma /
+// commit / wait).
 // Descriptor bit layouts follow the PTX ISA "wgmma matrix descriptor" table.
 #pragma once
 #include <cuda.h>
@@ -55,6 +56,33 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
+}
+// a phase that never completes is a bug (byte count mismatch): fail the launch instead of hanging the GPU
+__device__ __forceinline__ void mbar_wait_bounded(uint32_t bar, uint32_t parity) {
+  uint32_t spins = 0;
+  bool done;
+  do {
+    done = mbar_try_wait(bar, parity);
+    if (!done && ++spins > (1u << 22)) __trap();
+  } while (!done);
+}
+
+// ---- bulk copies (1-D TMA) ------------------------------------------------------------------------
+// `bytes` (a multiple of 16) from global to shared memory; completion is signalled on the mbarrier `bar` as tx bytes
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+// L2 policy for data read once: its lines are the first to be evicted
+__device__ __forceinline__ uint64_t policy_evict_first() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+// bulk_g2s with an L2 cache policy from createpolicy
+__device__ __forceinline__ void bulk_g2s_hint(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint64_t pol) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "l"(pol) : "memory");
 }
 
 // ---- TMA ----------------------------------------------------------------------------------------

@@ -120,7 +120,7 @@ typedef struct d3r_align_desc {
   /* ---- streaming kernel (csrc/align_stream.cu), used when every image has P % 4 == 0 and a pixel stride
    * that is a multiple of 4 (always true for DUSt3R inputs: H, W are multiples of the 16-pixel patch).
    * stream_kernel = 1 selects it; obs then holds the slot-interleaved layout written by
-   * d3r_align_pack_obs_stream (same 16 bytes per observation):
+   * d3r_align_pack_entries with stream_layout = 1 (same 16 bytes per observation):
    *   per entry: slots of 64 pixels = [32 x (xA,xB,yA,yB)] [32 x (zA,zB,wA,wB)] for the 32 pixel pairs
    *   (A,B) = (2j, 2j+1) of the slot, the loss coefficient folded into w; every image's slab is padded to
    *   whole slots with w = 0.
@@ -128,7 +128,7 @@ typedef struct d3r_align_desc {
    * [warp_item_ptr[w], warp_item_ptr[w+1]).                                                           */
   int32_t stream_kernel;
   int32_t stream_grid;          /* CTAs of the persistent grid                                       */
-  int32_t stream_ppt;           /* slots (64 pixels) per work item, 2..4                              */
+  int32_t stream_ppt;           /* slots (64 pixels) per work item, 3                                 */
   int32_t stream_window;        /* entries whose partial sums a warp keeps in shared memory            */
   int32_t n_items;
   int32_t reserved0;
@@ -160,7 +160,7 @@ int d3r_sizeof_align_item(void);
 /* Maximum pixels one CTA of the alignment kernel can take (compile-time constant of the library). */
 int d3r_align_chunk_pixels(void);
 /* Number of floats of `workspace` needed for a problem of this size. */
-int64_t d3r_align_workspace_floats(int32_t n_imgs, int32_t n_edges, int32_t n_chunks, int32_t max_chunks);
+int64_t d3r_align_workspace_floats(int32_t n_imgs, int32_t n_edges);
 /* Computes the transforms used by the first iteration from `small` (call once after the
  * parameters are (re)initialised or modified from the host). */
 int d3r_align_prepare(const d3r_align_desc* desc, void* stream);
@@ -176,9 +176,6 @@ int d3r_align_pts3d(const d3r_align_desc* desc, float* out_dev, void* stream);
 /* Debug aid: when dev_buf != NULL every CTA of the next alignment launches writes 4 uint64 %globaltimer stamps
  * (start, end of pixel phase, end/exit, end of small-parameter step) at dev_buf[4*cta]. */
 int d3r_align_set_debug(void* dev_buf);
-/* Packs pred (P,3) + weight (P) rows into the float4 observation layout. */
-int d3r_align_pack_obs(const float* pts_dev, const float* weight_dev, void* obs_dev, int64_t obs_off,
-                       int64_t n_pix, void* stream);
 
 /* Packs EVERY entry's observations in one launch, straight from the (device-resident) output of the forward:
  * replaces the ParameterStack copies + conf_trf of optimizer.py:50-57 / base_opt.py:72-75.  `table` (dev) has one

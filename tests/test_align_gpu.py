@@ -218,13 +218,14 @@ def test_config5_graph_50_views_1225_pairs_modular_matches_oracle(cuda_device):
     prob = AlignProblem.from_output(out, variant='per_edge')
     P0 = init_params(prob, seed=3)
     losses_ref, fin = align_oracle(prob, P0, niter=3)
-    net = _make('ModularPointCloudOptimizer', out, P0, cuda_device)
-    assert net.n_edges == 1225 and net._get_engine().kernel == 'stream'
-    net.compute_global_alignment(init=None, niter=3)
-    assert np.allclose(net.last_losses.cpu().numpy(), losses_ref, rtol=1e-5)
-    depth, poses, focals, pw = _final(net, 'ModularPointCloudOptimizer')
-    assert max(float((a - b).abs().max()) for a, b in zip(depth, fin['im_depthmaps'])) < 1e-4
-    assert float((poses - fin['im_poses']).abs().max()) < 1e-4 and float((pw - fin['pw_poses']).abs().max()) < 1e-4
+    for kernel in KERNELS:
+        net = _make('ModularPointCloudOptimizer', out, P0, cuda_device, kernel=kernel)
+        assert net.n_edges == 1225 and net._get_engine().kernel == kernel
+        net.compute_global_alignment(init=None, niter=3)
+        assert np.allclose(net.last_losses.cpu().numpy(), losses_ref, rtol=1e-5), kernel
+        depth, poses, focals, pw = _final(net, 'ModularPointCloudOptimizer')
+        assert max(float((a - b).abs().max()) for a, b in zip(depth, fin['im_depthmaps'])) < 1e-4, kernel
+        assert float((poses - fin['im_poses']).abs().max()) < 1e-4 and float((pw - fin['pw_poses']).abs().max()) < 1e-4, kernel
 
 
 def test_stream_kernel_entry_window_spill(cuda_device):
