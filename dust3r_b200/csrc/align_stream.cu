@@ -56,9 +56,6 @@ __device__ __forceinline__ f2 mul2(f2 a, f2 b) {
   unpack2(a, a0, a1); unpack2(b, b0, b1);
   return pack2(__fmul_rn(a0, b0), __fmul_rn(a1, b1));
 }
-__device__ __forceinline__ float rsqrt_approx(float x) { float y; asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float sqrt_approx(float x) { float y; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
-__device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
 using ptx::smem_u32;
 
@@ -209,7 +206,7 @@ __device__ __forceinline__ void entry_slots(const uint8_t* slot, int lane, const
       // torch's norm backward yields 0 at ||r|| == 0: r == 0 there, so a finite 1/||r|| stand-in gives g = 0
       float ra, rb;
       unpack2(rho2, ra, rb);
-      const f2 inv = pack2(rsqrt_approx(fmaxf(ra, 1e-36f)), rsqrt_approx(fmaxf(rb, 1e-36f)));
+      const f2 inv = pack2(ptx::rsqrt_approx(fmaxf(ra, 1e-36f)), ptx::rsqrt_approx(fmaxf(rb, 1e-36f)));
       acc[12] = fma2(w, mul2(rho2, inv), acc[12]);
       gs = mul2(w, inv);
     }
@@ -253,10 +250,10 @@ __device__ __forceinline__ void adam_slots(const d3r_align_desc& D, const uint8_
       const f2 v_new = fma2(mul2(bc2(1.f - D.beta2), gd), gd, mul2(pack2(vv.x, vv.y), bc2(D.beta2)));
       float va, vb;
       unpack2(v_new, va, vb);
-      const f2 denom = fma2(pack2(sqrt_approx(va), sqrt_approx(vb)), bc2(inv_bc2s), bc2(D.adam_eps));
+      const f2 denom = fma2(pack2(ptx::sqrt_approx(va), ptx::sqrt_approx(vb)), bc2(inv_bc2s), bc2(D.adam_eps));
       float da, db;
       unpack2(denom, da, db);
-      const f2 upd = mul2(m_new, pack2(rcp_approx(da), rcp_approx(db)));
+      const f2 upd = mul2(m_new, pack2(ptx::rcp_approx(da), ptx::rcp_approx(db)));
       const f2 ld_new = fma2(bc2(-step_size), upd, pack2(ld.x, ld.y));
       reinterpret_cast<f2*>(D.logd + pix0)[j] = ld_new;
       reinterpret_cast<f2*>(D.logd_m + pix0)[j] = m_new;

@@ -1,6 +1,8 @@
-// wgmma fused attention for head dim 64 (sm_90a).
+// wgmma fused attention for head dim 64 (sm_90a): the kernel, its host entry and the C ABI.
 //
 //   O = softmax(Q K^T * scale) V      per (image b, head h), bf16 in/out, fp32 softmax + accumulation
+//   O[b, i, h*64 + d] = softmax_j(scale * q[b,i,h,:] . k[b,j,h,:]) v[b,j,h,d]   replaces the materialised (B,H,N,N) fp32
+//   attention matrix of croco/models/blocks.py:105-109 / :161-165.
 //
 // Flash-attention dataflow on Hopper: a 128-query tile per CTA iteration, 128-key blocks, S and O in registers.
 // CTAs are PERSISTENT (1 per SM, 384 threads): each loops over (query tile, head, image) work items, so barrier set-up
@@ -15,20 +17,17 @@
 //   P_SMEM = false (default)  P stays in registers: the S accumulator fragment, packed to bf16, is exactly the A
 //                             fragment of the next wgmma
 //   P_SMEM = true             P goes through 128B-swizzled shared memory (both wgmma operands from shared memory);
-//                             kept as the A/B reference of the register path
+//                             kept as the A/B reference of the register path, selected by d3r_set_attention_impl(2)
 #include "d3r_common.cuh"
 #include "sm90_ptx.cuh"
 #include "elementwise.h"
 #include "prof.h"
-#include "attention_common.cuh"
 #include "pdl.cuh"
 
 namespace d3r {
 namespace attn {
 
 namespace wg {
-
-using namespace tcc;
 
 constexpr int BQ = 128, BK = 128, D = 64;
 constexpr int kThreads = 384;
@@ -165,7 +164,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
           mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
           const float m_new = fmaxf(m_run[hh], mx);   // finite: every block has at least one valid key
-          const float corr = fast_exp2((m_run[hh] - m_new) * scale_log2);
+          const float corr = ptx::ex2_approx((m_run[hh] - m_new) * scale_log2);
           m_run[hh] = m_new;
           l_run[hh] *= corr;
 #pragma unroll
@@ -177,10 +176,10 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
         for (int n = 0; n < 16; ++n)
 #pragma unroll
           for (int hh = 0; hh < 2; ++hh) {
-            const float p0 = fast_exp2(fmaf(s[4 * n + 2 * hh], scale_log2, -ms[hh]));
-            const float p1 = fast_exp2(fmaf(s[4 * n + 2 * hh + 1], scale_log2, -ms[hh]));
+            const float p0 = ptx::ex2_approx(fmaf(s[4 * n + 2 * hh], scale_log2, -ms[hh]));
+            const float p1 = ptx::ex2_approx(fmaf(s[4 * n + 2 * hh + 1], scale_log2, -ms[hh]));
             l_run[hh] += p0 + p1;
-            pk[2 * n + hh] = pack2(p0, p1);
+            pk[2 * n + hh] = pack_bf16x2(p0, p1);
           }
         // ---- O += P V_j ----
         ptx::mbar_wait(ptx::smem_u32(&v_full[st]), ph);
@@ -225,7 +224,7 @@ attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_consta
           __nv_bfloat16* orow = out + ((long long)b * Nq + qrow) * ldo + h * D + 2 * q;
 #pragma unroll
           for (int n = 0; n < 8; ++n)
-            *reinterpret_cast<uint32_t*>(orow + 8 * n) = pack2(o[4 * n + 2 * hh] * inv, o[4 * n + 2 * hh + 1] * inv);
+            *reinterpret_cast<uint32_t*>(orow + 8 * n) = pack_bf16x2(o[4 * n + 2 * hh] * inv, o[4 * n + 2 * hh + 1] * inv);
         }
       }
     }
@@ -252,20 +251,39 @@ static int launch_attention(const CUtensorMap& mq, const CUtensorMap& mk, const 
   return D3R_OK;
 }
 
-int attention_hd64_wgmma(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* out,
-                         long long ldo, int B, int heads, int Nq, int Nk, float scale, bool p_smem, cudaStream_t st) {
+// tokens of one image: [N][ld] bf16 -> 3-D map {cols, N, B}, box {64, box_rows, 1}: rows past N are zero-filled
+static int make_map(CUtensorMap* m, const void* base, long long ld, int cols, int N, int B, int box_rows) {
+  const cuuint64_t dims[3] = {(cuuint64_t)cols, (cuuint64_t)N, (cuuint64_t)B};
+  const cuuint64_t str[2] = {(cuuint64_t)ld * 2, (cuuint64_t)N * ld * 2};
+  const cuuint32_t box[3] = {64, (cuuint32_t)box_rows, 1};
+  return encode_tensor_map(m, base, 3, dims, str, box, "attention");
+}
+
+// 3 (default): P V with P in registers; 2: the same dataflow with P through shared memory, kept as the A/B reference --
+// both produce the same bits.
+static int g_impl = 3;
+
+int attention_hd64(const void* q, long long ldq, const void* k, long long ldk, const void* v, long long ldv, void* out,
+                   long long ldo, int B, int heads, int Nq, int Nk, float scale, cudaStream_t st) {
   D3R_CHECK_ARG(q && k && v && out && B > 0 && heads > 0 && Nq > 0 && Nk > 0, "attention: bad arguments");
   D3R_CHECK_ARG(ldq % 8 == 0 && ldk % 8 == 0 && ldv % 8 == 0 && ldo % 8 == 0, "attention: row strides must be multiples of 8");
   D3R_CHECK_ARG(((uintptr_t)q & 15) == 0 && ((uintptr_t)k & 15) == 0 && ((uintptr_t)v & 15) == 0 && ((uintptr_t)out & 15) == 0,
                 "attention: pointers must be 16-byte aligned");
   CUtensorMap mq, mk, mv;
   int rc;
-  if ((rc = tcc::make_map(&mq, q, ldq, heads * 64, Nq, B, wg::BQ))) return rc;
-  if ((rc = tcc::make_map(&mk, k, ldk, heads * 64, Nk, B, wg::BK))) return rc;
-  if ((rc = tcc::make_map(&mv, v, ldv, heads * 64, Nk, B, wg::BK))) return rc;
-  if (p_smem) return launch_attention<true>(mq, mk, mv, out, ldo, B, heads, Nq, Nk, scale, st);
+  if ((rc = make_map(&mq, q, ldq, heads * 64, Nq, B, wg::BQ))) return rc;
+  if ((rc = make_map(&mk, k, ldk, heads * 64, Nk, B, wg::BK))) return rc;
+  if ((rc = make_map(&mv, v, ldv, heads * 64, Nk, B, wg::BK))) return rc;
+  if (g_impl == 2) return launch_attention<true>(mq, mk, mv, out, ldo, B, heads, Nq, Nk, scale, st);
   return launch_attention<false>(mq, mk, mv, out, ldo, B, heads, Nq, Nk, scale, st);
 }
 
 }  // namespace attn
 }  // namespace d3r
+
+extern "C" void d3r_set_attention_impl(int32_t impl) { d3r::attn::g_impl = (impl == 2) ? 2 : 3; }
+
+extern "C" int d3r_attention_hd64(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out,
+                                  int64_t ldo, int32_t B, int32_t heads, int32_t Nq, int32_t Nk, float scale, void* stream) {
+  return d3r::attn::attention_hd64(q, ldq, k, ldk, v, ldv, out, ldo, B, heads, Nq, Nk, scale, (cudaStream_t)stream);
+}

@@ -6,15 +6,9 @@
 #include "elementwise.h"
 #include "prof.h"
 #include "pdl.cuh"
-#include <cuda_bf16.h>
 
 namespace d3r {
 namespace ew {
-
-__device__ __forceinline__ uint32_t pack2(float a, float b) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
 
 // ---- LayerNorm: one warp per row, row kept in registers (C <= 2048, C % 4 == 0) -----------------
 template <int MAXV>  // float4 per lane
@@ -61,7 +55,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
       const float4 gg = __ldg(g4 + c), bb = __ldg(b4 + c);
       const float y0 = (v[i].x - mean) * rstd * gg.x + bb.x, y1 = (v[i].y - mean) * rstd * gg.y + bb.y;
       const float y2 = (v[i].z - mean) * rstd * gg.z + bb.z, y3 = (v[i].w - mean) * rstd * gg.w + bb.w;
-      o[c] = make_uint2(pack2(y0, y1), pack2(y2, y3));
+      o[c] = make_uint2(pack_bf16x2(y0, y1), pack_bf16x2(y2, y3));
     }
   }
 }
@@ -86,7 +80,7 @@ __global__ void cast_kernel(const float4* __restrict__ x, uint2* __restrict__ o,
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n4) {
     const float4 v = x[i];
-    o[i] = make_uint2(pack2(v.x, v.y), pack2(v.z, v.w));
+    o[i] = make_uint2(pack_bf16x2(v.x, v.y), pack_bf16x2(v.z, v.w));
   }
 }
 int cast_f32_bf16(const float* x, void* out, size_t n, cudaStream_t st) {
@@ -139,8 +133,8 @@ __global__ void patch_im2col_kernel(const float* __restrict__ img, __nv_bfloat16
   const float4* src = reinterpret_cast<const float4*>(img + (((size_t)b * 3 + c) * H + ty * 16 + py) * W + tx * 16);
   uint4* dst = reinterpret_cast<uint4*>(out + tok * 768 + c * 256 + py * 16);
   const float4 a = src[0], bb = src[1], cc = src[2], d = src[3];
-  dst[0] = make_uint4(pack2(a.x, a.y), pack2(a.z, a.w), pack2(bb.x, bb.y), pack2(bb.z, bb.w));
-  dst[1] = make_uint4(pack2(cc.x, cc.y), pack2(cc.z, cc.w), pack2(d.x, d.y), pack2(d.z, d.w));
+  dst[0] = make_uint4(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w), pack_bf16x2(bb.x, bb.y), pack_bf16x2(bb.z, bb.w));
+  dst[1] = make_uint4(pack_bf16x2(cc.x, cc.y), pack_bf16x2(cc.z, cc.w), pack_bf16x2(d.x, d.y), pack_bf16x2(d.z, d.w));
 }
 int patch_im2col16(const float* img, void* out, int B, int H, int W, cudaStream_t st) {
   D3R_CHECK_ARG(H % 16 == 0 && W % 16 == 0, "patch_im2col: image %dx%d is not a multiple of the 16-pixel patch", H, W);
@@ -169,7 +163,7 @@ __device__ __forceinline__ uint4 lerp4(const uint4& a, const uint4& b, const uin
     const __nv_bfloat162 hd = *reinterpret_cast<const __nv_bfloat162*>(&dv[t]);
     const float lo = w00 * __low2float(ha) + w01 * __low2float(hb) + w10 * __low2float(hc) + w11 * __low2float(hd);
     const float hi = w00 * __high2float(ha) + w01 * __high2float(hb) + w10 * __high2float(hc) + w11 * __high2float(hd);
-    r[t] = pack2(lo, hi);
+    r[t] = pack_bf16x2(lo, hi);
   }
   return make_uint4(r[0], r[1], r[2], r[3]);
 }
@@ -264,22 +258,8 @@ int im2col_3x3_s2_bf16(const void* x, void* out, int B, int H, int W, int C, cud
   return D3R_OK;
 }
 
-// ---- postprocess (dust3r/heads/postprocess.py:10-58) ---------------------------------------------
-__device__ __forceinline__ void post_one(float x, float y, float z, float c, float* pts, float* conf, int depth_mode,
-                                         int conf_mode, float cmin, float cmax) {
-  float ox = x, oy = y, oz = z;
-  if (depth_mode != 0) {
-    const float d = sqrtf(x * x + y * y + z * z);
-    const float dc = fmaxf(d, 1e-8f);
-    const float s = (depth_mode == 2) ? expm1f(d) : d * d;
-    ox = x / dc * s; oy = y / dc * s; oz = z / dc * s;
-  }
-  pts[0] = ox; pts[1] = oy; pts[2] = oz;
-  if (conf_mode == 1) *conf = cmin + fminf(expf(c), cmax - cmin);
-  else if (conf_mode == 2) *conf = (cmax - cmin) * (1.f / (1.f + expf(-c))) + cmin;
-}
-
-// linear head: feat [B*gh*gw][nch*256] fp32, channel-major then (py,px)  -> pixel shuffle -> postprocess
+// ---- linear head: feat [B*gh*gw][nch*256] fp32, channel-major then (py,px)  -> pixel shuffle -> postprocess
+// (dust3r/heads/postprocess.py:10-58)
 __global__ void linear_head_post_kernel(const float* __restrict__ feat, float* __restrict__ pts3d, float* __restrict__ conf,
                                         int B, int gh, int gw, int nch, int depth_mode, int conf_mode, float cmin, float cmax) {
   pdl::sync_with_predecessor();   // PDL: nothing above touches memory produced by other kernels
@@ -292,9 +272,8 @@ __global__ void linear_head_post_kernel(const float* __restrict__ feat, float* _
   const size_t tok = ((size_t)b * gh + y / 16) * gw + x / 16;
   const int sub = (y % 16) * 16 + (x % 16);
   const float* f = feat + tok * (size_t)(nch * 256) + sub;
-  float c = nch > 3 ? f[3 * 256] : 0.f;
-  float dummy;
-  post_one(f[0], f[256], f[512], c, pts3d + idx * 3, nch > 3 ? conf + idx : &dummy, depth_mode, nch > 3 ? conf_mode : 0, cmin, cmax);
+  postprocess_pixel(f[0], f[256], f[512], [&] { return f[3 * 256]; }, pts3d, conf, (long long)idx, depth_mode, nch > 3 ? conf_mode : 0,
+                    cmin, cmax);
 }
 int linear_head_postprocess(const float* feat, float* pts3d, float* conf, int B, int gh, int gw, int nch, int depth_mode,
                             int conf_mode, float cmin, float cmax, cudaStream_t st) {

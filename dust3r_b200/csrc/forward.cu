@@ -354,35 +354,32 @@ static int decode_heads(const d3r_model* mp, const Ctx cv[2], const void* const 
   return D3R_OK;
 }
 
-// all images share one size: one encoder pass over the n_enc distinct images, pairs address them through idx1 / idx2
-static int forward(const d3r_model* mp, const float* imgs, int n_enc, const int32_t* idx1, const int32_t* idx2, int B, int H, int W,
-                   float* pts1, float* conf1, float* pts2, float* conf2, Arena& ar, cudaStream_t st) {
-  const d3r_model& m = *mp;
-  Ctx c{mp, st, H / m.patch, W / m.patch, (H / m.patch) * (W / m.patch)};
-  void* enc_out = nullptr;
-  RC(run_encoder(c, ar, imgs, n_enc, H, W, &enc_out));
-  const Ctx cv[2] = {c, c};
-  const void* enc[2] = {enc_out, enc_out};
-  const int32_t* maps[2] = {idx1, idx2};
-  // a dry (size-only) pass has no index lists; the gather path is what the real call takes
-  static const int32_t kDummy = 0;
-  if (ar.dry) maps[0] = maps[1] = &kDummy;
-  return decode_heads(mp, cv, enc, maps, B, pts1, conf1, pts2, conf2, ar, st);
+// One forward call.  Same-size (!mixed): imgs[0] holds n_enc images of H[0] x W[0] (H[1], W[1] equal), and pair b is
+// (image idx[0][b], image idx[1][b]), host arrays.  Mixed (two image sizes): imgs[br] holds the n_enc = B views br of
+// H[br] x W[br]; the reference encodes them separately (model.py:147-151) and the decoder cross-attends between the two
+// token grids.  Null pointers throughout for a dry (size-only) pass.
+struct Call {
+  bool mixed;
+  const float* imgs[2];
+  int n_enc, B, H[2], W[2];
+  const int32_t* idx[2];
+  float *pts[2], *conf[2];
+};
+
+static Ctx token_grid(const d3r_model* mp, cudaStream_t st, int H, int W) {
+  return Ctx{mp, st, H / mp->patch, W / mp->patch, (H / mp->patch) * (W / mp->patch)};
 }
 
-// the two views of every pair have different sizes (all first views H1 x W1, all second views H2 x W2): the reference
-// encodes them separately (model.py:147-151) and the decoder cross-attends between the two token grids
-static int forward_mixed(const d3r_model* mp, const float* imgs1, int H1, int W1, const float* imgs2, int H2, int W2, int B, float* pts1,
-                         float* conf1, float* pts2, float* conf2, Arena& ar, cudaStream_t st) {
-  const d3r_model& m = *mp;
-  const Ctx cv[2] = {Ctx{mp, st, H1 / m.patch, W1 / m.patch, (H1 / m.patch) * (W1 / m.patch)},
-                     Ctx{mp, st, H2 / m.patch, W2 / m.patch, (H2 / m.patch) * (W2 / m.patch)}};
+// same-size: one encoder pass over the n_enc distinct images, index gathers; mixed: one encoder pass per view, identity copies
+static int run(const d3r_model* mp, const Call& c, Arena& ar, cudaStream_t st) {
+  const Ctx cv[2] = {token_grid(mp, st, c.H[0], c.W[0]), token_grid(mp, st, c.H[1], c.W[1])};
   void* e[2] = {nullptr, nullptr};
-  RC(run_encoder(cv[0], ar, imgs1, B, H1, W1, &e[0]));
-  RC(run_encoder(cv[1], ar, imgs2, B, H2, W2, &e[1]));
+  RC(run_encoder(cv[0], ar, c.imgs[0], c.n_enc, c.H[0], c.W[0], &e[0]));
+  if (c.mixed) RC(run_encoder(cv[1], ar, c.imgs[1], c.n_enc, c.H[1], c.W[1], &e[1]));
+  else e[1] = e[0];
   const void* enc[2] = {e[0], e[1]};
-  const int32_t* maps[2] = {nullptr, nullptr};
-  return decode_heads(mp, cv, enc, maps, B, pts1, conf1, pts2, conf2, ar, st);
+  const int32_t* maps[2] = {c.mixed ? nullptr : c.idx[0], c.mixed ? nullptr : c.idx[1]};
+  return decode_heads(mp, cv, enc, maps, c.B, c.pts[0], c.conf[0], c.pts[1], c.conf[1], ar, st);
 }
 
 }  // namespace fwd
@@ -402,51 +399,54 @@ static int check_model(const d3r_model* m, int H, int W) {
   return D3R_OK;
 }
 
-extern "C" int64_t d3r_forward_workspace_bytes(const d3r_model* m, int32_t n_enc, int32_t B, int32_t H, int32_t W) {
-  if (check_model(m, H, W)) return -1;
+static int check_sizes(const d3r_model* m, const fwd::Call& c) {
+  RC(check_model(m, c.H[0], c.W[0]));
+  return c.mixed ? check_model(m, c.H[1], c.W[1]) : D3R_OK;
+}
+
+static int64_t workspace_bytes(const d3r_model* m, const fwd::Call& c) {
+  if (check_sizes(m, c)) return -1;
   fwd::Arena ar{nullptr, 0, 0, true};
-  if (fwd::forward(m, nullptr, n_enc, nullptr, nullptr, B, H, W, nullptr, nullptr, nullptr, nullptr, ar, 0)) return -1;
+  if (fwd::run(m, c, ar, 0)) return -1;
   return (int64_t)ar.off + 4096;
+}
+
+static int forward_call(const d3r_model* m, const fwd::Call& c, void* workspace_dev, int64_t workspace_bytes_given, void* stream) {
+  RC(check_sizes(m, c));
+  D3R_CHECK_ARG(c.imgs[0] && c.imgs[1] && (c.mixed || (c.idx[0] && c.idx[1])) && c.pts[0] && c.pts[1] && workspace_dev,
+                "forward: null buffer");
+  D3R_CHECK_ARG(c.n_enc > 0 && c.B > 0, "forward: empty batch");
+  for (int b = 0; !c.mixed && b < c.B; ++b)
+    D3R_CHECK_ARG(c.idx[0][b] >= 0 && c.idx[0][b] < c.n_enc && c.idx[1][b] >= 0 && c.idx[1][b] < c.n_enc, "forward: pair index out of range");
+  const int64_t need = workspace_bytes(m, c);
+  D3R_CHECK_ARG(need > 0 && workspace_bytes_given >= need, "forward: workspace of %lld bytes needed, %lld given", (long long)need,
+                (long long)workspace_bytes_given);
+  fwd::Arena ar{reinterpret_cast<uint8_t*>(workspace_dev), (size_t)workspace_bytes_given, 0, false};
+  const int rc = fwd::run(m, c, ar, (cudaStream_t)stream);
+  fwd::g_tap = {-1, nullptr, 0};
+  return rc;
+}
+
+extern "C" int64_t d3r_forward_workspace_bytes(const d3r_model* m, int32_t n_enc, int32_t B, int32_t H, int32_t W) {
+  return workspace_bytes(m, fwd::Call{false, {}, n_enc, B, {H, H}, {W, W}, {}, {}, {}});
 }
 
 extern "C" int d3r_forward_pairs(const d3r_model* m, const float* imgs_dev, int32_t n_enc, const int32_t* idx1_host,
                                  const int32_t* idx2_host, int32_t B, int32_t H, int32_t W, float* pts3d_1, float* conf_1,
                                  float* pts3d_2, float* conf_2, void* workspace_dev, int64_t workspace_bytes, void* stream) {
-  int rc = check_model(m, H, W);
-  if (rc) return rc;
-  D3R_CHECK_ARG(imgs_dev && idx1_host && idx2_host && pts3d_1 && pts3d_2 && workspace_dev, "forward: null buffer");
-  D3R_CHECK_ARG(n_enc > 0 && B > 0, "forward: empty batch");
-  for (int b = 0; b < B; ++b)
-    D3R_CHECK_ARG(idx1_host[b] >= 0 && idx1_host[b] < n_enc && idx2_host[b] >= 0 && idx2_host[b] < n_enc, "forward: pair index out of range");
-  const int64_t need = d3r_forward_workspace_bytes(m, n_enc, B, H, W);
-  D3R_CHECK_ARG(need > 0 && workspace_bytes >= need, "forward: workspace of %lld bytes needed, %lld given", (long long)need, (long long)workspace_bytes);
-  fwd::Arena ar{reinterpret_cast<uint8_t*>(workspace_dev), (size_t)workspace_bytes, 0, false};
-  rc = fwd::forward(m, imgs_dev, n_enc, idx1_host, idx2_host, B, H, W, pts3d_1, conf_1, pts3d_2, conf_2, ar, (cudaStream_t)stream);
-  fwd::g_tap = {-1, nullptr, 0};
-  return rc;
+  const fwd::Call c{false, {imgs_dev, imgs_dev}, n_enc, B, {H, H}, {W, W}, {idx1_host, idx2_host}, {pts3d_1, pts3d_2}, {conf_1, conf_2}};
+  return forward_call(m, c, workspace_dev, workspace_bytes, stream);
 }
 
 extern "C" int64_t d3r_forward_mixed_workspace_bytes(const d3r_model* m, int32_t B, int32_t H1, int32_t W1, int32_t H2, int32_t W2) {
-  if (check_model(m, H1, W1) || check_model(m, H2, W2)) return -1;
-  fwd::Arena ar{nullptr, 0, 0, true};
-  if (fwd::forward_mixed(m, nullptr, H1, W1, nullptr, H2, W2, B, nullptr, nullptr, nullptr, nullptr, ar, 0)) return -1;
-  return (int64_t)ar.off + 4096;
+  return workspace_bytes(m, fwd::Call{true, {}, B, B, {H1, H2}, {W1, W2}, {}, {}, {}});
 }
 
 extern "C" int d3r_forward_pairs_mixed(const d3r_model* m, const float* imgs1_dev, int32_t H1, int32_t W1, const float* imgs2_dev,
                                        int32_t H2, int32_t W2, int32_t B, float* pts3d_1, float* conf_1, float* pts3d_2,
                                        float* conf_2, void* workspace_dev, int64_t workspace_bytes, void* stream) {
-  int rc = check_model(m, H1, W1);
-  if (rc) return rc;
-  if ((rc = check_model(m, H2, W2))) return rc;
-  D3R_CHECK_ARG(imgs1_dev && imgs2_dev && pts3d_1 && pts3d_2 && workspace_dev, "forward: null buffer");
-  D3R_CHECK_ARG(B > 0, "forward: empty batch");
-  const int64_t need = d3r_forward_mixed_workspace_bytes(m, B, H1, W1, H2, W2);
-  D3R_CHECK_ARG(need > 0 && workspace_bytes >= need, "forward: workspace of %lld bytes needed, %lld given", (long long)need, (long long)workspace_bytes);
-  fwd::Arena ar{reinterpret_cast<uint8_t*>(workspace_dev), (size_t)workspace_bytes, 0, false};
-  rc = fwd::forward_mixed(m, imgs1_dev, H1, W1, imgs2_dev, H2, W2, B, pts3d_1, conf_1, pts3d_2, conf_2, ar, (cudaStream_t)stream);
-  fwd::g_tap = {-1, nullptr, 0};
-  return rc;
+  const fwd::Call c{true, {imgs1_dev, imgs2_dev}, B, B, {H1, H2}, {W1, W2}, {}, {pts3d_1, pts3d_2}, {conf_1, conf_2}};
+  return forward_call(m, c, workspace_dev, workspace_bytes, stream);
 }
 
 extern "C" int d3r_sizeof_model(void) { return (int)sizeof(d3r_model); }

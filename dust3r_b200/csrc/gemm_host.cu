@@ -2,50 +2,11 @@
 #include "gemm_wgmma.cuh"
 #include "gemm_host.h"
 #include "prof.h"
-#include <mutex>
 
 namespace d3r {
 namespace gemm {
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-        q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  });
-  return fn;
-}
-
-static int encode(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                  const cuuint32_t* box, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16) {
-  EncodeTiledFn fn = get_encode();
-  if (!fn) {
-    set_error("cuTensorMapEncodeTiled is not available from the CUDA driver");
-    return D3R_ERR_CUDA;
-  }
-  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(m, dtype, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides_bytes, box,
-                  estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed with CUresult %d (rank %d, dims %llu,%llu)", (int)r, rank,
-              (unsigned long long)dims[0], (unsigned long long)dims[1]);
-    return D3R_ERR_CUDA;
-  }
-  return D3R_OK;
-}
-
-bool use_pair(int bn, int num_kb);
-
-int pick_block_n(int N, int mode, uint32_t flags) {
+static int pick_block_n(int N, int mode, uint32_t flags) {
   if (flags & F_HEAD_FINAL) return 128;   // the head tail needs a whole 128-channel row in one tile
   // 128x256 tiles for the specialised epilogues (every ViT projection): half the A traffic per FLOP of 128x128
   if (N % 256 == 0 && pick_epi(mode, flags) != EPI_GENERIC) return 256;
@@ -59,9 +20,7 @@ int pick_block_n(int N, int mode, uint32_t flags) {
 // re-assembly), whose time goes to the epilogue rather than to operand traffic.
 static int g_impl = 2;
 static int g_pair_min_kb = 4;
-void set_impl(int impl) { g_impl = impl; }
-void set_pair_min_kb(int kb) { g_pair_min_kb = kb; }
-bool use_pair(int bn, int num_kb) { return bn >= 128 && (g_impl == 1 || (g_impl == 2 && num_kb >= g_pair_min_kb)); }
+static bool use_pair(int bn, int num_kb) { return bn >= 128 && (g_impl == 1 || (g_impl == 2 && num_kb >= g_pair_min_kb)); }
 
 template <int BN, int EPI, bool PAIR>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int m_tiles, int n_tiles, cudaStream_t st) {
@@ -116,11 +75,11 @@ static int dispatch(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const 
 }
 
 // B operand: [N][taps][Kc] bf16, K-major
-static int make_tmap_b(CUtensorMap* m, const void* B, int N, int taps, int Kc, int bn, int num_kb) {
+static int make_tmap_b(CUtensorMap* m, const void* B, int N, int taps, int Kc, int bn, int num_kb, const char* op) {
   cuuint64_t dims[3] = {(cuuint64_t)Kc, (cuuint64_t)taps, (cuuint64_t)N};
   cuuint64_t str[2] = {(cuuint64_t)Kc * 2, (cuuint64_t)taps * Kc * 2};
   cuuint32_t box[3] = {(cuuint32_t)BLOCK_K, 1, (cuuint32_t)(use_pair(bn, num_kb) ? bn / 2 : bn)};   // each CTA of a pair stages half of B
-  return encode(m, B, 3, dims, str, box);
+  return encode_tensor_map(m, B, 3, dims, str, box, op);
 }
 
 int gemm_bf16(const void* A, long long lda, const void* B, Params p, cudaStream_t st) {
@@ -137,10 +96,10 @@ int gemm_bf16(const void* A, long long lda, const void* B, Params p, cudaStream_
     cuuint64_t dims[2] = {(cuuint64_t)p.K, (cuuint64_t)p.M};
     cuuint64_t str[1] = {(cuuint64_t)lda * 2};
     cuuint32_t box[2] = {(cuuint32_t)BLOCK_K, (cuuint32_t)BLOCK_M};
-    int rc = encode(&ta, A, 2, dims, str, box);
+    int rc = encode_tensor_map(&ta, A, 2, dims, str, box, "gemm");
     if (rc) return rc;
   }
-  int rc = make_tmap_b(&tb, B, p.N, 1, p.K, bn, p.num_kb);
+  int rc = make_tmap_b(&tb, B, p.N, 1, p.K, bn, p.num_kb, "gemm");
   if (rc) return rc;
   return dispatch(bn, ta, tb, p, (p.M + BLOCK_M - 1) / BLOCK_M, st);
 }
@@ -168,10 +127,10 @@ int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, 
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t str[3] = {(cuuint64_t)Cin * 2, (cuuint64_t)W * Cin * 2, (cuuint64_t)H * W * Cin * 2};
     cuuint32_t box[4] = {(cuuint32_t)BLOCK_K, (cuuint32_t)p.tile_w, (cuuint32_t)p.tile_h, 1};
-    int rc = encode(&ta, x_nhwc, 4, dims, str, box);
+    int rc = encode_tensor_map(&ta, x_nhwc, 4, dims, str, box, "conv3x3");
     if (rc) return rc;
   }
-  int rc = make_tmap_b(&tb, w_packed, Cout, 9, Cin, bn, p.num_kb);
+  int rc = make_tmap_b(&tb, w_packed, Cout, 9, Cin, bn, p.num_kb, "conv3x3");
   if (rc) return rc;
   return dispatch(bn, ta, tb, p, B * p.tiles_x * p.tiles_y, st);
 }
@@ -182,8 +141,8 @@ int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, 
 // ---- building blocks exported through the C ABI (used by the unit tests and by forward.cu) ----
 using namespace d3r;
 
-extern "C" void d3r_set_gemm_impl(int32_t impl) { gemm::set_impl(impl); }
-extern "C" void d3r_set_gemm_pair_min_kblocks(int32_t kb) { gemm::set_pair_min_kb(kb); }
+extern "C" void d3r_set_gemm_impl(int32_t impl) { gemm::g_impl = impl; }
+extern "C" void d3r_set_gemm_pair_min_kblocks(int32_t kb) { gemm::g_pair_min_kb = kb; }
 
 extern "C" int d3r_gemm_bf16(const void* A, const void* B, void* out, const float* bias, const void* add0, void* out2,
                              int32_t M, int32_t N, int32_t K, int64_t ldo, uint32_t flags, const float* rope_cos,

@@ -4,9 +4,6 @@
 
 namespace d3r {
 namespace gemm {
-int pick_block_n(int N, int mode, uint32_t flags);
-void set_impl(int impl);
-void set_pair_min_kb(int kb);
 // A: [M][lda] bf16 row-major (K valid columns), B: [N][K] bf16.  p.{M,N,K,flags,out,...} filled by the caller.
 int gemm_bf16(const void* A, long long lda, const void* B, Params p, cudaStream_t st);
 // x: (B,H,W,Cin) bf16 NHWC, w_packed: [Cout][9][Cin] bf16, output (B,H,W,Cout).

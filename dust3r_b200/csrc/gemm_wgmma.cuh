@@ -114,26 +114,14 @@ __device__ __forceinline__ float gelu_erf(float x) {
   constexpr float kU = 0.84932180028801904f;            // sqrt(log2(e) / 2)
   constexpr float kP = 0.3275911f * 0.70710678118654752f / kU;
   const float u = fabsf(x) * kU;
-  float t, e;
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(t) : "f"(fmaf(kP, u, 1.f)));
+  const float t = ptx::rcp_approx(fmaf(kP, u, 1.f));
   float poly = fmaf(0.5f * 1.061405429f, t, 0.5f * -1.453152027f);
   poly = fmaf(poly, t, 0.5f * 1.421413741f);
   poly = fmaf(poly, t, 0.5f * -0.284496736f);
   poly = fmaf(poly, t, 0.5f * 0.254829592f);
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(-u * u));
+  const float e = ptx::ex2_approx(-u * u);
   const float h = x * (poly * t * e);
   return fmaxf(x, 0.f) - fabsf(h);
-}
-
-__device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(a, b);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-
-
-__device__ __forceinline__ float2 bf16x2_to_float2(uint32_t w) {
-  const __nv_bfloat162 h = *reinterpret_cast<const __nv_bfloat162*>(&w);
-  return make_float2(__low2float(h), __high2float(h));
 }
 
 template <int BLOCK_N, int EPI, bool PAIR>
@@ -370,24 +358,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           if (!valid[h] || q != 0) continue;
-          // dust3r/heads/postprocess.py: pts3d = xyz/|xyz| * f(|xyz|), conf = vmin + exp(x) (clipped)
-          const float x = head_acc[h][0] + s_w4[512 + 0], y = head_acc[h][1] + s_w4[512 + 1], z = head_acc[h][2] + s_w4[512 + 2];
-          float ox = x, oy = y, oz = z;
-          if (p.depth_mode != 0) {
-            const float d = sqrtf(x * x + y * y + z * z);
-            const float dc = fmaxf(d, 1e-8f);
-            const float s = (p.depth_mode == 2) ? expm1f(d) : d * d;
-            ox = x / dc * s; oy = y / dc * s; oz = z / dc * s;
-          }
-          float* o = p.pts3d + pix[h] * 3;
-          o[0] = ox; o[1] = oy; o[2] = oz;
-          if (p.conf_mode != 0) {
-            const float c = head_acc[h][3] + s_w4[512 + 3];
-            float r;
-            if (p.conf_mode == 1) r = p.conf_min + fminf(expf(c), p.conf_max - p.conf_min);
-            else r = (p.conf_max - p.conf_min) * (1.f / (1.f + expf(-c))) + p.conf_min;
-            p.conf[pix[h]] = r;
-          }
+          postprocess_pixel(head_acc[h][0] + s_w4[512 + 0], head_acc[h][1] + s_w4[512 + 1], head_acc[h][2] + s_w4[512 + 2],
+                            [&] { return head_acc[h][3] + s_w4[512 + 3]; }, p.pts3d, p.conf, pix[h], p.depth_mode, p.conf_mode,
+                            p.conf_min, p.conf_max);
         }
         continue;
       }
@@ -424,11 +397,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
               v0 += r.x; v1 += r.y;
             }
             *o = make_float2(v0, v1);
-            if (flags & F_OUT2_BF16) *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out2) + off) = pack_bf16(v0, v1);
+            if (flags & F_OUT2_BF16) *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out2) + off) = pack_bf16x2(v0, v1);
           } else {
-            *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + off) = pack_bf16(v0, v1);
+            *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out) + off) = pack_bf16x2(v0, v1);
             if (flags & F_OUT2_RELU)
-              *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out2) + off) = pack_bf16(fmaxf(v0, 0.f), fmaxf(v1, 0.f));
+              *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.out2) + off) = pack_bf16x2(fmaxf(v0, 0.f), fmaxf(v1, 0.f));
           }
         }
       }

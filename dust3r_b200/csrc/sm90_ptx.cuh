@@ -1,6 +1,6 @@
 // Thin inline-PTX wrappers for the Hopper (sm_90a) primitives used by the dust3r_b200 kernels:
 // mbarrier, bulk copies (cp.async.bulk), TMA (cp.async.bulk.tensor, with cluster multicast), clusters, wgmma (fence / mma /
-// commit / wait).
+// commit / wait), and the MUFU approximations.
 // Descriptor bit layouts follow the PTX ISA "wgmma matrix descriptor" table.
 #pragma once
 #include <cuda.h>
@@ -136,6 +136,12 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank)
       "mbarrier.arrive.shared::cluster.b64 _, [raddr];\n"
       "}\n" ::"r"(bar), "r"(rank) : "memory");
 }
+
+// ---- MUFU approximations (flush-to-zero).  Not volatile: the compiler may schedule, merge or drop them like arithmetic.
+__device__ __forceinline__ float ex2_approx(float x) { float y; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ float rsqrt_approx(float x) { float y; asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ float sqrt_approx(float x) { float y; asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
 
 // ---- register budget of warp-specialised kernels ------------------------------------------------------
 template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }

@@ -226,9 +226,7 @@ class AsymmetricCroCo3DStereo(nn.Module, _HubMixin, **_hub_kwargs):
                 raise AssertionError(f'true_shape {(h, w)} does not match the image tensor {(Hv, Wv)}')
         if (H, W) != (H2, W2):
             # model.py:147-151: the two views are encoded separately; the decoder cross-attends between the two grids
-            res1, res2 = self._packed.forward_mixed(img1.float().contiguous(), img2.float().contiguous())
-            res2['pts3d_in_other_view'] = res2.pop('pts3d')
-            return res1, res2
+            return _in_other_view(self._packed.forward_mixed(img1.float().contiguous(), img2.float().contiguous()))
         # model.py:153-170: a batch [(a,b),(b,a),...] only encodes its even half
         if is_symmetrized(view1, view2):
             imgs = torch.cat((img1[::2], img2[::2]), dim=0)
@@ -241,9 +239,7 @@ class AsymmetricCroCo3DStereo(nn.Module, _HubMixin, **_hub_kwargs):
             imgs = torch.cat((img1, img2), dim=0)
             idx1 = np.arange(B, dtype=np.int32)
             idx2 = B + np.arange(B, dtype=np.int32)
-        res1, res2 = self._packed.forward(imgs.float().contiguous(), idx1, idx2, B, H, W)
-        res2['pts3d_in_other_view'] = res2.pop('pts3d')
-        return res1, res2
+        return _in_other_view(self._packed.forward(imgs.float().contiguous(), idx1, idx2, B, H, W))
 
 
     def _forward_many_ar(self, view1, view2, port1, port2):
@@ -288,9 +284,15 @@ class AsymmetricCroCo3DStereo(nn.Module, _HubMixin, **_hub_kwargs):
         B = len(idx1)
         assert len(idx2) == B and B > 0
         H, W = int(imgs.shape[-2]), int(imgs.shape[-1])
-        res1, res2 = self._packed.forward(imgs.float().contiguous(), np.asarray(idx1, dtype=np.int32), np.asarray(idx2, dtype=np.int32), B, H, W)
-        res2['pts3d_in_other_view'] = res2.pop('pts3d')
-        return res1, res2
+        return _in_other_view(self._packed.forward(imgs.float().contiguous(), np.asarray(idx1, dtype=np.int32),
+                                                   np.asarray(idx2, dtype=np.int32), B, H, W))
+
+
+def _in_other_view(res):
+    """Output naming of the reference (model.py:210): view 2's points are expressed in view 1's frame."""
+    res1, res2 = res
+    res2['pts3d_in_other_view'] = res2.pop('pts3d')
+    return res1, res2
 
 
 class _PackedModel:
@@ -423,67 +425,42 @@ class _PackedModel:
         self._ws = None
         self._ws_key = None
 
-    def workspace(self, n_enc, B, H, W):
-        key = (n_enc, B, H, W)
+    def _run(self, launch, query, dims, inputs, B, sizes, debug=None):
+        """One call of d3r_forward_pairs / d3r_forward_pairs_mixed (`launch`): the workspace, sized by `query` on the
+        call's shape `dims` and kept while the shape stays the same, and one ({'pts3d','conf'}) dict per view."""
+        key = (query.__name__,) + dims
         if self._ws_key != key:
-            need = self.lib.d3r_forward_workspace_bytes(C.byref(self.cmodel), n_enc, B, H, W)
+            need = query(C.byref(self.cmodel), *dims)
             if need <= 0:
                 _lib.check(-1)
             self._ws = None   # free the old one first
             self._ws = torch.empty((need,), dtype=torch.uint8, device=self.device)
             self._ws_key = key
-        return self._ws
+        dev = self.device
+        res = tuple({'pts3d': torch.empty((B, H, W, 3), dtype=torch.float32, device=dev)} for H, W in sizes)
+        if self.cmodel.nch > 3:
+            for r, (H, W) in zip(res, sizes):
+                r['conf'] = torch.empty((B, H, W), dtype=torch.float32, device=dev)
+        if debug is not None:
+            stage, buf = debug
+            _lib.check(self.lib.d3r_forward_set_debug(stage, buf.data_ptr(), buf.numel()))
+        outs = [r[k].data_ptr() if k in r else None for r in res for k in ('pts3d', 'conf')]
+        with torch.cuda.device(dev):
+            _lib.check(launch(C.byref(self.cmodel), *inputs, *outs, self._ws.data_ptr(), self._ws.numel(), _lib.stream_ptr()))
+        return res
 
     def forward_mixed(self, imgs1, imgs2):
         """imgs1 (B,3,H1,W1), imgs2 (B,3,H2,W2) fp32 CUDA with different sizes -> ({'pts3d','conf'}, {'pts3d','conf'})."""
         B = int(imgs1.shape[0])
         assert int(imgs2.shape[0]) == B
         H1, W1, H2, W2 = int(imgs1.shape[-2]), int(imgs1.shape[-1]), int(imgs2.shape[-2]), int(imgs2.shape[-1])
-        key = ('mixed', B, H1, W1, H2, W2)
-        if self._ws_key != key:
-            need = self.lib.d3r_forward_mixed_workspace_bytes(C.byref(self.cmodel), B, H1, W1, H2, W2)
-            if need <= 0:
-                _lib.check(-1)
-            self._ws = None
-            self._ws = torch.empty((need,), dtype=torch.uint8, device=self.device)
-            self._ws_key = key
-        dev = self.device
-        has_conf = self.cmodel.nch > 3
-        pts1 = torch.empty((B, H1, W1, 3), dtype=torch.float32, device=dev)
-        pts2 = torch.empty((B, H2, W2, 3), dtype=torch.float32, device=dev)
-        conf1 = torch.empty((B, H1, W1), dtype=torch.float32, device=dev) if has_conf else None
-        conf2 = torch.empty((B, H2, W2), dtype=torch.float32, device=dev) if has_conf else None
-        with torch.cuda.device(dev):
-            _lib.check(self.lib.d3r_forward_pairs_mixed(C.byref(self.cmodel), imgs1.data_ptr(), H1, W1, imgs2.data_ptr(), H2, W2, B,
-                                                        pts1.data_ptr(), conf1.data_ptr() if has_conf else None,
-                                                        pts2.data_ptr(), conf2.data_ptr() if has_conf else None,
-                                                        self._ws.data_ptr(), self._ws.numel(), _lib.stream_ptr()))
-        r1, r2 = {'pts3d': pts1}, {'pts3d': pts2}
-        if has_conf:
-            r1['conf'], r2['conf'] = conf1, conf2
-        return r1, r2
+        return self._run(self.lib.d3r_forward_pairs_mixed, self.lib.d3r_forward_mixed_workspace_bytes, (B, H1, W1, H2, W2),
+                         (imgs1.data_ptr(), H1, W1, imgs2.data_ptr(), H2, W2, B), B, ((H1, W1), (H2, W2)))
 
     def forward(self, imgs, idx1, idx2, B, H, W, debug=None):
         """imgs: (n_enc,3,H,W) fp32 CUDA.  Returns ({'pts3d','conf'}, {'pts3d','conf'}) CUDA fp32 tensors."""
         n_enc = int(imgs.shape[0])
-        ws = self.workspace(n_enc, B, H, W)
-        dev = self.device
-        has_conf = self.cmodel.nch > 3
-        pts1 = torch.empty((B, H, W, 3), dtype=torch.float32, device=dev)
-        pts2 = torch.empty((B, H, W, 3), dtype=torch.float32, device=dev)
-        conf1 = torch.empty((B, H, W), dtype=torch.float32, device=dev) if has_conf else None
-        conf2 = torch.empty((B, H, W), dtype=torch.float32, device=dev) if has_conf else None
         i1 = (C.c_int32 * B)(*[int(v) for v in idx1])
         i2 = (C.c_int32 * B)(*[int(v) for v in idx2])
-        if debug is not None:
-            stage, buf = debug
-            _lib.check(self.lib.d3r_forward_set_debug(stage, buf.data_ptr(), buf.numel()))
-        with torch.cuda.device(dev):
-            _lib.check(self.lib.d3r_forward_pairs(C.byref(self.cmodel), imgs.data_ptr(), n_enc, i1, i2, B, H, W,
-                                                  pts1.data_ptr(), conf1.data_ptr() if has_conf else None,
-                                                  pts2.data_ptr(), conf2.data_ptr() if has_conf else None,
-                                                  ws.data_ptr(), ws.numel(), _lib.stream_ptr()))
-        r1, r2 = {'pts3d': pts1}, {'pts3d': pts2}
-        if has_conf:
-            r1['conf'], r2['conf'] = conf1, conf2
-        return r1, r2
+        return self._run(self.lib.d3r_forward_pairs, self.lib.d3r_forward_workspace_bytes, (n_enc, B, H, W),
+                         (imgs.data_ptr(), n_enc, i1, i2, B, H, W), B, ((H, W), (H, W)), debug)
