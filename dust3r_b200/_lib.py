@@ -62,6 +62,8 @@ def _declare(lib):
         getattr(lib, name).argtypes = [C.POINTER(AlignDesc), vp]
     lib.d3r_align_run.restype = C.c_int
     lib.d3r_align_run.argtypes = [C.POINTER(AlignDesc), i32, i32, vp]
+    lib.d3r_align_loss_grad.restype = C.c_int
+    lib.d3r_align_loss_grad.argtypes = [C.POINTER(AlignDesc), vp, vp, vp, vp]
     lib.d3r_align_overflow_flag.restype = C.c_int
     lib.d3r_align_overflow_flag.argtypes = [C.POINTER(AlignDesc), C.POINTER(C.c_int32), vp]
     lib.d3r_align_pts3d.restype = C.c_int

@@ -12,6 +12,7 @@ from copy import deepcopy
 
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from ..utils.geometry import inv
 from ..utils.image import rgb
@@ -267,16 +268,34 @@ class BasePCOptimizer(nn.Module):
         eng = self._engine if self._engine is not None else self._build_engine()
         return eng
 
+    def _engine_params(self):
+        """Every parameter the engine optimises, in the order of _engine_grads."""
+        raise NotImplementedError()
+
+    def _engine_grads(self, eng, logd_grad, small_grad):
+        """Gradients of _engine_params() from the flat gradients of AlignEngine.loss_and_grad, each shaped like its
+        parameter."""
+        raise NotImplementedError()
+
     def forward(self, ret_details=False):
-        """Objective at the current parameters (a CUDA scalar tensor; no autograd graph — gradients
-        are analytic inside the fused kernel)."""
-        if ret_details:
-            raise NotImplementedError('ret_details is not provided by the fused kernel')
+        """Objective at the current parameters (a CUDA scalar tensor).  With grad mode on and a parameter that requires
+        grad, the loss carries an autograd graph: backward() hands the fused kernel's analytic gradients to the
+        parameters.  ret_details=True also returns the (n, n) CPU tensor of per-edge losses li + lj (-1 off the edges)."""
         eng = self._get_engine()
-        pull = self._engine_push(eng)
-        loss = eng.evaluate_loss()
-        del pull
-        return loss
+        self._engine_push(eng)
+        params = self._engine_params()
+        if not ret_details and not (torch.is_grad_enabled() and any(p.requires_grad for p in params)):
+            return eng.evaluate_loss()
+        loss, logd_grad, small_grad, ent = eng.loss_and_grad(entry_loss=ret_details)
+        loss = _FusedObjective.apply(loss, self._engine_grads(eng, logd_grad, small_grad), *params)
+        if not ret_details:
+            return loss
+        # per-edge pixel means: the entries carry the coefficient 1 / (area * n_edges)
+        per_edge = (ent.sum(dim=1) * self.n_edges).cpu()
+        details = -torch.ones((self.n_imgs, self.n_imgs))
+        for e, (i, j) in enumerate(self.edges):
+            details[i, j] = per_edge[e]
+        return loss, details
 
     @torch.no_grad()
     def compute_global_alignment(self, init=None, niter_PnP=10, **kw):
@@ -298,6 +317,22 @@ class BasePCOptimizer(nn.Module):
 
     def show(self, *a, **kw):
         raise NotImplementedError('visualisation is outside the two hot paths (SURVEY §2 #14)')
+
+
+class _FusedObjective(torch.autograd.Function):
+    """Attaches the gradients the fused kernel computed with the loss to the parameters: backward returns
+    grad_output x the stored gradient of every parameter that requires grad."""
+
+    @staticmethod
+    def forward(ctx, loss, grads, *params):
+        ctx.grads = grads
+        return loss.clone()
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_output):
+        need = ctx.needs_input_grad[2:]
+        return (None, None) + tuple(g * grad_output if want else None for g, want in zip(ctx.grads, need))
 
 
 @torch.no_grad()

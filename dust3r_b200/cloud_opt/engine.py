@@ -307,16 +307,20 @@ class AlignEngine:
         self.norm_pw_scale = bool(norm_pw_scale)
         self._prepared = False
 
-    def get_small(self):
+    def split_small(self, flat):
+        """Views of a flat buffer in the `small` layout -- the parameters or their gradients -- one per parameter kind,
+        shaped like the stacked parameters; im_focals is (n, 1) with a tied focal (both slots hold the same value)."""
         n, E = self.n, self.E
         o = self._offsets()
-        s = self.small
-        f = s[o['focals']:o['pp']].reshape(n, 2)
-        return dict(im_poses=s[o['poses']:o['focals']].reshape(n, 7).clone(),
-                    im_focals=(f[:, :1] if self.tied_focal else f).clone(),
-                    im_pp=s[o['pp']:o['pw']].reshape(n, 2).clone(),
-                    pw_poses=s[o['pw']:o['adapt']].reshape(E, 8).clone(),
-                    pw_adaptors=s[o['adapt']:].reshape(E, 2).clone())
+        f = flat[o['focals']:o['pp']].reshape(n, 2)
+        return dict(im_poses=flat[o['poses']:o['focals']].reshape(n, 7),
+                    im_focals=f[:, :1] if self.tied_focal else f,
+                    im_pp=flat[o['pp']:o['pw']].reshape(n, 2),
+                    pw_poses=flat[o['pw']:o['adapt']].reshape(E, 8),
+                    pw_adaptors=flat[o['adapt']:].reshape(E, 2))
+
+    def get_small(self):
+        return {k: v.clone() for k, v in self.split_small(self.small).items()}
 
     def reset_adam(self):
         self.small_m.zero_()
@@ -419,6 +423,24 @@ class AlignEngine:
         d = self._desc(eval_only=True)
         self._call(self.lib.d3r_align_run, C.byref(d), 0, 1)
         return self.loss_out[0]
+
+    def loss_and_grad(self, entry_loss=False):
+        """net.forward() + loss.backward() at the current parameters in one launch (d3r_align_loss_grad); nothing is
+        updated.  Returns (loss, logd_grad, small_grad, entry_loss): a 0-dim loss, dL/dlog-depth laid out like `logd`
+        (0 on padding pixels), dL/d(raw parameter) in the `small` layout (split it with split_small) and, when asked
+        for, the (E, 2) coefficient-weighted loss of every (edge, side), else None.  Every tensor is freshly allocated,
+        so results of two calls never alias."""
+        dev = self.device
+        loss = torch.zeros((), dtype=torch.float32, device=dev)
+        logd_grad = torch.zeros_like(self.logd)
+        small_grad = torch.empty((self.n_small,), dtype=torch.float32, device=dev)
+        ent = torch.empty((self.E, 2), dtype=torch.float32, device=dev) if entry_loss else None
+        self.prepare()
+        d = self._desc()
+        d.loss_out = loss.data_ptr()
+        self._call(self.lib.d3r_align_loss_grad, C.byref(d), logd_grad.data_ptr(), small_grad.data_ptr(),
+                   ent.data_ptr() if ent is not None else None)
+        return loss, logd_grad, small_grad, ent
 
     def pts3d(self):
         """(sum stride_i, 3) world points of every image's pixels."""

@@ -50,6 +50,18 @@ class ModularPointCloudOptimizer(BasePCOptimizer):
             self.pw_adaptors.data.copy_(s['pw_adaptors'])
         return pull
 
+    def _engine_params(self):
+        return [*self.im_depthmaps, *self.im_poses, *self.im_focals, *self.im_pp, self.pw_poses, self.pw_adaptors]
+
+    def _engine_grads(self, eng, logd_grad, small_grad):
+        g = eng.split_small(small_grad)
+        depth, off = [], 0
+        for H, W in self.imshapes:
+            depth.append(logd_grad[off:off + H * W].view(H, W))
+            off += H * W
+        return [*depth, *g['im_poses'].unbind(0), *g['im_focals'].unbind(0), *g['im_pp'].unbind(0), g['pw_poses'],
+                g['pw_adaptors']]
+
     # ---------------------------------------------------------------- fixing parameters to known values
     # A preset writes the value into the per-image parameter and switches its gradient off; the fused step receives the
     # flags as its trainable mask (see _engine_push), so a preset image keeps exactly the value given here.

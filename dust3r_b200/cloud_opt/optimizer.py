@@ -89,6 +89,19 @@ class PointCloudOptimizer(BasePCOptimizer):
             self.pw_adaptors.data.copy_(s['pw_adaptors'])
         return pull
 
+    def _engine_params(self):
+        return [self.im_depthmaps, self.im_poses, self.im_focals, self.im_pp, self.pw_poses, self.pw_adaptors]
+
+    def _engine_grads(self, eng, logd_grad, small_grad):
+        g = eng.split_small(small_grad)
+        return [logd_grad.view(self.n_imgs, self.max_area), g['im_poses'], g['im_focals'], g['im_pp'], g['pw_poses'],
+                g['pw_adaptors']]
+
+    def forward(self, ret_details=False):
+        if ret_details:      # the reference's PointCloudOptimizer.forward has no per-edge details (optimizer.py:188-201)
+            raise NotImplementedError('ret_details is only provided by the per-edge objective (ModularPointCloudOptimizer)')
+        return super().forward()
+
     # ---------------------------------------------------------------- fixing parameters to known values
     # The stacked optimizer keeps one tensor per parameter kind, so a preset must cover EVERY image and freezes the
     # whole kind (use ModularPointCloudOptimizer to pin a subset of the cameras).

@@ -420,6 +420,57 @@ static __device__ __noinline__ void small_param_step(const d3r_align_desc& D, co
 }
 
 
+// Outputs of a gradient launch (d3r_align_loss_grad): the gradient-export instantiations of both pixel kernels write the
+// per-pixel log-depth gradient to logd_grad in their depth stage, and their last CTA runs small_grad_step instead of the
+// small-parameter step.
+struct GradOut {
+  float* logd_grad;     // [sum stride_i]
+  float* small_grad;    // [11n + 10E] flat parameter layout
+  float* entry_loss;    // [E][2] or nullptr
+};
+
+// Gradient export in place of the small-parameter step: the loss (same order as small_param_step, so bit-identical to
+// eval_only), the raw gradients of every parameter written to go.small_grad with the log-scale coupling folded in -- the
+// values adam_param would feed Adam -- and optionally the per-entry loss.  No Adam step, no refresh; the accumulators
+// are cleared as after any launch.
+static __device__ __noinline__ void small_grad_step(const d3r_align_desc& D, const Workspace& ws, GradOut go, float* s_red) {
+  const int n = D.n_imgs, E = D.n_edges;
+  const SmallLayout L(n, E);
+  float lpart = 0.f;
+  int bad = 0;
+  for (int k = threadIdx.x; k < 2 * E; k += blockDim.x) lpart += fix_get(ws.ent_acc + k * kEntVals + 12, bad);
+  const float loss = block_sum8(lpart, s_red);
+  if (threadIdx.x == 0) D.loss_out[0] = loss;
+
+  float coupl = 0.f;
+  for (int e = threadIdx.x; e < E; e += blockDim.x) {
+    const int ei = D.edge_ent[e * 2 + 0], ej = D.edge_ent[e * 2 + 1];
+    float si[12], sj[12], c[kGeomE];
+#pragma unroll
+    for (int k = 0; k < 12; ++k) { si[k] = fix_get(ws.ent_acc + ei * kEntVals + k, bad); sj[k] = fix_get(ws.ent_acc + ej * kEntVals + k, bad); }
+    if (go.entry_loss) {
+      go.entry_loss[e * 2 + 0] = fix_get(ws.ent_acc + ei * kEntVals + 12, bad);
+      go.entry_loss[e * 2 + 1] = fix_get(ws.ent_acc + ej * kEntVals + 12, bad);
+    }
+    load_row(ws.geomE + int64_t(e) * kGeomE, c);
+    coupl += edge_grad(D, L, e, si, sj, c, go.small_grad);
+  }
+  for (int r = 0, i = img_of_thread(0); i < n; i = img_of_thread(++r)) {
+    float S[kImgVals], c[kGeomI];
+#pragma unroll
+    for (int k = 0; k < kImgVals; ++k) S[k] = fix_get(ws.img_acc + i * kImgVals + k, bad);
+    load_row(ws.geomI + int64_t(i) * kGeomI, c);
+    image_grad(D, L, i, S, c, go.small_grad);
+  }
+  fix_report(bad, ws.flags);
+  // every accumulator has been read (barrier inside block_sum8): fold in the coupling, clear for the next launch
+  const float coupling = block_sum8(coupl, s_red + 16) / float(E);
+  if (D.norm_pw_scale)
+    for (int e = threadIdx.x; e < E; e += blockDim.x) go.small_grad[L.pw + e * 8 + 7] -= coupling;   // written by this thread above
+  for (int k = threadIdx.x; k < 2 * E * kEntVals; k += blockDim.x) ws.ent_acc[k] = 0;
+  for (int k = threadIdx.x; k < n * kImgVals; k += blockDim.x) ws.img_acc[k] = 0;
+}
+
 // ---- latency-optimised small-parameter step for graphs with one thread per edge / per image (E, n <= blockDim) ----
 // The tail of a 60-microsecond iteration is bound by the dependent instruction chain of whichever thread does the most,
 // so the work is cut three ways:
@@ -579,21 +630,40 @@ static __device__ __forceinline__ void small_step(const d3r_align_desc& D, const
 // last CTA is still in its small-parameter step; the kernels call pdl::sync_with_predecessor() before they read what that
 // step wrote.  The shared-memory opt-in is a per-device function attribute (a process may drive several GPUs), so it is
 // set on every call; two CTAs per SM need the maximum carve-out.
-static int launch_iterations(void (*kernel)(d3r_align_desc, int), const d3r_align_desc* desc, int grid, int threads, size_t smem,
-                             int it_begin, int it_end, cudaStream_t st) {
+template <typename Arg>
+static int alignment_launch_config(void (*kernel)(d3r_align_desc, Arg), int grid, int threads, size_t smem, cudaStream_t st,
+                                   cudaLaunchConfig_t& cfg, cudaLaunchAttribute& at) {
   D3R_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   D3R_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
-  cudaLaunchConfig_t cfg = {};
+  cfg = {};
   cfg.gridDim = dim3((unsigned)grid);
   cfg.blockDim = dim3((unsigned)threads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at;
+  at.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  at.val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = &at;
   cfg.numAttrs = 1;
+  return D3R_OK;
+}
+
+static int launch_iterations(void (*kernel)(d3r_align_desc, int), const d3r_align_desc* desc, int grid, int threads, size_t smem,
+                             int it_begin, int it_end, cudaStream_t st) {
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute at;
+  if (int rc = alignment_launch_config(kernel, grid, threads, smem, st, cfg, at)) return rc;
   for (int it = it_begin; it < it_end; ++it) D3R_CUDA(cudaLaunchKernelEx(&cfg, kernel, *desc, it));
+  D3R_LAUNCH_CHECK();
+  return D3R_OK;
+}
+
+// One launch of a gradient-export kernel (same launch attributes as an iteration).
+static int launch_gradient(void (*kernel)(d3r_align_desc, GradOut), const d3r_align_desc* desc, int grid, int threads, size_t smem,
+                           const GradOut& go, cudaStream_t st) {
+  cudaLaunchConfig_t cfg;
+  cudaLaunchAttribute at;
+  if (int rc = alignment_launch_config(kernel, grid, threads, smem, st, cfg, at)) return rc;
+  D3R_CUDA(cudaLaunchKernelEx(&cfg, kernel, *desc, go));
   D3R_LAUNCH_CHECK();
   return D3R_OK;
 }

@@ -80,9 +80,11 @@ __device__ __forceinline__ float butterfly16(float (&v)[kRedVals], int lane) {
   return v[0];
 }
 
-template <bool kL2, int PPT>
-__global__ void __launch_bounds__(kThreads, 2)
-align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
+// Body of both instantiation families: kGrad = false is the training iteration (align_iter_kernel), kGrad = true the
+// gradient export (align_grad_kernel): the depth stage writes dL/dlog-depth to go.logd_grad instead of running Adam, and
+// the last CTA runs small_grad_step.
+template <bool kGrad, bool kL2, int PPT>
+__device__ __forceinline__ void iter_body(const d3r_align_desc& D, int it, const GradOut& go) {
   constexpr int kSlots = PPT * kThreads;     // pixel slots of this instantiation (>= chunk_px)
   extern __shared__ __align__(128) uint8_t s_dyn[];
   float4* s_obs = reinterpret_cast<float4*>(s_dyn);                                   // [kStages][kSlots]
@@ -238,8 +240,8 @@ align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
   float S[kRedVals];
 #pragma unroll
   for (int k = 0; k < kRedVals; ++k) S[k] = 0.f;
-  if (!D.eval_only) {
-    const float step_size = D.sched[it * 4 + 1], bc2s = D.sched[it * 4 + 2];
+  if (kGrad || !D.eval_only) {
+    const float step_size = kGrad ? 0.f : D.sched[it * 4 + 1], bc2s = kGrad ? 1.f : D.sched[it * 4 + 2];
 #pragma unroll
     for (int k = 0; k < PPT; ++k) {
       const int q = tid + k * kThreads;
@@ -251,11 +253,15 @@ align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
         const float c0 = d * (float(u) - cx) * ifx, c1 = d * (float(v) - cy) * ify;
         // dX/dlogd = R c  (c is linear in d)
         const float gd = G[k][0] * (X[k][0] - T[0]) + G[k][1] * (X[k][1] - T[1]) + G[k][2] * (X[k][2] - T[2]);
-        float m = D.logd_m[poff + p], vv = D.logd_v[poff + p];
-        const float nld = adam_update(ld, gd, m, vv, D.beta1, D.beta2, step_size, bc2s, D.adam_eps);
-        D.logd[poff + p] = nld;
-        D.logd_m[poff + p] = m;
-        D.logd_v[poff + p] = vv;
+        if (kGrad) {
+          go.logd_grad[poff + p] = gd;
+        } else {
+          float m = D.logd_m[poff + p], vv = D.logd_v[poff + p];
+          const float nld = adam_update(ld, gd, m, vv, D.beta1, D.beta2, step_size, bc2s, D.adam_eps);
+          D.logd[poff + p] = nld;
+          D.logd_m[poff + p] = m;
+          D.logd_v[poff + p] = vv;
+        }
         S[0] += G[k][0] * c0; S[1] += G[k][0] * c1; S[2] += G[k][0] * d;
         S[3] += G[k][1] * c0; S[4] += G[k][1] * c1; S[5] += G[k][1] * d;
         S[6] += G[k][2] * c0; S[7] += G[k][2] * c1; S[8] += G[k][2] * d;
@@ -277,7 +283,7 @@ align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
   }
   if (dbg && tid == 0) dbg[1] = gtime();
 
-  prefetch_small_step_inputs(D, ws, it, int((size_t(kStages) * PPT * kThreads * sizeof(float4)) / 4), tid, kThreads);
+  if (!kGrad) prefetch_small_step_inputs(D, ws, it, int((size_t(kStages) * PPT * kThreads * sizeof(float4)) / 4), tid, kThreads);
   // ---- grid ticket: the last CTA to finish runs the small-parameter step ----
   __syncthreads();
   if (tid == 0) s_flag = (grid_ticket(D.counters) == int(gridDim.x) - 1);
@@ -288,8 +294,23 @@ align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
   }
   if (tid == 0) D.counters[0] = 0;   // re-arm for the next launch
   if (dbg && tid == 0) dbg[2] = gtime();
-  small_step(D, ws, it, s_red, reinterpret_cast<float*>(s_dyn), int((size_t(kStages) * PPT * kThreads * sizeof(float4)) / 4));
+  if (kGrad)
+    small_grad_step(D, ws, go, s_red);
+  else
+    small_step(D, ws, it, s_red, reinterpret_cast<float*>(s_dyn), int((size_t(kStages) * PPT * kThreads * sizeof(float4)) / 4));
   if (dbg && tid == 0) dbg[3] = gtime();
+}
+
+template <bool kL2, int PPT>
+__global__ void __launch_bounds__(kThreads, 2)
+align_iter_kernel(const __grid_constant__ d3r_align_desc D, int it) {
+  iter_body<false, kL2, PPT>(D, it, GradOut{});
+}
+
+template <bool kL2, int PPT>
+__global__ void __launch_bounds__(kThreads, 2)
+align_grad_kernel(const __grid_constant__ d3r_align_desc D, GradOut go) {
+  iter_body<true, kL2, PPT>(D, 0, go);
 }
 
 __global__ void __launch_bounds__(kThreads) pts3d_kernel(const __grid_constant__ d3r_align_desc D, float* out) {
@@ -317,7 +338,7 @@ __global__ void __launch_bounds__(kThreads) pts3d_kernel(const __grid_constant__
 }  // namespace d3r
 
 namespace d3r { namespace align {
-int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, cudaStream_t st);
+int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, const GradOut* go, cudaStream_t st);
 int stream_set_debug(unsigned long long* p);
 } }
 
@@ -335,12 +356,13 @@ extern "C" int d3r_sizeof_align_desc(void) { return (int)sizeof(d3r_align_desc);
 
 extern "C" int64_t d3r_align_workspace_floats(int32_t n_imgs, int32_t n_edges) { return workspace_floats(n_imgs, n_edges); }
 
-static int validate(const d3r_align_desc* d) {
+// optimizer_state: the call reads the Adam moments, the trainable flags and the schedule (everything but a gradient launch)
+static int validate(const d3r_align_desc* d, bool optimizer_state = true) {
   D3R_CHECK_ARG(d != nullptr, "d3r_align: null descriptor");
   D3R_CHECK_ARG(d->n_imgs > 0 && d->n_edges > 0 && d->n_entries == 2 * d->n_edges, "d3r_align: bad sizes");
   D3R_CHECK_ARG(d->n_chunks > 0 && d->max_chunks > 0 && d->max_deg > 0, "d3r_align: bad chunking");
-  D3R_CHECK_ARG(d->obs && d->logd && d->logd_m && d->logd_v && d->small && d->small_m && d->small_v &&
-                    d->small_trainable && d->workspace && d->sched && d->loss_out && d->counters,
+  D3R_CHECK_ARG(d->obs && d->logd && d->small && d->workspace && d->loss_out && d->counters, "d3r_align: null buffer");
+  D3R_CHECK_ARG(!optimizer_state || (d->logd_m && d->logd_v && d->small_m && d->small_v && d->small_trainable && d->sched),
                 "d3r_align: null buffer");
   D3R_CHECK_ARG(d->chunk_px > 0 && d->chunk_px <= kChunk, "d3r_align: chunk_px=%d must be in [1, %d]", d->chunk_px, kChunk);
   return D3R_OK;
@@ -354,20 +376,22 @@ extern "C" int d3r_align_prepare(const d3r_align_desc* desc, void* stream) {
   return D3R_OK;
 }
 
+// go == nullptr: iterations [it_begin, it_end); otherwise one gradient launch
 template <bool kL2, int PPT>
-static int launch_iters(const d3r_align_desc* desc, int it_begin, int it_end, cudaStream_t st) {
+static int launch_iters(const d3r_align_desc* desc, int it_begin, int it_end, const GradOut* go, cudaStream_t st) {
   const size_t smem = size_t(kStages) * PPT * kThreads * sizeof(float4) + size_t(kEntTile) * kWarps * kEntVals * sizeof(float);
+  if (go) return launch_gradient(align_grad_kernel<kL2, PPT>, desc, desc->n_chunks, kThreads, smem, *go, st);
   return launch_iterations(align_iter_kernel<kL2, PPT>, desc, desc->n_chunks, kThreads, smem, it_begin, it_end, st);
 }
 
 template <bool kL2>
-static int launch_ppt(const d3r_align_desc* desc, int it_begin, int it_end, cudaStream_t st) {
+static int launch_ppt(const d3r_align_desc* desc, int it_begin, int it_end, const GradOut* go, cudaStream_t st) {
   const int ppt = (desc->chunk_px + kThreads - 1) / kThreads;   // pixel slots per thread this problem needs
-  if (ppt <= 4) return launch_iters<kL2, 4>(desc, it_begin, it_end, st);
-  if (ppt == 5) return launch_iters<kL2, 5>(desc, it_begin, it_end, st);
-  if (ppt == 6) return launch_iters<kL2, 6>(desc, it_begin, it_end, st);
-  if (ppt == 7) return launch_iters<kL2, 7>(desc, it_begin, it_end, st);
-  return launch_iters<kL2, 8>(desc, it_begin, it_end, st);
+  if (ppt <= 4) return launch_iters<kL2, 4>(desc, it_begin, it_end, go, st);
+  if (ppt == 5) return launch_iters<kL2, 5>(desc, it_begin, it_end, go, st);
+  if (ppt == 6) return launch_iters<kL2, 6>(desc, it_begin, it_end, go, st);
+  if (ppt == 7) return launch_iters<kL2, 7>(desc, it_begin, it_end, go, st);
+  return launch_iters<kL2, 8>(desc, it_begin, it_end, go, st);
 }
 
 extern "C" int d3r_align_run(const d3r_align_desc* desc, int32_t it_begin, int32_t it_end, void* stream) {
@@ -379,9 +403,21 @@ extern "C" int d3r_align_run(const d3r_align_desc* desc, int32_t it_begin, int32
     D3R_CUDA(cudaMemsetAsync(ws0.flags, 0, sizeof(int), (cudaStream_t)stream));
   }
   prof::Scope scope(desc->stream_kernel ? "align_stream" : "align_iter", (cudaStream_t)stream, 0.0, 0.0, it_end - it_begin);
-  if (desc->stream_kernel) return launch_stream(desc, it_begin, it_end, (cudaStream_t)stream);
-  return desc->dist_l2 ? launch_ppt<true>(desc, it_begin, it_end, (cudaStream_t)stream)
-                       : launch_ppt<false>(desc, it_begin, it_end, (cudaStream_t)stream);
+  if (desc->stream_kernel) return launch_stream(desc, it_begin, it_end, nullptr, (cudaStream_t)stream);
+  return desc->dist_l2 ? launch_ppt<true>(desc, it_begin, it_end, nullptr, (cudaStream_t)stream)
+                       : launch_ppt<false>(desc, it_begin, it_end, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_align_loss_grad(const d3r_align_desc* desc, float* logd_grad, float* small_grad, float* entry_loss, void* stream) {
+  int rc = validate(desc, false);
+  if (rc) return rc;
+  D3R_CHECK_ARG(logd_grad && small_grad, "d3r_align_loss_grad: null gradient buffer");
+  const Workspace ws0 = carve(desc->workspace, desc->n_imgs, desc->n_edges);
+  D3R_CUDA(cudaMemsetAsync(ws0.flags, 0, sizeof(int), (cudaStream_t)stream));   // the overflow flag reports on this launch
+  prof::Scope scope("align_grad", (cudaStream_t)stream, 0.0, 0.0, 1);
+  const GradOut go{logd_grad, small_grad, entry_loss};
+  if (desc->stream_kernel) return launch_stream(desc, 0, 1, &go, (cudaStream_t)stream);
+  return desc->dist_l2 ? launch_ppt<true>(desc, 0, 1, &go, (cudaStream_t)stream) : launch_ppt<false>(desc, 0, 1, &go, (cudaStream_t)stream);
 }
 
 /* 1 if a fixed-point accumulator overflowed (|partial sum| >= 2^18) since the flag was last cleared. */

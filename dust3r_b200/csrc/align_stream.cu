@@ -95,7 +95,7 @@ __device__ __forceinline__ float warp_transpose_sum(const float (&a)[NV], float*
 // including the instructions and inputs of the small-parameter step, which one CTA then re-fetches from DRAM on the critical
 // path.  Among themselves evict_first lines still age in order, so the reversed traversal of odd iterations keeps finding the
 // tail of the previous pass.
-template <int PPT, int NST>
+template <bool kGrad, int PPT, int NST>
 __device__ __forceinline__ void produce_next(const d3r_align_desc& D, const Workspace& ws, const d3r_align_item* item_tab,
                                              ProdState* ps, uint8_t* ring, uint64_t* full) {
   constexpr int kStage = kHdrBytes + PPT * kSlotBytes;
@@ -131,6 +131,11 @@ __device__ __forceinline__ void produce_next(const d3r_align_desc& D, const Work
     ps->row = row + kEdgeT;
     ps->obs = obs + ps->slab_units;
     ps->phase = phase + 1;
+  } else if (kGrad) {                               // MV of a gradient launch: image row only
+    ptx::mbar_arrive_expect_tx(bar, 64u);
+    ptx::bulk_g2s(dst, ps->irow, 64u, bar);
+    ps->item = item + 1;
+    ps->phase = 0;
   } else {                                           // MV: image row | log-depth | exp_avg | exp_avg_sq
     const uint32_t px_bytes = ps->px_bytes;
     const int64_t pix0 = ps->pix0;
@@ -221,10 +226,11 @@ __device__ __forceinline__ void entry_slots(const uint8_t* slot, int lane, const
   for (int v = 0; v < kEntVals; ++v) { float lo, hi; unpack2(acc[v], lo, hi); a13[v] = lo + hi; }
 }
 
-template <int NS, int PPT>
+// kGrad: gd goes to logd_grad (gradient launch) instead of into the Adam update; the image sums are the same
+template <bool kGrad, int NS, int PPT>
 __device__ __forceinline__ void adam_slots(const d3r_align_desc& D, const uint8_t* slot, int lane, int npx, int64_t pix0,
                                            float step_size, float inv_bc2s, const f2 (&X)[PPT][3], const f2 (&G)[PPT][3],
-                                           float (&s12)[kImgVals]) {
+                                           float* logd_grad, float (&s12)[kImgVals]) {
   const float4 i2 = reinterpret_cast<const float4*>(slot)[2];   // R8 T0 T1 T2
   const float2* ldp = reinterpret_cast<const float2*>(slot + kHdrBytes);
   const float2* mp = reinterpret_cast<const float2*>(slot + kHdrBytes + PPT * 256);
@@ -243,6 +249,10 @@ __device__ __forceinline__ void adam_slots(const d3r_align_desc& D, const uint8_
       S[3] = fma2(G[kk][1], y0, S[3]); S[4] = fma2(G[kk][1], y1, S[4]); S[5] = fma2(G[kk][1], y2, S[5]);
       S[6] = fma2(G[kk][2], y0, S[6]); S[7] = fma2(G[kk][2], y1, S[7]); S[8] = fma2(G[kk][2], y2, S[8]);
       S[9] = add2(S[9], G[kk][0]); S[10] = add2(S[10], G[kk][1]); S[11] = add2(S[11], G[kk][2]);
+      if (kGrad) {
+        reinterpret_cast<f2*>(logd_grad + pix0)[j] = gd;
+        continue;
+      }
       const float2 ld = ldp[j], mm = mp[j], vv = vp[j];
       // torch.optim.Adam: m += (1-b1)(g-m); v = v*b2 + (1-b2) g g; p -= step * m / (sqrt(v)/sqrt(bc2) + eps)
       const f2 m_old = pack2(mm.x, mm.y);
@@ -264,9 +274,11 @@ __device__ __forceinline__ void adam_slots(const d3r_align_desc& D, const uint8_
   for (int v = 0; v < kImgVals; ++v) { float lo, hi; unpack2(S[v], lo, hi); s12[v] = lo + hi; }
 }
 
-template <bool kL2, int PPT, int NST>
-__global__ void __launch_bounds__(kSThreads, 2)
-align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
+// Body of both instantiation families: kGrad = false is the training iteration (align_stream_kernel), kGrad = true the
+// gradient export (align_stream_grad_kernel): its MV stage brings only the image row, writes dL/dlog-depth to go.logd_grad
+// and still forms the image sums; the last CTA runs small_grad_step.
+template <bool kGrad, bool kL2, int PPT, int NST>
+__device__ __forceinline__ void stream_body(const d3r_align_desc& D, int it, const GradOut& go) {
   static_assert(PPT == 3, "the per-slot specialisations below are written for 3 slots per item");
   constexpr int kStage = kHdrBytes + PPT * kSlotBytes;
   extern __shared__ __align__(128) uint8_t s_dyn[];
@@ -306,12 +318,12 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
   pdl::sync_with_predecessor();
   if (dbg && lane == 0) dbg[1] = gtime();
   if (lane == 0)
-    for (int s = 0; s < NST; ++s) produce_next<PPT, NST>(D, ws, item_tab, ps, ring, full);
+    for (int s = 0; s < NST; ++s) produce_next<kGrad, PPT, NST>(D, ws, item_tab, ps, ring, full);
   __syncwarp();
 
-  const float step_size = D.sched[it * 4 + 1];
-  const float inv_bc2s = 1.f / D.sched[it * 4 + 2];
-  const bool train = !D.eval_only;
+  const float step_size = kGrad ? 0.f : D.sched[it * 4 + 1];
+  const float inv_bc2s = kGrad ? 1.f : 1.f / D.sched[it * 4 + 2];
+  const bool train = kGrad || !D.eval_only;
 
   int si = 0;                           // ring slot of the next stage to consume
   uint32_t par = 0;                     // its mbarrier phase parity
@@ -351,7 +363,7 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
     else if (nslots == 2) unproject_slots<2, PPT>(slot, lane, npx, X, G);
     else unproject_slots<1, PPT>(slot, lane, npx, X, G);
     __syncwarp();
-    if (lane == 0) produce_next<PPT, NST>(D, ws, item_tab, ps, ring, full);
+    if (lane == 0) produce_next<kGrad, PPT, NST>(D, ws, item_tab, ps, ring, full);
     advance();
 
     if (simg != img) { flush_image(); simg = img; }
@@ -379,7 +391,7 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
       if (!(lane & 1) && lane < 2 * kEntVals) s_acc[kin * kEntVals + (lane >> 1)] += tot;
       ptx::fence_proxy_async();
       __syncwarp();
-      if (lane == 0) produce_next<PPT, NST>(D, ws, item_tab, ps, ring, full);
+      if (lane == 0) produce_next<kGrad, PPT, NST>(D, ws, item_tab, ps, ring, full);
       advance();
     }
 
@@ -388,16 +400,16 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
     ptx::mbar_wait_bounded(smem_u32(&full[si]), par);
     if (train) {
       float s12[kImgVals];
-      if (nslots == 3) adam_slots<3, PPT>(D, slot, lane, npx, pix0, step_size, inv_bc2s, X, G, s12);
-      else if (nslots == 2) adam_slots<2, PPT>(D, slot, lane, npx, pix0, step_size, inv_bc2s, X, G, s12);
-      else adam_slots<1, PPT>(D, slot, lane, npx, pix0, step_size, inv_bc2s, X, G, s12);
+      if (nslots == 3) adam_slots<kGrad, 3, PPT>(D, slot, lane, npx, pix0, step_size, inv_bc2s, X, G, go.logd_grad, s12);
+      else if (nslots == 2) adam_slots<kGrad, 2, PPT>(D, slot, lane, npx, pix0, step_size, inv_bc2s, X, G, go.logd_grad, s12);
+      else adam_slots<kGrad, 1, PPT>(D, slot, lane, npx, pix0, step_size, inv_bc2s, X, G, go.logd_grad, s12);
       __syncwarp();
       const float tot = warp_transpose_sum<kImgVals>(s12, reinterpret_cast<float*>(slot + kHdrBytes), lane);
       if (!(lane & 1) && lane < 2 * kImgVals) s_img[lane >> 1] += tot;
       ptx::fence_proxy_async();
     }
     __syncwarp();
-    if (lane == 0) produce_next<PPT, NST>(D, ws, item_tab, ps, ring, full);
+    if (lane == 0) produce_next<kGrad, PPT, NST>(D, ws, item_tab, ps, ring, full);
     advance();
     if (deg > Wn) flush_entries();        // a spilled image starts its next item from window 0 again
   }
@@ -405,7 +417,7 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
   flush_image();
   if (dbg && lane == 0) dbg[2] = gtime();
   const int scr_floats = int(size_t(kSWarps) * per_warp / 4);
-  if (warp == 0) prefetch_small_step_inputs(D, ws, it, scr_floats, lane, 32);
+  if (!kGrad && warp == 0) prefetch_small_step_inputs(D, ws, it, scr_floats, lane, 32);
 
   // ---- grid ticket: the last CTA to finish runs the small-parameter step ----
   __syncthreads();
@@ -415,8 +427,23 @@ align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
   if (!s_flag) return;
   if (tid == 0) D.counters[0] = 0;   // re-arm for the next launch
   // every stage this CTA issued has been consumed: the ring is idle and serves as the small step's scratch
-  small_step(D, ws, it, s_red, reinterpret_cast<float*>(s_dyn), scr_floats);
+  if (kGrad)
+    small_grad_step(D, ws, go, s_red);
+  else
+    small_step(D, ws, it, s_red, reinterpret_cast<float*>(s_dyn), scr_floats);
   D3R_TSTAMP(5);
+}
+
+template <bool kL2, int PPT, int NST>
+__global__ void __launch_bounds__(kSThreads, 2)
+align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
+  stream_body<false, kL2, PPT, NST>(D, it, GradOut{});
+}
+
+template <bool kL2, int PPT, int NST>
+__global__ void __launch_bounds__(kSThreads, 2)
+align_stream_grad_kernel(const __grid_constant__ d3r_align_desc D, GradOut go) {
+  stream_body<true, kL2, PPT, NST>(D, 0, go);
 }
 
 // ---- one launch packs every entry (device-resident forward output -> observation layout) ----------------------
@@ -469,7 +496,8 @@ size_t stream_smem_bytes(int ppt, int nst, int window) {
   return size_t(kSWarps) * (size_t(nst) * (kHdrBytes + ppt * kSlotBytes) + size_t(acc_floats) * 4);
 }
 
-int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, cudaStream_t st) {
+// go == nullptr: iterations [it_begin, it_end); otherwise one gradient launch
+int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, const GradOut* go, cudaStream_t st) {
   D3R_CHECK_ARG(desc->items && desc->warp_item_ptr && desc->n_items > 0 && desc->stream_grid > 0,
                 "d3r_align_run: streaming kernel selected without a work-item table");
   D3R_CHECK_ARG(desc->stream_ppt == 3, "d3r_align_run: stream_ppt=%d is not built (3)", desc->stream_ppt);
@@ -479,10 +507,15 @@ int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, cudaStre
   const bool deep = stream_smem_bytes(3, 4, desc->stream_window) <= budget;
   D3R_CHECK_ARG(deep || stream_smem_bytes(3, 3, desc->stream_window) <= budget, "d3r_align_run: stream_window=%d does not fit shared memory",
                 desc->stream_window);
+  const size_t smem = stream_smem_bytes(3, deep ? 4 : 3, desc->stream_window);
+  if (go) {
+    void (*kernel)(d3r_align_desc, GradOut) = desc->dist_l2 ? (deep ? align_stream_grad_kernel<true, 3, 4> : align_stream_grad_kernel<true, 3, 3>)
+                                                            : (deep ? align_stream_grad_kernel<false, 3, 4> : align_stream_grad_kernel<false, 3, 3>);
+    return launch_gradient(kernel, desc, desc->stream_grid, kSThreads, smem, *go, st);
+  }
   void (*kernel)(d3r_align_desc, int) = desc->dist_l2 ? (deep ? align_stream_kernel<true, 3, 4> : align_stream_kernel<true, 3, 3>)
                                                       : (deep ? align_stream_kernel<false, 3, 4> : align_stream_kernel<false, 3, 3>);
-  return launch_iterations(kernel, desc, desc->stream_grid, kSThreads, stream_smem_bytes(3, deep ? 4 : 3, desc->stream_window),
-                           it_begin, it_end, st);
+  return launch_iterations(kernel, desc, desc->stream_grid, kSThreads, smem, it_begin, it_end, st);
 }
 
 }  // namespace align

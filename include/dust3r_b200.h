@@ -166,6 +166,15 @@ int64_t d3r_align_workspace_floats(int32_t n_imgs, int32_t n_edges);
 int d3r_align_prepare(const d3r_align_desc* desc, void* stream);
 /* Runs iterations [it_begin, it_end) (indices into sched / loss_out).  Asynchronous. */
 int d3r_align_run(const d3r_align_desc* desc, int32_t it_begin, int32_t it_end, void* stream);
+/* Objective and its gradient at the current parameters (net.forward() + loss.backward()): one launch of the pixel kernel
+ * the descriptor selects + the last-CTA small step.  Updates no parameter or Adam moment; reads neither sched nor the moments
+ * (logd_m, logd_v, small_m, small_v, small_trainable and sched may be NULL).  Call d3r_align_prepare first when `small` changed.
+ * loss -> desc->loss_out[0] (bit-identical to an eval_only run).  logd_grad [sum stride_i]: dL/dlog-depth (padding pixels are
+ * not written: pass a zeroed buffer).  small_grad [11n+10E]: dL/d(raw parameter) in the `small` layout, complete: log-scale
+ * mean coupling and adaptor mean removal folded in; with tied focals both focal slots hold the full dL/dfocal.  Gradients of
+ * every parameter, whatever small_trainable says.  entry_loss (may be NULL) [E][2]: coefficient-weighted loss of (edge, side).
+ * Sets the overflow flag like a run; leaves the accumulators cleared, so a following d3r_align_run is unaffected. */
+int d3r_align_loss_grad(const d3r_align_desc* desc, float* logd_grad, float* small_grad, float* entry_loss, void* stream);
 /* Cross-CTA sums use order-independent 2^40 fixed-point integer atomics (bit-reproducible).  *host_out = 1 when a
  * partial sum (|x| >= 2^18) or a total (|x| >= 2^22) left the supported range (unreasonably scaled scene, NaN / Inf input)
  * since iteration 0 of the current d3r_align_run batch. */
