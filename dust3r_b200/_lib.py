@@ -81,6 +81,10 @@ def _declare(lib):
     lib.d3r_image_resize_crop_normalize.restype = C.c_int
     lib.d3r_image_resize_crop_normalize.argtypes = [vp, i32, i32, i32, i32, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32,
                                                     vp, vp, vp, vp]
+    lib.d3r_segment_sky_workspace_bytes.restype = i64
+    lib.d3r_segment_sky_workspace_bytes.argtypes = [i32, i64]
+    lib.d3r_segment_sky.restype = C.c_int
+    lib.d3r_segment_sky.argtypes = [i32, vp, vp, i32, i64, vp, vp, vp, i64, vp]
     for name in ('d3r_sizeof_align_item', 'd3r_sizeof_pack_entry', 'd3r_align_stream_slots_per_item',
                  'd3r_align_stream_warps_per_cta', 'd3r_align_stream_max_window'):
         getattr(lib, name).restype = C.c_int

@@ -16,10 +16,12 @@ from torch.autograd.function import once_differentiable
 
 from ..utils.geometry import inv
 from ..utils.image import rgb
+from ..viz import segment_sky
 from . import pose_param
 from .commons import ALL_DISTS, NoGradParamDict, edge_str, get_conf_trf, get_imshapes
 from .engine import AlignEngine
 from .pointcloud_filter import clean_pointcloud
+from .scene_ops import segment_sky_host_images
 
 
 class BasePCOptimizer(nn.Module):
@@ -313,7 +315,20 @@ class BasePCOptimizer(nn.Module):
 
     @torch.no_grad()
     def mask_sky(self):
-        raise NotImplementedError('sky segmentation (viz) is outside the two hot paths')
+        """base_opt.py:289-295: a copy of the scene whose im_conf is 0 on the sky pixels of every image (viz.segment_sky); the
+        scene itself is left as it is.  On a CUDA scene one batched kernel call segments all images.  The copy does not share
+        the alignment engine: it builds its own when it is next aligned."""
+        if self.imgs is None:
+            raise ValueError('mask_sky needs the images: build the scene from views that carry "img"')
+        res = deepcopy(self, {id(self.__dict__.get('_engine')): None})    # the memo entry copies the engine as None
+        res._engine = None
+        if self.device.type == 'cuda':
+            skies = segment_sky_host_images(self.imgs, self.device)
+        else:
+            skies = [segment_sky(img) for img in self.imgs]
+        for conf, sky in zip(res.im_conf, skies):
+            conf[sky.to(conf.device)] = 0
+        return res
 
     def show(self, *a, **kw):
         raise NotImplementedError('visualisation is outside the two hot paths (SURVEY §2 #14)')

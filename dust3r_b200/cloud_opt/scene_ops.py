@@ -5,6 +5,7 @@ csrc/scene_ops.cu.  Each takes CUDA fp32 tensors on an H100 and mirrors the host
   rigid_registration    cloud_opt/commons.py             (roma.rigid_points_registration as used by init_im_poses.py)
   weiszfeld_focal       post_process.py                  (dust3r/post_process.py:12-60)
   nearest_neighbours    utils/geometry.py                (find_reciprocal_matches, dust3r/utils/geometry.py:345-361)
+  segment_sky           viz.py                           (dust3r/viz.py:345-381, csrc/sky_ops.cu)
 
 The host ports dispatch here when their inputs live on the GPU; CPU tensors keep the reference's own CPU algorithms (as the
 reference does: these run once per scene, not per iteration)."""
@@ -113,3 +114,56 @@ def nearest_neighbours(queries, points):
     with torch.cuda.device(dev):
         _lib.check(lib.d3r_nearest_neighbours(int(q.shape[0]), int(p.shape[0]), q.data_ptr(), p.data_ptr(), nn.data_ptr(), _stream(dev)))
     return nn.long()
+
+
+def _quantise(x):
+    """np.uint8(255 * x.clip(0, 1)) as numpy computes it (product in x's dtype, truncation toward zero); uint8 passes through."""
+    return x if x.dtype == torch.uint8 else (255 * x.clamp(0, 1)).to(torch.uint8)
+
+
+def _segment_sky_u8(rgb, shapes):
+    """rgb: flat uint8 CUDA tensor holding the (H, W, 3) images of `shapes` back to back -> list of (H, W) bool masks."""
+    dev = rgb.device
+    _lib.require_cuda_device(dev)
+    lib = _lib.get_lib()
+    n = len(shapes)
+    areas = [h * w for h, w in shapes]
+    off = np.zeros(n + 1, dtype=np.int64)
+    off[1:] = np.cumsum(areas)
+    total = int(off[-1])
+    assert rgb.numel() == 3 * total and rgb.dtype == torch.uint8
+    hw = torch.tensor(shapes, dtype=torch.int32, device=dev)
+    offd = torch.from_numpy(off[:n]).to(dev)
+    out = torch.empty((total,), dtype=torch.uint8, device=dev)
+    ws = torch.empty((int(lib.d3r_segment_sky_workspace_bytes(n, total)),), dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        _lib.check(lib.d3r_segment_sky(n, hw.data_ptr(), offd.data_ptr(), int(max(areas)), total, rgb.data_ptr(), out.data_ptr(),
+                                       ws.data_ptr(), ws.numel(), _stream(dev)))
+    sky = out.view(torch.bool)
+    return [sky[off[i]:off[i + 1]].view(shapes[i]) for i in range(n)]
+
+
+@torch.no_grad()
+def segment_sky(images):
+    """List of (H, W, 3) RGB CUDA tensors (float in [0, 1] as scene.imgs holds them, or uint8; any mix of sizes) -> list of (H, W)
+    bool sky masks on the device, one batched call (dust3r/viz.py:345-381, bit-exact)."""
+    if not images:
+        return []
+    shapes = [tuple(x.shape[:2]) for x in images]
+    assert all(x.ndim == 3 and x.shape[2] == 3 for x in images), 'segment_sky takes (H, W, 3) RGB images'
+    rgb = torch.cat([_quantise(x).reshape(-1) for x in images])
+    return _segment_sky_u8(rgb, shapes)
+
+
+@torch.no_grad()
+def segment_sky_host_images(images, device):
+    """Like segment_sky for (H, W, 3) float32 numpy arrays in host memory (scene.imgs): the floats go up in one pinned copy and are
+    quantised on the device."""
+    if any(np.asarray(x).dtype != np.float32 for x in images):     # other dtypes are quantised in their own precision
+        return segment_sky([torch.from_numpy(np.asarray(x)).to(device) for x in images])
+    shapes = [tuple(x.shape[:2]) for x in images]
+    assert all(x.ndim == 3 and x.shape[2] == 3 for x in images), 'segment_sky takes (H, W, 3) RGB images'
+    total = 3 * sum(h * w for h, w in shapes)
+    host = torch.empty((total,), dtype=torch.float32, pin_memory=True)
+    np.concatenate([np.asarray(x, dtype=np.float32).reshape(-1) for x in images], out=host.numpy())
+    return _segment_sky_u8(_quantise(host.to(device, non_blocking=True)), shapes)

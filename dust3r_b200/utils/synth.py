@@ -145,6 +145,33 @@ def many_ar_inputs(H: int, W: int, seed: int = 9):
             dict(img=img2, true_shape=ts2, instance=['4', '5', '6', '7']))
 
 
+def synth_sky_image(H: int, W: int, seed: int = 0):
+    """An outdoor scene as scene.imgs holds it: float32 (H, W, 3) RGB in [0, 1].  A blue-to-hazy sky with bright clouds above a
+    wavy horizon, textured dark ground below it with a few bright patches, sensor noise everywhere -- input of the sky
+    segmentation tests and benchmark (sky, clouds and bright ground patches give components of many sizes)."""
+    g = _gen(seed, f'sky{H}x{W}')
+    y = torch.linspace(0, 1, H)[:, None]
+    x = torch.linspace(0, 1, W)[None, :]
+    ph = torch.rand((3,), generator=g) * 6.28
+    horizon = 0.45 + 0.1 * torch.sin(6.28 * x + ph[0]) + 0.05 * torch.sin(17 * x + ph[1])
+    t = (y / horizon).clamp(0, 1)[..., None]
+    sky = (1 - t) * torch.tensor([0.25, 0.45, 0.85]) + t * torch.tensor([0.75, 0.8, 0.9])
+    for _ in range(5):      # clouds: soft bright ellipses
+        c = torch.rand((4,), generator=g)
+        d = ((x - c[0]) / (0.05 + 0.15 * c[2])) ** 2 + ((y - 0.3 * c[1]) / (0.02 + 0.05 * c[3])) ** 2
+        sky = sky + 0.5 * torch.exp(-d)[..., None]
+    low = torch.rand((1, 3, max(H // 8, 1), max(W // 8, 1)), generator=g)
+    tex = torch.nn.functional.interpolate(low, size=(H, W), mode='bilinear', align_corners=False)[0].permute(1, 2, 0)
+    ground = torch.tensor([0.3, 0.25, 0.15]) + 0.25 * (tex - 0.5)
+    for _ in range(3):      # bright patches on the ground (walls, snow): sky-coloured but not sky
+        r = torch.rand((4,), generator=g)
+        y0, x0 = int((0.6 + 0.3 * r[0]) * H), int(r[1] * W * 0.8)
+        ground[y0:y0 + 2 + int(r[2] * H * 0.15), x0:x0 + 2 + int(r[3] * W * 0.2)] = 0.92
+    img = torch.where((y < horizon)[..., None], sky, ground)
+    img = img + 0.04 * torch.randn((H, W, 3), generator=g)
+    return img.clamp(0, 1).numpy()
+
+
 def synth_photo(H: int, W: int, seed: int = 0):
     """A decoded 'photograph': uint8 (H, W, 3) numpy array with natural-image statistics (smooth colour fields, a few hard
     edges, sensor noise) -- input of the load_images preprocessing tests (edges and noise exercise the negative lobes and the

@@ -298,6 +298,18 @@ int d3r_image_resize_crop_normalize(const uint8_t* src_dev, int32_t H0, int32_t 
                                     const int32_t* ybounds_dev, const int32_t* ycoefs_dev, int32_t ky, int32_t row0, int32_t rows,
                                     int32_t crop_x0, int32_t crop_y0, int32_t H2, int32_t W2, const float* lut_dev, uint8_t* tmp_dev,
                                     float* out_dev, void* stream);
+/* segment_sky (dust3r/viz.py:345-381, behind BasePCOptimizer.mask_sky, dust3r/cloud_opt/base_opt.py:289-295), bit-exact, for
+ * n images of any mix of sizes in one call (seven launches whatever the content):
+ *   rgb [total_px][3] uint8, image i = pixels [off[i], off[i] + hw[2i] * hw[2i+1]) row-major: the bytes uint8(255 * clip(img, 0, 1))
+ *   -> sky_out [total_px] uint8 0 / 1.  OpenCV's 8-bit HSV of the bytes read as BGR, the reference's colour thresholds, a 5x5
+ *   binary opening with zero padding, 8-connected components; a pixel is sky when its component has 2 * area > the largest
+ *   component's area of its image (none when the opened mask is empty).
+ * max_area = largest hw[2i] * hw[2i+1]; total_px = sum of the image areas (< 2^31); images must not overlap.  sky_out also serves
+ * as scratch during the call.  The workspace (labels, areas, eroded mask, per-image maxima) needs
+ * d3r_segment_sky_workspace_bytes(n_imgs, total_px) bytes (0 for an empty batch) and no initialisation. */
+int64_t d3r_segment_sky_workspace_bytes(int32_t n_imgs, int64_t total_px);
+int d3r_segment_sky(int32_t n_imgs, const int32_t* hw_dev, const int64_t* off_dev, int32_t max_area, int64_t total_px,
+                    const uint8_t* rgb_dev, uint8_t* sky_out_dev, void* workspace_dev, int64_t workspace_bytes, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Path 1 — pairwise forward: replaces AsymmetricCroCo3DStereo.forward (dust3r/model.py:199-211 =
