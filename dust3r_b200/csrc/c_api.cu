@@ -30,7 +30,7 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
 int encode_tensor_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                      const cuuint32_t* box, const char* op) {
+                      const cuuint32_t* box, const char* op, CUtensorMapDataType dtype) {
   static EncodeTiledFn fn = nullptr;
   static std::once_flag once;
   std::call_once(once, [] {
@@ -44,7 +44,7 @@ int encode_tensor_map(CUtensorMap* m, const void* base, int rank, const cuuint64
     return D3R_ERR_CUDA;
   }
   const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, estr,
+  CUresult r = fn(m, dtype, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes, box, estr,
                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {

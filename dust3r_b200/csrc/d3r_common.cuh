@@ -84,10 +84,11 @@ __device__ __forceinline__ void postprocess_pixel(float x, float y, float z, Con
 
 int num_sms();
 
-// Tensor map of a bf16 tensor for TMA loads: 128B swizzle, L2 256B promotion, out-of-bounds elements read as zero.
-// dims[0] is the contiguous dimension; strides_bytes holds the rank - 1 outer strides.  `op` names the caller in errors.
+// Tensor map of a bf16 (or `dtype`) tensor for TMA: 128B swizzle, L2 256B promotion, out-of-bounds elements read as zero
+// and not written.  dims[0] is the contiguous dimension; strides_bytes holds the rank - 1 outer strides.  `op` names the
+// caller in errors.
 int encode_tensor_map(CUtensorMap* m, const void* base, int rank, const cuuint64_t* dims, const cuuint64_t* strides_bytes,
-                      const cuuint32_t* box, const char* op);
+                      const cuuint32_t* box, const char* op, CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
 
 // cudaFuncSetAttribute is per device / context: a launch site keeps one bit per device in a static mask and opts in the first time it
 // launches on each device of the process (a process may drive several GPUs: global_aligner(out, 'cuda:1') next to a model on cuda:0)

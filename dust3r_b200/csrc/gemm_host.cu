@@ -22,11 +22,17 @@ static int g_impl = 2;
 static int g_pair_min_kb = 4;
 static bool use_pair(int bn, int num_kb) { return bn >= 128 && (g_impl == 1 || (g_impl == 2 && num_kb >= g_pair_min_kb)); }
 
-template <int BN, int EPI, bool PAIR>
-static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int m_tiles, int n_tiles, cudaStream_t st) {
+// 0: register-store epilogues everywhere (the bit-identical A/B reference), 1 (default): the specialised epilogues on
+// 128x256 tiles stage their output in shared memory and write it by TMA store / TMA reduce-add, when TMA can address it
+static int g_store = 1;
+
+template <int BN, int EPI, bool PAIR, bool TMA_STORE = false>
+static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const Params& p, int m_tiles, int n_tiles,
+                  cudaStream_t st) {
+  constexpr int kSmem = Cfg<BN, TMA_STORE>::kSmemBytes;
   static unsigned long long attr_devices = 0;
   if (first_launch_on_this_device(attr_devices))
-    D3R_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, EPI, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::kSmemBytes));
+    D3R_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, EPI, PAIR, TMA_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
   int grid;
   if (PAIR) {
     const int items = ((m_tiles + 1) / 2) * n_tiles;
@@ -43,32 +49,46 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const Params& p,
   char detail[96];
   snprintf(detail, sizeof(detail), "M=%d N=%d K=%d flags=0x%x mode=%d epi=%d", p.M, p.N, p.K, (unsigned)p.flags, p.mode, EPI);
   prof::Scope scope(tag, st, 2.0 * double(p.M) * double(p.N) * double(p.K), 0.0, 1, detail);
-  D3R_CUDA(pdl::launch_clustered(gemm_kernel<BN, EPI, PAIR>, dim3(grid), dim3(kNumThreads), size_t(Cfg<BN>::kSmemBytes), st, PAIR ? 2 : 1, ta, tb, p));
+  D3R_CUDA(pdl::launch_clustered(gemm_kernel<BN, EPI, PAIR, TMA_STORE>, dim3(grid), dim3(kNumThreads), size_t(kSmem), st, PAIR ? 2 : 1,
+                                 ta, tb, to, p));
   D3R_LAUNCH_CHECK();
   return D3R_OK;
 }
 
+// `to` != nullptr: the output tensor map of the TMA-store epilogue (BLOCK_N 256, specialised epilogue).  The
+// register-store kernels do not read their output map; they are passed tb in its place.
 template <int BN, bool PAIR>
-static int dispatch_epi(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int m_tiles, int n_tiles, cudaStream_t st) {
-  switch (epi) {
-    case EPI_RESID: return launch<BN, EPI_RESID, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
-    case EPI_ACT: return launch<BN, EPI_ACT, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
-    case EPI_ROPE: return launch<BN, EPI_ROPE, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
+static int dispatch_epi(int epi, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* to, const Params& p, int m_tiles,
+                        int n_tiles, cudaStream_t st) {
+  if constexpr (BN == 256) {
+    if (to) {
+      switch (epi) {
+        case EPI_RESID: return launch<BN, EPI_RESID, PAIR, true>(ta, tb, *to, p, m_tiles, n_tiles, st);
+        case EPI_ACT: return launch<BN, EPI_ACT, PAIR, true>(ta, tb, *to, p, m_tiles, n_tiles, st);
+        case EPI_ROPE: return launch<BN, EPI_ROPE, PAIR, true>(ta, tb, *to, p, m_tiles, n_tiles, st);
+      }
+    }
   }
-  if constexpr (BN == 128) return launch<128, EPI_GENERIC, PAIR>(ta, tb, p, m_tiles, n_tiles, st);
+  switch (epi) {
+    case EPI_RESID: return launch<BN, EPI_RESID, PAIR>(ta, tb, tb, p, m_tiles, n_tiles, st);
+    case EPI_ACT: return launch<BN, EPI_ACT, PAIR>(ta, tb, tb, p, m_tiles, n_tiles, st);
+    case EPI_ROPE: return launch<BN, EPI_ROPE, PAIR>(ta, tb, tb, p, m_tiles, n_tiles, st);
+  }
+  if constexpr (BN == 128) return launch<128, EPI_GENERIC, PAIR>(ta, tb, tb, p, m_tiles, n_tiles, st);
   set_error("no BLOCK_N %d kernel for the generic epilogue", BN);
   return D3R_ERR_INVALID;
 }
 
-static int dispatch(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const Params& p, int m_tiles, cudaStream_t st) {
+static int dispatch(int bn, const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap* to, const Params& p, int m_tiles,
+                    cudaStream_t st) {
   const int n_tiles = (p.N + bn - 1) / bn;
   // epilogue specialisations exist for BLOCK_N 128 and 256 (every hot projection of the two ViTs has N % 256 == 0)
   const int epi = (bn >= 128) ? pick_epi(p.mode, p.flags) : EPI_GENERIC;
   const bool pair = use_pair(bn, p.num_kb);
   switch (bn) {
-    case 256: return pair ? dispatch_epi<256, true>(epi, ta, tb, p, m_tiles, n_tiles, st) : dispatch_epi<256, false>(epi, ta, tb, p, m_tiles, n_tiles, st);
-    case 128: return pair ? dispatch_epi<128, true>(epi, ta, tb, p, m_tiles, n_tiles, st) : dispatch_epi<128, false>(epi, ta, tb, p, m_tiles, n_tiles, st);
-    case 64: return launch<64, EPI_GENERIC, false>(ta, tb, p, m_tiles, n_tiles, st);
+    case 256: return pair ? dispatch_epi<256, true>(epi, ta, tb, to, p, m_tiles, n_tiles, st) : dispatch_epi<256, false>(epi, ta, tb, to, p, m_tiles, n_tiles, st);
+    case 128: return pair ? dispatch_epi<128, true>(epi, ta, tb, nullptr, p, m_tiles, n_tiles, st) : dispatch_epi<128, false>(epi, ta, tb, nullptr, p, m_tiles, n_tiles, st);
+    case 64: return launch<64, EPI_GENERIC, false>(ta, tb, tb, p, m_tiles, n_tiles, st);
   }
   set_error("unsupported BLOCK_N %d", bn);
   return D3R_ERR_INVALID;
@@ -101,7 +121,20 @@ int gemm_bf16(const void* A, long long lda, const void* B, Params p, cudaStream_
   }
   int rc = make_tmap_b(&tb, B, p.N, 1, p.K, bn, p.num_kb, "gemm");
   if (rc) return rc;
-  return dispatch(bn, ta, tb, p, (p.M + BLOCK_M - 1) / BLOCK_M, st);
+  // TMA-store epilogue: [M, N] output boxes of 64 rows x 128 B; TMA needs a 16-byte aligned base and row stride
+  CUtensorMap to;
+  const bool f32 = (p.flags & F_RESID_INPLACE) != 0;
+  const long long row_bytes = p.ldo * (f32 ? 4 : 2);
+  const bool staged = g_store == 1 && bn == 256 && pick_epi(p.mode, p.flags) != EPI_GENERIC && p.ldo >= p.N && row_bytes % 16 == 0 &&
+                      (reinterpret_cast<uintptr_t>(p.out) & 15) == 0;
+  if (staged) {
+    cuuint64_t dims[2] = {(cuuint64_t)p.N, (cuuint64_t)p.M};
+    cuuint64_t str[1] = {(cuuint64_t)row_bytes};
+    cuuint32_t box[2] = {(cuuint32_t)(f32 ? 32 : 64), 64};
+    rc = encode_tensor_map(&to, p.out, 2, dims, str, box, "gemm output", f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16);
+    if (rc) return rc;
+  }
+  return dispatch(bn, ta, tb, staged ? &to : nullptr, p, (p.M + BLOCK_M - 1) / BLOCK_M, st);
 }
 
 int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, int Cin, int Cout, Params p, cudaStream_t st) {
@@ -132,7 +165,7 @@ int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, 
   }
   int rc = make_tmap_b(&tb, w_packed, Cout, 9, Cin, bn, p.num_kb, "conv3x3");
   if (rc) return rc;
-  return dispatch(bn, ta, tb, p, B * p.tiles_x * p.tiles_y, st);
+  return dispatch(bn, ta, tb, nullptr, p, B * p.tiles_x * p.tiles_y, st);
 }
 
 }  // namespace gemm
@@ -143,6 +176,7 @@ using namespace d3r;
 
 extern "C" void d3r_set_gemm_impl(int32_t impl) { gemm::g_impl = impl; }
 extern "C" void d3r_set_gemm_pair_min_kblocks(int32_t kb) { gemm::g_pair_min_kb = kb; }
+extern "C" void d3r_set_gemm_store(int32_t store) { gemm::g_store = store; }
 
 extern "C" int d3r_gemm_bf16(const void* A, const void* B, void* out, const float* bias, const void* add0, void* out2,
                              int32_t M, int32_t N, int32_t K, int64_t ldo, uint32_t flags, const float* rope_cos,

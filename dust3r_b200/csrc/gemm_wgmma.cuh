@@ -7,7 +7,9 @@
 //   warpgroup 0     TMA producer : one elected thread, cp.async.bulk.tensor -> 128B-swizzled smem ring (kStages deep);
 //                                  it runs ahead into the next tile while the consumers drain the current one
 //   warpgroups 1,2  consumers    : wgmma m64 x BLOCK_N x k16 on rows [64 (wg-1), 64 wg) of the 128-row tile, then the
-//                                  fused epilogue straight from the accumulator registers -> global
+//                                  fused epilogue from the accumulator registers -> global, either stored straight
+//                                  from the registers or (TMA_STORE) staged in shared memory and written by TMA while
+//                                  the consumers go on to the next tile
 //
 // CTA pairs (PAIR = true): a cluster of two CTAs works on two M tiles that share one N tile; each CTA loads half of the
 // B tile and multicasts it into both CTAs' shared memory, so B crosses L2 -> SM once per pair.  A ring slot is refilled
@@ -97,12 +99,17 @@ __host__ __device__ inline int pick_epi(int mode, uint32_t flags) {
   return EPI_GENERIC;
 }
 
-template <int BLOCK_N>
+// Shared memory: the ring, then (TMA_STORE) the epilogue's staging buffers, two per consumer warpgroup, each 64 rows of
+// 128 B; then the barriers and (register-store kernels) the head tail's weights, which only EPI_GENERIC reads.
+template <int BLOCK_N, bool TMA_STORE = false>
 struct Cfg {
   static constexpr int kStageA = BLOCK_M * BLOCK_K * 2;
   static constexpr int kStageB = BLOCK_N * BLOCK_K * 2;
   static constexpr int kStages = (BLOCK_N == 256) ? 4 : (BLOCK_N == 128) ? 6 : 8;
-  static constexpr int kSmemBytes = kStages * (kStageA + kStageB) + 1024 /*align*/ + 256 /*barriers*/ + (4 * 128 + 16) * 4 /*head*/;
+  static constexpr int kRing = kStages * (kStageA + kStageB);
+  static constexpr int kOutBuf = 64 * 128;
+  static constexpr int kStaging = TMA_STORE ? 2 * 2 * kOutBuf : 0;
+  static constexpr int kSmemBytes = kRing + kStaging + 1024 /*align*/ + 256 /*barriers*/ + (TMA_STORE ? 0 : (4 * 128 + 16) * 4) /*head*/;
   static_assert(kSmemBytes <= 227 * 1024, "shared memory of one CTA");
 };
 
@@ -124,16 +131,22 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaxf(x, 0.f) - fabsf(h);
 }
 
-template <int BLOCK_N, int EPI, bool PAIR>
+// TMA_STORE (specialised epilogues at BLOCK_N = 256 only): the epilogue stages the tile in shared memory 64 rows at a
+// time and one thread per warpgroup writes it with a TMA store (bf16) or TMA reduce-add (EPI_RESID) through tmap_o, which
+// the register-store kernels do not read.
+template <int BLOCK_N, int EPI, bool PAIR, bool TMA_STORE>
 __global__ void __launch_bounds__(kNumThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const Params p) {
-  using C = Cfg<BLOCK_N>;
+gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+            const __grid_constant__ CUtensorMap tmap_o, const Params p) {
+  static_assert(!TMA_STORE || (BLOCK_N == 256 && EPI != EPI_GENERIC), "TMA-store epilogue: specialised epilogues on 128x256 tiles");
+  using C = Cfg<BLOCK_N, TMA_STORE>;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms (the same offset in both CTAs of a pair: multicast writes by offset)
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smem_a = smem;
   uint8_t* smem_b = smem + C::kStages * C::kStageA;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kStages * (C::kStageA + C::kStageB));
+  uint8_t* smem_o = smem + C::kRing;              // [2 warpgroups][2 buffers][64 rows][128 B] (TMA_STORE)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kRing + C::kStaging);
   uint64_t* full_bar = bars;                      // [kStages]
   uint64_t* empty_bar = bars + C::kStages;        // [kStages]
   float* s_w4 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);  // [4][128] + [4]
@@ -151,13 +164,14 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   if (threadIdx.x == 0) {
     ptx::prefetch_tmap(&tmap_a);
     ptx::prefetch_tmap(&tmap_b);
+    if constexpr (TMA_STORE) ptx::prefetch_tmap(&tmap_o);
     for (int s = 0; s < C::kStages; ++s) {
       ptx::mbar_init(ptx::smem_u32(&full_bar[s]), 1);
       ptx::mbar_init(ptx::smem_u32(&empty_bar[s]), (PAIR ? 2 : 1) * kConsumerWarps);
     }
     ptx::fence_barrier_init();
   }
-  if ((p.flags & F_HEAD_FINAL) && threadIdx.x >= 128) {
+  if (!TMA_STORE && (p.flags & F_HEAD_FINAL) && threadIdx.x >= 128) {
     for (int i = threadIdx.x - 128; i < 4 * 128 + 4; i += 256) s_w4[i] = (i < 512) ? p.w4[i] : p.b4[i - 512];
   }
   __syncthreads();
@@ -217,6 +231,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     float acc[BLOCK_N / 2];
     int stage = 0;
     uint32_t phase = 0;
+    uint32_t out_chunk = 0;                  // TMA_STORE: chunks this warpgroup has staged so far (buffer = out_chunk & 1)
     auto release = [&](int s) {
       if (lane == 0) {
         if constexpr (PAIR) {
@@ -333,6 +348,48 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           }
         }
       }
+      if constexpr (TMA_STORE) {
+        // (3) staged stores: the warpgroup's 64 x 256 result leaves in chunks of 64 rows x 128 B (64 bf16 or 32 fp32
+        //     columns), each written into a 128B-swizzled buffer (16-byte unit u of row r at u ^ (r & 7), the layout the
+        //     tensor map's swizzle expects) and handed to the TMA unit by thread 0 of the warpgroup.  Two buffers
+        //     alternate.  Before the barrier that hands chunk i over, thread 0 waits until chunk i - 1's transfer has read
+        //     its buffer, so the barrier also frees that buffer for chunk i + 1.  The transfers of a tile's last chunks
+        //     overlap the next tile's main loop; rows past M are clipped by the tensor map.
+        constexpr bool kF32 = (EPI == EPI_RESID);
+        constexpr int kChunkCols = kF32 ? 32 : 64;
+        constexpr int kChunkNB = kChunkCols / 8;
+        const bool issuer = (threadIdx.x & 127) == 0;
+        const uint32_t sw = lane >> 2;           // (row & 7) of both rows this thread holds
+#pragma unroll
+        for (int c = 0; c < BLOCK_N / kChunkCols; ++c) {
+          const uint32_t buf = ptx::smem_u32(smem_o + (wg * 2 + (out_chunk & 1)) * C::kOutBuf);
+#pragma unroll
+          for (int j = 0; j < kChunkNB; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const uint32_t row = wq * 16 + (lane >> 2) + 8 * h;
+              float v0 = acc[4 * (c * kChunkNB + j) + 2 * h], v1 = acc[4 * (c * kChunkNB + j) + 2 * h + 1];
+              if (flags & F_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+              if constexpr (kF32) {
+                // columns 8j + 2q, +1: bytes 32j + 8q of the row
+                ptx::st_shared_v2_f32(buf + row * 128 + (((2 * j + (q >> 1)) ^ sw) << 4) + (q & 1) * 8, v0, v1);
+              } else {
+                ptx::st_shared_b32(buf + row * 128 + ((j ^ sw) << 4) + q * 4, pack_bf16x2(v0, v1));
+              }
+            }
+          ptx::fence_proxy_async();
+          if (issuer) ptx::bulk_wait_group_read<0>();
+          ptx::named_bar_sync(1 + wg, 128);
+          if (issuer) {
+            const int c0 = tn * BLOCK_N + c * kChunkCols, r0 = tm * BLOCK_M + wg * 64;
+            if constexpr (kF32) ptx::tma_reduce_add_2d(&tmap_o, buf, c0, r0);
+            else ptx::tma_store_2d(&tmap_o, buf, c0, r0);
+            ptx::bulk_commit_group();
+          }
+          ++out_chunk;
+        }
+        continue;
+      }
       if (flags & F_HEAD_FINAL) {
         // relu(conv) . w4 over the 128 channels of a row (the whole row is in this tile): this thread's 32 columns,
         // then the four threads of a row quad
@@ -405,6 +462,10 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
           }
         }
       }
+    }
+    // the output is complete when the grid is: a dependent launch (PDL) starts on that guarantee
+    if constexpr (TMA_STORE) {
+      if ((threadIdx.x & 127) == 0) ptx::bulk_wait_group<0>();
     }
   }
   if constexpr (PAIR) ptx::cluster_sync();   // no CTA leaves while its partner may still arrive on its barriers

@@ -1,6 +1,6 @@
 // Thin inline-PTX wrappers for the Hopper (sm_90a) primitives used by the dust3r_b200 kernels:
-// mbarrier, bulk copies (cp.async.bulk), TMA (cp.async.bulk.tensor, with cluster multicast), clusters, wgmma (fence / mma /
-// commit / wait), and the MUFU approximations.
+// mbarrier, bulk copies (cp.async.bulk), TMA (cp.async.bulk.tensor loads with cluster multicast, stores and reduce-adds),
+// clusters, wgmma (fence / mma / commit / wait), and the MUFU approximations.
 // Descriptor bit layouts follow the PTX ISA "wgmma matrix descriptor" table.
 #pragma once
 #include <cuda.h>
@@ -115,6 +115,29 @@ __device__ __forceinline__ void tma_load_3d_mc(uint32_t dst, const void* tmap, u
       ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "h"(mask)
       : "memory");
 }
+
+// shared -> global tensor stores of one box, tracked as bulk async-groups of the issuing thread.  Elements outside the
+// tensor map's bounds are not written.  The source must have been written before a fence_proxy_async().
+__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+// global += shared, element-wise in the tensor map's type, performed by the memory system
+__device__ __forceinline__ void tma_reduce_add_2d(const void* tmap, uint32_t src, int c0, int c1) {
+  asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(src), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read their shared-memory source
+template <int N> __device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups are still incomplete (their global writes not yet performed)
+template <int N> __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+__device__ __forceinline__ void st_shared_v2_f32(uint32_t addr, float a, float b) {
+  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
+}
+// barrier of the `count` threads (a multiple of 32) that name barrier `id` (0 is __syncthreads')
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t count) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory"); }
 
 // ---- clusters -------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {

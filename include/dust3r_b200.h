@@ -256,6 +256,12 @@ int d3r_attention_hd64(const void* q_dev, int64_t ldq, const void* k_dev, int64_
 void d3r_set_gemm_impl(int32_t impl);
 /* Tuning aid for impl 2: minimum number of 64-wide k-blocks for which the CTA-pair kernel is used (default 4). */
 void d3r_set_gemm_pair_min_kblocks(int32_t kblocks);
+/* Selects how the specialised epilogues on 128x256 tiles (bias / GELU / ReLU -> bf16, bias + RoPE -> bf16, fp32 residual
+ * update) write their result: 1 (default) = staged in shared memory and written by TMA store, or TMA reduce-add for the
+ * residual update, overlapping the next tile's main loop; 0 = every thread stores straight from its accumulator
+ * registers (A/B reference, bit-identical).  With 1, an output whose base or row stride (ldo * element size) is not a
+ * multiple of 16 bytes takes the register stores. */
+void d3r_set_gemm_store(int32_t store);
 
 /* Selects the attention kernel: 3 (default) = wgmma kernel (64 query rows per warpgroup, 128-key blocks) with P kept in
  * registers (A-from-registers wgmma); 2 = the same dataflow with P through shared memory (A/B reference). */
