@@ -286,3 +286,51 @@ int linear_head_postprocess(const float* feat, float* pts3d, float* conf, int B,
 
 }  // namespace ew
 }  // namespace d3r
+
+// ---- building blocks exported through the C ABI (used by the unit tests; forward.cu calls d3r::ew directly) ----
+using namespace d3r;
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
+
+extern "C" int d3r_layernorm_bf16(const float* x, const float* g, const float* b, void* out, int32_t M, int32_t C, float eps,
+                                  void* stream) {
+  D3R_CHECK_ARG(x && g && b && out, "layernorm: null buffer");
+  D3R_CHECK_ARG(M > 0 && C > 0, "layernorm: bad shape M=%d C=%d", M, C);
+  D3R_CHECK_ARG(aligned16(x) && aligned16(g) && aligned16(b) && (reinterpret_cast<uintptr_t>(out) & 7) == 0,
+                "layernorm: x, g, b must be 16-byte and out 8-byte aligned");
+  return ew::layernorm(x, g, b, out, nullptr, M, C, eps, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_upsample2x_bf16(const void* x, void* out, int32_t B, int32_t H, int32_t W, int32_t C, int32_t Ho, int32_t Wo,
+                                   void* stream) {
+  D3R_CHECK_ARG(x && out, "upsample2x: null buffer");
+  D3R_CHECK_ARG(B > 0 && B <= 65535 && H > 0 && W > 0 && C > 0 && Ho > 0 && Wo > 0, "upsample2x: bad shape B=%d H=%d W=%d C=%d Ho=%d Wo=%d",
+                B, H, W, C, Ho, Wo);
+  D3R_CHECK_ARG(aligned16(x) && aligned16(out), "upsample2x: buffers must be 16-byte aligned");
+  return ew::upsample2x_bf16(x, out, B, H, W, C, Ho, Wo, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_im2col_3x3_s2_bf16(const void* x, void* out, int32_t B, int32_t H, int32_t W, int32_t C, void* stream) {
+  D3R_CHECK_ARG(x && out, "im2col_s2: null buffer");
+  D3R_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0, "im2col_s2: bad shape B=%d H=%d W=%d C=%d", B, H, W, C);
+  D3R_CHECK_ARG(aligned16(x) && aligned16(out), "im2col_s2: buffers must be 16-byte aligned");
+  return ew::im2col_3x3_s2_bf16(x, out, B, H, W, C, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_patch_im2col16(const float* img, void* out, int32_t B, int32_t H, int32_t W, void* stream) {
+  D3R_CHECK_ARG(img && out, "patch_im2col: null buffer");
+  D3R_CHECK_ARG(B > 0 && H > 0 && W > 0, "patch_im2col: bad shape B=%d H=%d W=%d", B, H, W);
+  D3R_CHECK_ARG(aligned16(img) && aligned16(out), "patch_im2col: buffers must be 16-byte aligned");
+  return ew::patch_im2col16(img, out, B, H, W, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_linear_head_postprocess(const float* feat, float* pts3d, float* conf, int32_t B, int32_t gh, int32_t gw, int32_t nch,
+                                           int32_t depth_mode, int32_t conf_mode, float conf_min, float conf_max, void* stream) {
+  D3R_CHECK_ARG(feat && pts3d, "linear_head_postprocess: null buffer");
+  D3R_CHECK_ARG(B > 0 && gh > 0 && gw > 0, "linear_head_postprocess: bad shape B=%d gh=%d gw=%d", B, gh, gw);
+  D3R_CHECK_ARG(nch == 3 || nch == 4, "linear_head_postprocess: nch=%d must be 3 or 4", nch);
+  D3R_CHECK_ARG(depth_mode >= 0 && depth_mode <= 2, "linear_head_postprocess: depth_mode %d out of range", depth_mode);
+  D3R_CHECK_ARG(conf_mode >= 0 && conf_mode <= 2, "linear_head_postprocess: conf_mode %d out of range", conf_mode);
+  D3R_CHECK_ARG(nch == 3 || conf_mode == 0 || conf, "linear_head_postprocess: conf_mode %d without a conf buffer", conf_mode);
+  return ew::linear_head_postprocess(feat, pts3d, conf, B, gh, gw, nch, depth_mode, conf_mode, conf_min, conf_max, (cudaStream_t)stream);
+}

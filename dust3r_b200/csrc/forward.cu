@@ -82,16 +82,6 @@ static int conv3(const Ctx& c, const void* x, const d3r_linear& w, int B, int H,
   return gemm::conv3x3_bf16(x, w.w, B, H, W, Cin, Cout, p, c.st);
 }
 
-// k == stride transposed convolution: rows = input pixels, columns = (ky,kx,co)
-static int convT(const Ctx& c, const void* x, const d3r_linear& w, int B, int h, int wd, int Cin, int Cout, int k, void* out) {
-  Params p{};
-  p.M = B * h * wd; p.N = k * k * Cout; p.K = Cin;
-  p.flags = gemm::F_CONVT | (w.b ? gemm::F_BIAS : 0);
-  p.out = out; p.bias = w.b; p.ldo = 0;
-  p.tk = k; p.th_in = h; p.tw_in = wd; p.tCout = Cout;
-  return gemm::gemm_bf16(x, Cin, w.w, p, c.st);
-}
-
 // ---- encoder ---------------------------------------------------------------------------------
 static int run_encoder(const Ctx& c, Arena& ar, const float* imgs, int n_enc, int H, int W, void** enc_out_bf16) {
   const d3r_model& m = *c.m;
@@ -191,9 +181,9 @@ static int run_dpt(const Ctx& c, Arena& ar, const d3r_dpt_head& hd, const void* 
 
   // act_postprocess (dpt_block.py:341-398)
   RC(linear(c, tok[0], dims[0], hd.act_conv[0], Mt, ld[0], dims[0], a0, 0));
-  RC(convT(c, a0, hd.act0_up, B, gh, gw, 96, 96, 4, l[0]));
+  RC(gemm::conv_transpose_bf16(a0, hd.act0_up.w, l[0], hd.act0_up.b, B, gh, gw, 96, 96, 4, c.st));
   RC(linear(c, tok[1], dims[1], hd.act_conv[1], Mt, ld[1], dims[1], a1, 0));
-  RC(convT(c, a1, hd.act1_up, B, gh, gw, 192, 192, 2, l[1]));
+  RC(gemm::conv_transpose_bf16(a1, hd.act1_up.w, l[1], hd.act1_up.b, B, gh, gw, 192, 192, 2, c.st));
   RC(linear(c, tok[2], dims[2], hd.act_conv[2], Mt, ld[2], dims[2], l[2], 0));
   RC(linear(c, tok[3], dims[3], hd.act_conv[3], Mt, ld[3], dims[3], a3, 0));
   RC(ew::im2col_3x3_s2_bf16(a3, col, B, gh, gw, 768, c.st));
@@ -235,16 +225,8 @@ static int run_dpt(const Ctx& c, Arena& ar, const d3r_dpt_head& hd, const void* 
   const int Hp = Hs[0] * 2, Wp = Ws[0] * 2;
   RC(conv3(c, path, hd.head0, B, Hp, Wp, F, 128, h0, 0));
   RC(ew::upsample2x_bf16(h0, h1, B, Hp, Wp, 128, Hf, Wf, c.st));
-  {
-    Params p{};
-    p.flags = gemm::F_HEAD_FINAL | (hd.head2.b ? gemm::F_BIAS : 0);
-    p.bias = hd.head2.b;
-    p.w4 = hd.head4_w; p.b4 = hd.head4_b;
-    p.pts3d = pts3d; p.conf = conf;
-    p.depth_mode = m.depth_mode; p.conf_mode = (m.nch > 3 && conf) ? m.conf_mode : 0;
-    p.conf_min = m.conf_min; p.conf_max = m.conf_max;
-    RC(gemm::conv3x3_bf16(h1, hd.head2.w, B, Hf, Wf, 128, 128, p, c.st));
-  }
+  RC(gemm::conv3x3_head_tail(h1, hd.head2.w, hd.head2.b, hd.head4_w, hd.head4_b, pts3d, conf, B, Hf, Wf, m.depth_mode,
+                             (m.nch > 3 && conf) ? m.conf_mode : 0, m.conf_min, m.conf_max, c.st));
   return D3R_OK;
 }
 

@@ -168,6 +168,41 @@ int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, 
   return dispatch(bn, ta, tb, nullptr, p, B * p.tiles_x * p.tiles_y, st);
 }
 
+// rows = input pixels, columns = (ky,kx,co).  The epilogue stores column pairs (co, co + 1), so Cout must be even for a
+// pair to stay inside one kernel position.
+int conv_transpose_bf16(const void* x_nhwc, const void* w_packed, void* out, const float* bias, int B, int h, int w, int Cin, int Cout,
+                        int k, cudaStream_t st) {
+  D3R_CHECK_ARG(x_nhwc && w_packed && out, "conv_transpose: null buffer");
+  D3R_CHECK_ARG(B > 0 && h > 0 && w > 0 && Cin > 0 && Cout > 0 && k > 0, "conv_transpose: bad shape B=%d h=%d w=%d Cin=%d Cout=%d k=%d", B,
+                h, w, Cin, Cout, k);
+  D3R_CHECK_ARG(Cin % 8 == 0, "conv_transpose: Cin=%d must be a multiple of 8", Cin);
+  D3R_CHECK_ARG(Cout % 2 == 0 && (k * k * Cout) % 32 == 0, "conv_transpose: Cout=%d must be even and k*k*Cout=%d a multiple of 32", Cout,
+                k * k * Cout);
+  Params p{};
+  p.M = B * h * w; p.N = k * k * Cout; p.K = Cin;
+  p.flags = F_CONVT | (bias ? F_BIAS : 0);
+  p.out = out; p.bias = bias; p.ldo = 0;
+  p.tk = k; p.th_in = h; p.tw_in = w; p.tCout = Cout;
+  return gemm_bf16(x_nhwc, Cin, w_packed, p, st);
+}
+
+int conv3x3_head_tail(const void* x_nhwc, const void* w_packed, const float* bias, const float* w4, const float* b4, float* pts3d,
+                      float* conf, int B, int H, int W, int depth_mode, int conf_mode, float conf_min, float conf_max, cudaStream_t st) {
+  D3R_CHECK_ARG(x_nhwc && w_packed && w4 && b4 && pts3d, "conv3x3_head_tail: null buffer");
+  D3R_CHECK_ARG(B > 0 && H > 0 && W > 0, "conv3x3_head_tail: bad shape B=%d H=%d W=%d", B, H, W);
+  D3R_CHECK_ARG(depth_mode >= 0 && depth_mode <= 2, "conv3x3_head_tail: depth_mode %d out of range", depth_mode);
+  D3R_CHECK_ARG(conf_mode >= 0 && conf_mode <= 2, "conv3x3_head_tail: conf_mode %d out of range", conf_mode);
+  D3R_CHECK_ARG(conf_mode == 0 || conf, "conv3x3_head_tail: conf_mode %d without a conf buffer", conf_mode);
+  Params p{};
+  p.flags = F_HEAD_FINAL | (bias ? F_BIAS : 0);
+  p.bias = bias;
+  p.w4 = w4; p.b4 = b4;
+  p.pts3d = pts3d; p.conf = conf;
+  p.depth_mode = depth_mode; p.conf_mode = conf_mode;
+  p.conf_min = conf_min; p.conf_max = conf_max;
+  return conv3x3_bf16(x_nhwc, w_packed, B, H, W, 128, 128, p, st);
+}
+
 }  // namespace gemm
 }  // namespace d3r
 
@@ -188,7 +223,8 @@ extern "C" int d3r_gemm_bf16(const void* A, const void* B, void* out, const floa
   p.rope_cos = rope_cos; p.rope_sin = rope_sin; p.rope_cols = rope_cols; p.tokens_per_img = tokens_per_img; p.grid_w = grid_w;
   D3R_CHECK_ARG(!(flags & gemm::F_BIAS) || bias, "gemm: F_BIAS without bias");
   D3R_CHECK_ARG(!(flags & gemm::F_ROPE) || (rope_cos && rope_sin && tokens_per_img > 0 && grid_w > 0), "gemm: F_ROPE without tables");
-  D3R_CHECK_ARG(!(flags & (gemm::F_CONVT | gemm::F_HEAD_FINAL)), "gemm: use the dedicated entry points for convT / head tail");
+  D3R_CHECK_ARG(!(flags & (gemm::F_CONVT | gemm::F_HEAD_FINAL)),
+                "gemm: F_CONVT / F_HEAD_FINAL have their own entry points, d3r_conv_transpose_bf16 / d3r_conv3x3_head_tail");
   return gemm::gemm_bf16(A, K, B, p, (cudaStream_t)stream);
 }
 
@@ -200,4 +236,16 @@ extern "C" int d3r_conv3x3_bf16(const void* x_nhwc, const void* w_packed, void* 
   p.out = out; p.out2 = out2; p.add0 = add0; p.add1 = add1; p.bias = bias;
   D3R_CHECK_ARG(!(flags & (gemm::F_CONVT | gemm::F_HEAD_FINAL | gemm::F_ROPE)), "conv3x3: unsupported flag");
   return gemm::conv3x3_bf16(x_nhwc, w_packed, B, H, W, Cin, Cout, p, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_conv_transpose_bf16(const void* x_nhwc, const void* w_packed, void* out, const float* bias, int32_t B, int32_t h,
+                                       int32_t w, int32_t Cin, int32_t Cout, int32_t k, void* stream) {
+  return gemm::conv_transpose_bf16(x_nhwc, w_packed, out, bias, B, h, w, Cin, Cout, k, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_conv3x3_head_tail(const void* x_nhwc, const void* w_packed, const float* bias, const float* w4, const float* b4,
+                                     float* pts3d, float* conf, int32_t B, int32_t H, int32_t W, int32_t depth_mode, int32_t conf_mode,
+                                     float conf_min, float conf_max, void* stream) {
+  return gemm::conv3x3_head_tail(x_nhwc, w_packed, bias, w4, b4, pts3d, conf, B, H, W, depth_mode, conf_mode, conf_min, conf_max,
+                                 (cudaStream_t)stream);
 }

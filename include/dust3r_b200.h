@@ -250,6 +250,44 @@ int d3r_attention_hd64(const void* q_dev, int64_t ldq, const void* k_dev, int64_
                        void* out_dev, int64_t ldo, int32_t B, int32_t heads, int32_t Nq, int32_t Nk, float scale,
                        void* stream);
 
+/* ConvTranspose2d with kernel == stride == k (dpt_block.py act_postprocess 0 / 1) as a GEMM whose epilogue scatters each
+ * input pixel's k x k x Cout block: x (B,h,w,Cin) bf16 NHWC; w_packed [(ky*k+kx)*Cout + co][Cin] bf16 (the torch weight
+ * (Cin,Cout,k,k) permuted to (ky,kx,co,ci)); bias [Cout] fp32 or NULL; out (B,h*k,w*k,Cout) bf16 NHWC.
+ * Cin % 8 == 0, Cout even, k*k*Cout % 32 == 0. */
+int d3r_conv_transpose_bf16(const void* x_nhwc_dev, const void* w_packed_dev, void* out_dev, const float* bias_dev, int32_t B,
+                            int32_t h, int32_t w, int32_t Cin, int32_t Cout, int32_t k, void* stream);
+
+/* DPT head tail (dpt_head.py head.2 .. head.4 + postprocess.py), fused into one conv's epilogue: conv3x3 128->128 (+ bias, may
+ * be NULL) -> ReLU -> 1x1 conv to 4 channels (w4 [4][128], b4 [4] fp32; rows past the model's channels zero) -> pointmap
+ * postprocess.  x (B,H,W,128) bf16 NHWC, w_packed [128][9][128] bf16; pts3d (B,H,W,3) fp32; conf (B,H,W) fp32, written only
+ * when conf_mode != 0.  depth_mode 0 linear, 1 square, 2 exp; conf_mode 0 none, 1 exp, 2 sigmoid, in [conf_min, conf_max]. */
+int d3r_conv3x3_head_tail(const void* x_nhwc_dev, const void* w_packed_dev, const float* bias_dev, const float* w4_dev,
+                          const float* b4_dev, float* pts3d_dev, float* conf_dev, int32_t B, int32_t H, int32_t W, int32_t depth_mode,
+                          int32_t conf_mode, float conf_min, float conf_max, void* stream);
+
+/* LayerNorm of fp32 rows to bf16 (nn.LayerNorm of the ViT blocks): x [M][C] fp32, g / b [C] fp32, out [M][C] bf16.
+ * C % 4 == 0, C <= 2048; x, g, b 16-byte aligned. */
+int d3r_layernorm_bf16(const float* x_dev, const float* g_dev, const float* b_dev, void* out_dev, int32_t M, int32_t C, float eps,
+                       void* stream);
+
+/* Bilinear x2 upsample, align_corners=True (dpt_block.py F.interpolate), cropped: x (B,H,W,C) bf16 NHWC -> out (B,Ho,Wo,C), the
+ * top-left Ho x Wo of the (2H, 2W) upsample.  Ho <= 2H, Wo <= 2W, C/8 a power of two; buffers 16-byte aligned. */
+int d3r_upsample2x_bf16(const void* x_dev, void* out_dev, int32_t B, int32_t H, int32_t W, int32_t C, int32_t Ho, int32_t Wo,
+                        void* stream);
+
+/* im2col of the 3x3 stride-2 pad-1 conv (act_postprocess 3): x (B,H,W,C) bf16 NHWC -> out [B*Ho*Wo][9][C] with
+ * Ho = ceil(H/2), Wo = ceil(W/2), tap = ky*3+kx, zero outside the image.  C % 8 == 0. */
+int d3r_im2col_3x3_s2_bf16(const void* x_dev, void* out_dev, int32_t B, int32_t H, int32_t W, int32_t C, void* stream);
+
+/* Patch im2col of the 16x16 patch embedding: img (B,3,H,W) fp32 -> out [B*(H/16)*(W/16)][3*16*16] bf16 (round to nearest
+ * even), column c*256 + py*16 + px (the Conv2d weight flatten).  H, W multiples of 16. */
+int d3r_patch_im2col16(const float* img_dev, void* out_dev, int32_t B, int32_t H, int32_t W, void* stream);
+
+/* Linear head tail (heads/linear_head.py + postprocess.py): feat [B*gh*gw][nch*256] fp32 (channel-major, then py*16+px)
+ * -> pixel shuffle -> pts3d (B,16gh,16gw,3), conf (B,16gh,16gw) fp32 (conf written only when nch == 4 and conf_mode != 0). */
+int d3r_linear_head_postprocess(const float* feat_dev, float* pts3d_dev, float* conf_dev, int32_t B, int32_t gh, int32_t gw,
+                                int32_t nch, int32_t depth_mode, int32_t conf_mode, float conf_min, float conf_max, void* stream);
+
 /* Selects the GEMM / conv kernel family: 0 = 1-CTA kernels, 1 = CTA-pair kernels (a cluster of two CTAs on two
  * M tiles sharing one multicast B tile), 2 (default) = CTA-pair kernels from 4 k-blocks of 64 on (K >= 256), 1-CTA
  * for shorter reductions. */

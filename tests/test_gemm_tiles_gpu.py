@@ -43,27 +43,35 @@ def gemm_impl(request):
 
 
 @pytest.mark.timeout(300)
-@pytest.mark.parametrize('Bimg,gh,gw', [(3, 6, 10), (5, 12, 16)])
-def test_gemm_rope_bf16_matches_oracle(cuda_device, Bimg, gh, gw):
-    """QKV projection with fused 2D RoPE stored as bf16 == oracle rope2d(linear) (croco/models/pos_embed.py:113-157)."""
+@pytest.mark.parametrize('Bimg,gh,gw,kv', [pytest.param(3, 6, 10, False, id='3-6-10'), pytest.param(5, 12, 16, False, id='5-12-16'),
+                                           pytest.param(3, 21, 32, True, id='kv-3-21-32'),
+                                           pytest.param(3, 32, 21, False, id='portrait-3-32-21')])
+def test_gemm_rope_bf16_matches_oracle(cuda_device, Bimg, gh, gw, kv):
+    """QKV projection with fused 2D RoPE stored as bf16 == oracle rope2d(linear) (croco/models/pos_embed.py:113-157).
+    kv: the decoder's fused k|v projection of the cross attention, rope_cols = N / 2: k rotated, v left as it is.  The
+    portrait grid (gh > gw) has row positions past gw."""
     from oracle.forward_oracle import rope2d, positions, rope_tables
     nh, hd = 4, 64
     Cdim = nh * hd
     Ntok = gh * gw
     M = Bimg * Ntok
+    parts = 2 if kv else 3
     x = _rand((M, Cdim), cuda_device, seed=31).bfloat16()
-    Wqkv = _rand((3 * Cdim, Cdim), cuda_device, scale=Cdim ** -0.5, seed=32).bfloat16()
-    bias = _rand((3 * Cdim,), cuda_device, seed=33)
+    Wqkv = _rand((parts * Cdim, Cdim), cuda_device, scale=Cdim ** -0.5, seed=32).bfloat16()
+    bias = _rand((parts * Cdim,), cuda_device, seed=33)
     cos, sin = rope_tables(hd, max(gh, gw), 100.0)
     cos, sin = cos.to(cuda_device).contiguous(), sin.to(cuda_device).contiguous()
-    out = gemm(x, Wqkv, bias, F_BIAS | F_ROPE, rope=(cos, sin, 2 * Cdim, Ntok, gw))
-    lin = (x.float() @ Wqkv.float().T + bias).cpu().reshape(Bimg, Ntok, 3, nh, hd).permute(2, 0, 3, 1, 4)
+    out = gemm(x, Wqkv, bias, F_BIAS | F_ROPE, rope=(cos, sin, (parts - 1) * Cdim, Ntok, gw))
+    lin = (x.float() @ Wqkv.float().T + bias).cpu().reshape(Bimg, Ntok, parts, nh, hd).permute(2, 0, 3, 1, 4)
     pos = positions(Bimg, gh, gw)
-    q = rope2d(lin[0], pos, 100.0)
-    k = rope2d(lin[1], pos, 100.0)
-    ref = torch.stack((q, k, lin[2]), 0).permute(1, 3, 0, 2, 4).reshape(M, 3 * Cdim)
+    rotated = [rope2d(lin[i], pos, 100.0) for i in range(parts - 1)]
+    ref = torch.stack(rotated + [lin[parts - 1]], 0).permute(1, 3, 0, 2, 4).reshape(M, parts * Cdim)
     assert torch.isfinite(out.float()).all()
     assert (out.float().cpu() - ref).abs().max().item() <= 2e-2 * max(1.0, ref.abs().max().item())
+    if kv:
+        # v is the plain projection: within one bf16 rounding of it, never rotated
+        v = lin[1].permute(0, 2, 1, 3).reshape(M, Cdim)
+        assert ((out.float().cpu()[:, Cdim:] - v).abs() <= 2.0 ** -8 * v.abs() + 1e-3).all()
 
 
 @pytest.mark.timeout(300)
