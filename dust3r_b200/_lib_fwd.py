@@ -72,6 +72,8 @@ def declare(lib):
     lib.d3r_set_gemm_impl.argtypes = [i32]
     lib.d3r_set_gemm_store.restype = None
     lib.d3r_set_gemm_store.argtypes = [i32]
+    lib.d3r_set_conv_store.restype = None
+    lib.d3r_set_conv_store.argtypes = [i32]
     lib.d3r_set_attention_impl.restype = None
     lib.d3r_set_attention_impl.argtypes = [i32]
     lib.d3r_forward_workspace_bytes.restype = i64

@@ -6,8 +6,15 @@
 namespace d3r {
 namespace gemm {
 
-static int pick_block_n(int N, int mode, uint32_t flags) {
+// conv_m_tiles > 0: a 3x3 conv with the staged epilogue (Cout 256 or 128) over that many 128-pixel tiles.  A 128x256 tile
+// holds all 256 output channels, so each A tile is read once instead of once per 128-channel half, at 7.6 instead of
+// 11.4 KB of operands per MFLOP.  It is used when there are at least 4 waves of CTA-pair work items at that width
+// (levels 0 and 1 of the DPT head at B = 32: 1536 and 384 items for 66 pairs).  With fewer, the partly filled last wave
+// of double-size items costs more than the operand traffic saves (level 2: 96 items, i.e. 2 rounds of 256-wide items
+// against 3 of 128-wide ones, which take half as long; level 3: 32 items, half the SMs idle), and 128x128 tiles are used.
+static int pick_block_n(int N, int mode, uint32_t flags, int conv_m_tiles = 0) {
   if (flags & F_HEAD_FINAL) return 128;   // the head tail needs a whole 128-channel row in one tile
+  if (conv_m_tiles > 0) return (N == 256 && (conv_m_tiles + 1) / 2 >= 4 * (num_sms() / 2)) ? 256 : 128;
   // 128x256 tiles for the specialised epilogues (every ViT projection): half the A traffic per FLOP of 128x128
   if (N % 256 == 0 && pick_epi(mode, flags) != EPI_GENERIC) return 256;
   if (N % 128 == 0) return 128;
@@ -25,6 +32,27 @@ static bool use_pair(int bn, int num_kb) { return bn >= 128 && (g_impl == 1 || (
 // 0: register-store epilogues everywhere (the bit-identical A/B reference), 1 (default): the specialised epilogues on
 // 128x256 tiles stage their output in shared memory and write it by TMA store / TMA reduce-add, when TMA can address it
 static int g_store = 1;
+// 0: the 3x3 convolutions on the register-store EPI_GENERIC kernels with 128-wide tiles (the bit-identical A/B
+// reference), 1 (default): Cout 256 / 128 convs on conv_kernel, with the staged TMA epilogue, when TMA can address every
+// tensor the epilogue touches
+static int g_conv_store = 1;
+
+static int grid_for(bool pair, int m_tiles, int n_tiles) {
+  if (pair) {
+    const int items = ((m_tiles + 1) / 2) * n_tiles;
+    const int max_clusters = num_sms() / 2;
+    return 2 * (items < max_clusters ? items : max_clusters);
+  }
+  const int items = m_tiles * n_tiles;
+  return items < num_sms() ? items : num_sms();
+}
+
+static const char* prof_tag(const Params& p, int bn, bool pair) {
+  return (p.mode == 1) ? ((p.flags & F_HEAD_FINAL) ? (pair ? "conv3x3_head_tail_2cta" : "conv3x3_head_tail")
+                                                   : (pair ? "conv3x3_wgmma_2cta" : "conv3x3_wgmma"))
+                       : (bn == 256 ? (pair ? "gemm_wgmma_2cta_bn256" : "gemm_wgmma_bn256")
+                                    : (pair ? "gemm_wgmma_2cta_bn128" : (bn == 128 ? "gemm_wgmma_bn128" : "gemm_wgmma_bn64")));
+}
 
 template <int BN, int EPI, bool PAIR, bool TMA_STORE = false>
 static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const Params& p, int m_tiles, int n_tiles,
@@ -33,24 +61,29 @@ static int launch(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMa
   static unsigned long long attr_devices = 0;
   if (first_launch_on_this_device(attr_devices))
     D3R_CUDA(cudaFuncSetAttribute(gemm_kernel<BN, EPI, PAIR, TMA_STORE>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
-  int grid;
-  if (PAIR) {
-    const int items = ((m_tiles + 1) / 2) * n_tiles;
-    const int max_clusters = num_sms() / 2;
-    grid = 2 * (items < max_clusters ? items : max_clusters);
-  } else {
-    const int items = m_tiles * n_tiles;
-    grid = items < num_sms() ? items : num_sms();
-  }
-  const char* tag = (p.mode == 1) ? ((p.flags & F_HEAD_FINAL) ? (PAIR ? "conv3x3_head_tail_2cta" : "conv3x3_head_tail")
-                                                              : (PAIR ? "conv3x3_wgmma_2cta" : "conv3x3_wgmma"))
-                                  : (BN == 256 ? (PAIR ? "gemm_wgmma_2cta_bn256" : "gemm_wgmma_bn256")
-                                               : (PAIR ? "gemm_wgmma_2cta_bn128" : (BN == 128 ? "gemm_wgmma_bn128" : "gemm_wgmma_bn64")));
+  const int grid = grid_for(PAIR, m_tiles, n_tiles);
   char detail[96];
   snprintf(detail, sizeof(detail), "M=%d N=%d K=%d flags=0x%x mode=%d epi=%d", p.M, p.N, p.K, (unsigned)p.flags, p.mode, EPI);
-  prof::Scope scope(tag, st, 2.0 * double(p.M) * double(p.N) * double(p.K), 0.0, 1, detail);
+  prof::Scope scope(prof_tag(p, BN, PAIR), st, 2.0 * double(p.M) * double(p.N) * double(p.K), 0.0, 1, detail);
   D3R_CUDA(pdl::launch_clustered(gemm_kernel<BN, EPI, PAIR, TMA_STORE>, dim3(grid), dim3(kNumThreads), size_t(kSmem), st, PAIR ? 2 : 1,
                                  ta, tb, to, p));
+  D3R_LAUNCH_CHECK();
+  return D3R_OK;
+}
+
+// conv_kernel: profiled under the conv tags with epi=0, like the EPI_GENERIC launches it stands in for
+template <int BN, bool PAIR>
+static int launch_conv(const CUtensorMap& ta, const CUtensorMap& tb, const CUtensorMap& to, const ConvMaps& cm, const Params& p,
+                       int m_tiles, int n_tiles, cudaStream_t st) {
+  constexpr int kSmem = Cfg<BN, true>::kSmemBytes;
+  static unsigned long long attr_devices = 0;
+  if (first_launch_on_this_device(attr_devices))
+    D3R_CUDA(cudaFuncSetAttribute(conv_kernel<BN, PAIR>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmem));
+  const int grid = grid_for(PAIR, m_tiles, n_tiles);
+  char detail[96];
+  snprintf(detail, sizeof(detail), "M=%d N=%d K=%d flags=0x%x mode=%d epi=%d", p.M, p.N, p.K, (unsigned)p.flags, p.mode, EPI_GENERIC);
+  prof::Scope scope(prof_tag(p, BN, PAIR), st, 2.0 * double(p.M) * double(p.N) * double(p.K), 0.0, 1, detail);
+  D3R_CUDA(pdl::launch_clustered(conv_kernel<BN, PAIR>, dim3(grid), dim3(kNumThreads), size_t(kSmem), st, PAIR ? 2 : 1, ta, tb, to, cm, p));
   D3R_LAUNCH_CHECK();
   return D3R_OK;
 }
@@ -137,6 +170,18 @@ int gemm_bf16(const void* A, long long lda, const void* B, Params p, cudaStream_
   return dispatch(bn, ta, tb, staged ? &to : nullptr, p, (p.M + BLOCK_M - 1) / BLOCK_M, st);
 }
 
+// (B,H,W,C) bf16 NHWC as a 4D map (C, W, H, B) with boxes of 64 channels x 64 pixels (bw = min(tile_w, 64) by 64 / bw rows):
+// one consumer warpgroup's rows of a conv tile
+static int make_tmap_conv_io(CUtensorMap* m, const void* base, int B, int H, int W, int C, int tile_w, const char* op) {
+  const int bw = tile_w < 64 ? tile_w : 64;
+  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+  cuuint64_t str[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  cuuint32_t box[4] = {64, (cuuint32_t)bw, (cuuint32_t)(64 / bw), 1};
+  return encode_tensor_map(m, base, 4, dims, str, box, op);
+}
+
+static bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
+
 int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, int Cin, int Cout, Params p, cudaStream_t st) {
   D3R_CHECK_ARG(x_nhwc && w_packed, "conv3x3: null operand");
   D3R_CHECK_ARG(Cin % 8 == 0 && Cout % 32 == 0, "conv3x3: Cin=%d must be a multiple of 8 and Cout=%d of 32", Cin, Cout);
@@ -154,7 +199,12 @@ int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, 
   p.tiles_x = (W + p.tile_w - 1) / p.tile_w;
   p.tiles_y = (H + p.tile_h - 1) / p.tile_h;
   p.ldo = Cout;
-  const int bn = pick_block_n(p.N, p.mode, p.flags);
+  const int m_tiles = B * p.tiles_x * p.tiles_y;
+  // staged epilogue: Cout 256 / 128 (whole 64-channel boxes), the flags EPI_CONV covers, every tensor 16-byte aligned
+  const bool staged = g_conv_store == 1 && (Cout == 256 || Cout == 128) && (p.flags & ~EpiMask<EPI_CONV>::value) == 0 &&
+                      aligned16(p.out) && (!(p.flags & F_OUT2_RELU) || aligned16(p.out2)) && (!(p.flags & F_ADD0) || aligned16(p.add0)) &&
+                      (!(p.flags & F_ADD1) || aligned16(p.add1));
+  const int bn = pick_block_n(p.N, p.mode, p.flags, staged ? m_tiles : 0);
   CUtensorMap ta, tb;
   {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
@@ -165,7 +215,23 @@ int conv3x3_bf16(const void* x_nhwc, const void* w_packed, int B, int H, int W, 
   }
   int rc = make_tmap_b(&tb, w_packed, Cout, 9, Cin, bn, p.num_kb, "conv3x3");
   if (rc) return rc;
-  return dispatch(bn, ta, tb, nullptr, p, B * p.tiles_x * p.tiles_y, st);
+  if (!staged) return dispatch(bn, ta, tb, nullptr, p, m_tiles, st);
+  CUtensorMap to;
+  ConvMaps cm;
+  rc = make_tmap_conv_io(&to, p.out, B, H, W, Cout, p.tile_w, "conv3x3 output");
+  if (rc) return rc;
+  cm.out2 = cm.add0 = cm.add1 = to;   // maps the flags leave unused stay valid (the kernel prefetches all three)
+  const struct { uint32_t flag; const void* base; CUtensorMap* map; const char* op; } io[3] = {
+      {F_OUT2_RELU, p.out2, &cm.out2, "conv3x3 out2"}, {F_ADD0, p.add0, &cm.add0, "conv3x3 add0"}, {F_ADD1, p.add1, &cm.add1, "conv3x3 add1"}};
+  for (const auto& t : io) {
+    if (!(p.flags & t.flag)) continue;
+    rc = make_tmap_conv_io(t.map, t.base, B, H, W, Cout, p.tile_w, t.op);
+    if (rc) return rc;
+  }
+  const int n_tiles = Cout / bn;
+  const bool pair = use_pair(bn, p.num_kb);
+  if (bn == 256) return pair ? launch_conv<256, true>(ta, tb, to, cm, p, m_tiles, n_tiles, st) : launch_conv<256, false>(ta, tb, to, cm, p, m_tiles, n_tiles, st);
+  return pair ? launch_conv<128, true>(ta, tb, to, cm, p, m_tiles, n_tiles, st) : launch_conv<128, false>(ta, tb, to, cm, p, m_tiles, n_tiles, st);
 }
 
 // rows = input pixels, columns = (ky,kx,co).  The epilogue stores column pairs (co, co + 1), so Cout must be even for a
@@ -212,6 +278,7 @@ using namespace d3r;
 extern "C" void d3r_set_gemm_impl(int32_t impl) { gemm::g_impl = impl; }
 extern "C" void d3r_set_gemm_pair_min_kblocks(int32_t kb) { gemm::g_pair_min_kb = kb; }
 extern "C" void d3r_set_gemm_store(int32_t store) { gemm::g_store = store; }
+extern "C" void d3r_set_conv_store(int32_t store) { gemm::g_conv_store = store; }
 
 extern "C" int d3r_gemm_bf16(const void* A, const void* B, void* out, const float* bias, const void* add0, void* out2,
                              int32_t M, int32_t N, int32_t K, int64_t ldo, uint32_t flags, const float* rope_cos,

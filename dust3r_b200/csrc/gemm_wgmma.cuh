@@ -86,11 +86,21 @@ struct Params {
 //   EPI_RESID    out(f32) += acc + bias (the residual stream update)
 //   EPI_ACT      bias / GELU / ReLU -> bf16
 //   EPI_ROPE     bias + 2D RoPE -> bf16 (q,k,v projections)
-enum : int { EPI_GENERIC = 0, EPI_RESID = 1, EPI_ACT = 2, EPI_ROPE = 3 };
+//   EPI_CONV     the DPT 3x3 convolutions: bias, up to two bf16 addends, ReLU, raw + ReLU copy (conv_kernel only; the
+//                launch is reported as the generic epilogue, whose conv launches it replaces)
+enum : int { EPI_GENERIC = 0, EPI_RESID = 1, EPI_ACT = 2, EPI_ROPE = 3, EPI_CONV = 4 };
 template <int EPI> struct EpiMask { static constexpr uint32_t value = 0xFFFFFFFFu; };
 template <> struct EpiMask<EPI_RESID> { static constexpr uint32_t value = F_BIAS | F_RESID_INPLACE; };
 template <> struct EpiMask<EPI_ACT> { static constexpr uint32_t value = F_BIAS | F_GELU | F_RELU; };
 template <> struct EpiMask<EPI_ROPE> { static constexpr uint32_t value = F_BIAS | F_ROPE; };
+template <> struct EpiMask<EPI_CONV> { static constexpr uint32_t value = F_BIAS | F_RELU | F_ADD0 | F_ADD1 | F_OUT2_RELU; };
+
+// The conv epilogue's other NHWC tensors (B,H,W,Cout) bf16, as 4D tensor maps with boxes of 64 channels x one
+// warpgroup's 64 pixels: out2 (F_OUT2_RELU), add0 (F_ADD0), add1 (F_ADD1).  Maps a launch does not use are not read.
+struct ConvMaps {
+  CUtensorMap out2, add0, add1;
+};
+
 __host__ __device__ inline int pick_epi(int mode, uint32_t flags) {
   if (mode != 0) return EPI_GENERIC;
   if ((flags & ~F_BIAS) == F_RESID_INPLACE) return EPI_RESID;
@@ -131,14 +141,16 @@ __device__ __forceinline__ float gelu_erf(float x) {
   return fmaxf(x, 0.f) - fabsf(h);
 }
 
-// TMA_STORE (specialised epilogues at BLOCK_N = 256 only): the epilogue stages the tile in shared memory 64 rows at a
-// time and one thread per warpgroup writes it with a TMA store (bf16) or TMA reduce-add (EPI_RESID) through tmap_o, which
-// the register-store kernels do not read.
+// TMA_STORE (specialised projection epilogues at BLOCK_N = 256, the conv epilogue at BLOCK_N = 256 / 128): the epilogue
+// stages the tile in shared memory 64 rows at a time and one thread per warpgroup writes it with a TMA store (bf16) or TMA
+// reduce-add (EPI_RESID) through tmap_o, which the register-store kernels do not read.  cm: EPI_CONV only.
+// The body of gemm_kernel and conv_kernel (below): producer, main loop and every epilogue.
 template <int BLOCK_N, int EPI, bool PAIR, bool TMA_STORE>
-__global__ void __launch_bounds__(kNumThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-            const __grid_constant__ CUtensorMap tmap_o, const Params p) {
-  static_assert(!TMA_STORE || (BLOCK_N == 256 && EPI != EPI_GENERIC), "TMA-store epilogue: specialised epilogues on 128x256 tiles");
+__device__ __forceinline__ void gemm_body(const CUtensorMap& tmap_a, const CUtensorMap& tmap_b, const CUtensorMap& tmap_o,
+                                          const ConvMaps* cm, const Params& p) {
+  static_assert(EPI == EPI_CONV ? (TMA_STORE && (BLOCK_N == 256 || BLOCK_N == 128))
+                                : (!TMA_STORE || (BLOCK_N == 256 && EPI != EPI_GENERIC)),
+                "TMA-store epilogue: specialised projection epilogues on 128x256 tiles, the conv epilogue on 128x256 / 128x128");
   using C = Cfg<BLOCK_N, TMA_STORE>;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment for the 128B swizzle atoms (the same offset in both CTAs of a pair: multicast writes by offset)
@@ -149,6 +161,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + C::kRing + C::kStaging);
   uint64_t* full_bar = bars;                      // [kStages]
   uint64_t* empty_bar = bars + C::kStages;        // [kStages]
+  uint64_t* add_bar = bars + 2 * C::kStages;      // [2 warpgroups] (EPI_CONV: addend chunks landed)
   float* s_w4 = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);  // [4][128] + [4]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -168,6 +181,13 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     for (int s = 0; s < C::kStages; ++s) {
       ptx::mbar_init(ptx::smem_u32(&full_bar[s]), 1);
       ptx::mbar_init(ptx::smem_u32(&empty_bar[s]), (PAIR ? 2 : 1) * kConsumerWarps);
+    }
+    if constexpr (EPI == EPI_CONV) {
+      ptx::prefetch_tmap(&cm->out2);
+      ptx::prefetch_tmap(&cm->add0);
+      ptx::prefetch_tmap(&cm->add1);
+      ptx::mbar_init(ptx::smem_u32(&add_bar[0]), 1);
+      ptx::mbar_init(ptx::smem_u32(&add_bar[1]), 1);
     }
     ptx::fence_barrier_init();
   }
@@ -242,8 +262,38 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
         }
       }
     };
+    // EPI_CONV: this warpgroup's 64 pixels of conv tile tm are one (64 ch, bw, bh, 1) box of the NHWC output maps at
+    // (x, y, b) = conv_box(tm) (bw = min(tile_w, 64), bh = 64 / bw): row r of the box is row 64 wg + r of the tile.  Pixels
+    // past W / H, and the missing M tile of an odd count in the CTA pair, lie outside the maps and are not written.
+    const bool conv_issuer = EPI == EPI_CONV && (threadIdx.x & 127) == 0;
+    const bool conv_two = EPI == EPI_CONV && (flags & (F_OUT2_RELU | F_ADD1)) != 0;   // two staging buffers per chunk (else one, alternating)
+    const bool conv_add = EPI == EPI_CONV && (flags & (F_ADD0 | F_ADD1)) != 0;
+    uint32_t add_phase = 0;
+    auto conv_box = [&](int tm, int& bx, int& by, int& bb) {
+      bb = tm / (p.tiles_y * p.tiles_x);
+      const int r = tm - bb * (p.tiles_y * p.tiles_x);
+      bx = (r % p.tiles_x) * p.tile_w + (64 * wg) % p.tile_w;
+      by = (r / p.tiles_x) * p.tile_h + (64 * wg) / p.tile_w;
+    };
+    auto out_buf = [&](int i) { return ptx::smem_u32(smem_o + (wg * 2 + i) * C::kOutBuf); };
+    // (conv_issuer) TMA-load the addends of channels [ch, ch + 64) of tile tm into the buffer(s) that chunk is staged in, once
+    // the stores that last read them are done; completion on add_bar[wg]
+    auto issue_addends = [&](int tm, int ch) {
+      int bx, by, bb;
+      conv_box(tm, bx, by, bb);
+      const uint32_t b0 = conv_two ? out_buf(0) : out_buf(out_chunk & 1);
+      if (conv_two) ptx::bulk_wait_group_read<0>();
+      else ptx::bulk_wait_group_read<1>();
+      const uint32_t bar = ptx::smem_u32(&add_bar[wg]);
+      ptx::mbar_arrive_expect_tx(bar, uint32_t(C::kOutBuf) * (((flags & F_ADD0) ? 1u : 0u) + ((flags & F_ADD1) ? 1u : 0u)));
+      if (flags & F_ADD0) ptx::tma_load_4d(b0, &cm->add0, bar, ch, bx, by, bb);
+      if (flags & F_ADD1) ptx::tma_load_4d(out_buf(1), &cm->add1, bar, ch, bx, by, bb);
+    };
     for (int item = first_item; item < total_items; item += item_stride) {
       const int tn = item % n_tiles, tm = (item / n_tiles) * (PAIR ? 2 : 1) + int(rank);
+      if constexpr (EPI == EPI_CONV) {
+        if (conv_add && conv_issuer) issue_addends(tm, tn * BLOCK_N);   // lands while the main loop runs
+      }
       // ---- main loop: one wgmma group per k-block; a slot is released once the group after it has been issued ----
       int prev = -1;
       for (int kb = 0; kb < p.num_kb; ++kb) {
@@ -347,6 +397,57 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
             }
           }
         }
+      }
+      if constexpr (EPI == EPI_CONV) {
+        // (3) conv: the warpgroup's 64 pixels x BLOCK_N channels leave in chunks of 64 channels, one tensor-map box each,
+        //     staged in the 128B-swizzled layout of the projections' chunks below.  The addends arrive by TMA in the
+        //     buffer the chunk is staged in (add1 in the second one) and are replaced in place by the result; out2 =
+        //     relu(result) leaves through the second buffer.  With one buffer per chunk (no add1 / out2) the two buffers
+        //     alternate between chunks.  Same arithmetic order as the register path: acc + bias, + add0, + add1, ReLU.
+        int bx, by, bb;
+        conv_box(tm, bx, by, bb);
+        const uint32_t sw = lane >> 2;           // (row & 7) of both rows this thread holds
+#pragma unroll
+        for (int c = 0; c < BLOCK_N / 64; ++c) {
+          const uint32_t b0 = conv_two ? out_buf(0) : out_buf(out_chunk & 1), b1 = out_buf(1);
+          if (conv_add) {
+            ptx::mbar_wait(ptx::smem_u32(&add_bar[wg]), add_phase);
+            add_phase ^= 1;
+          } else if (conv_two) {
+            if (conv_issuer) ptx::bulk_wait_group_read<0>();   // both buffers free again
+            ptx::named_bar_sync(1 + wg, 128);
+          }
+#pragma unroll
+          for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const uint32_t off = (wq * 16 + (lane >> 2) + 8 * h) * 128 + ((j ^ sw) << 4) + q * 4;
+              float v0 = acc[4 * (c * 8 + j) + 2 * h], v1 = acc[4 * (c * 8 + j) + 2 * h + 1];
+              if (flags & F_ADD0) {
+                const float2 a = bf16x2_to_float2(ptx::ld_shared_b32(b0 + off));
+                v0 += a.x; v1 += a.y;
+              }
+              if (flags & F_ADD1) {
+                const float2 a = bf16x2_to_float2(ptx::ld_shared_b32(b1 + off));
+                v0 += a.x; v1 += a.y;
+              }
+              if (flags & F_RELU) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+              ptx::st_shared_b32(b0 + off, pack_bf16x2(v0, v1));
+              if (flags & F_OUT2_RELU) ptx::st_shared_b32(b1 + off, pack_bf16x2(fmaxf(v0, 0.f), fmaxf(v1, 0.f)));
+            }
+          ptx::fence_proxy_async();
+          if (!conv_add && !conv_two && conv_issuer) ptx::bulk_wait_group_read<0>();   // the other buffer free for chunk c + 1
+          ptx::named_bar_sync(1 + wg, 128);
+          const int ch = tn * BLOCK_N + c * 64;
+          if (conv_issuer) {
+            ptx::tma_store_4d(&tmap_o, b0, ch, bx, by, bb);
+            if (flags & F_OUT2_RELU) ptx::tma_store_4d(&cm->out2, b1, ch, bx, by, bb);
+            ptx::bulk_commit_group();
+          }
+          ++out_chunk;
+          if (conv_add && conv_issuer && c + 1 < BLOCK_N / 64) issue_addends(tm, ch + 64);
+        }
+        continue;
       }
       if constexpr (TMA_STORE) {
         // (3) staged stores: the warpgroup's 64 x 256 result leaves in chunks of 64 rows x 128 B (64 bf16 or 32 fp32
@@ -469,6 +570,22 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ 
     }
   }
   if constexpr (PAIR) ptx::cluster_sync();   // no CTA leaves while its partner may still arrive on its barriers
+}
+
+template <int BLOCK_N, int EPI, bool PAIR, bool TMA_STORE>
+__global__ void __launch_bounds__(kNumThreads, 1)
+gemm_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+            const __grid_constant__ CUtensorMap tmap_o, const Params p) {
+  gemm_body<BLOCK_N, EPI, PAIR, TMA_STORE>(tmap_a, tmap_b, tmap_o, nullptr, p);
+}
+
+// The DPT 3x3 convolutions (mode 1) with the staged conv epilogue (EPI_CONV): BLOCK_N = Cout = 256 or 128, output
+// through the 4D map tmap_o, out2 / addends through cm.
+template <int BLOCK_N, bool PAIR>
+__global__ void __launch_bounds__(kNumThreads, 1)
+conv_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
+            const __grid_constant__ CUtensorMap tmap_o, const __grid_constant__ ConvMaps cm, const Params p) {
+  gemm_body<BLOCK_N, EPI_CONV, PAIR, true>(tmap_a, tmap_b, tmap_o, &cm, p);
 }
 
 }  // namespace gemm

@@ -122,6 +122,10 @@ __device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src, int
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.tile.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(src), "r"(c0), "r"(c1) : "memory");
 }
+__device__ __forceinline__ void tma_store_4d(const void* tmap, uint32_t src, int c0, int c1, int c2, int c3) {
+  asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.tile.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+               ::"l"(reinterpret_cast<uint64_t>(tmap)), "r"(src), "r"(c0), "r"(c1), "r"(c2), "r"(c3) : "memory");
+}
 // global += shared, element-wise in the tensor map's type, performed by the memory system
 __device__ __forceinline__ void tma_reduce_add_2d(const void* tmap, uint32_t src, int c0, int c1) {
   asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
@@ -133,6 +137,11 @@ template <int N> __device__ __forceinline__ void bulk_wait_group_read() { asm vo
 // at most N of this thread's bulk groups are still incomplete (their global writes not yet performed)
 template <int N> __device__ __forceinline__ void bulk_wait_group() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
 __device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory"); }
+__device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
+  return v;
+}
 __device__ __forceinline__ void st_shared_v2_f32(uint32_t addr, float a, float b) {
   asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(a), "f"(b) : "memory");
 }

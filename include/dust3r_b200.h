@@ -300,6 +300,12 @@ void d3r_set_gemm_pair_min_kblocks(int32_t kblocks);
  * registers (A/B reference, bit-identical).  With 1, an output whose base or row stride (ldo * element size) is not a
  * multiple of 16 bytes takes the register stores. */
 void d3r_set_gemm_store(int32_t store);
+/* Selects how the 3x3 convolutions with Cout 256 or 128 (d3r_conv3x3_bf16 and the DPT head; not the head tail) run:
+ * 1 (default) = 128x256 tiles where the launch has at least 4 waves of work at that width, else 128x128, with the
+ * epilogue staged in shared memory (addends loaded into it by TMA) and written by TMA store, overlapping the next tile's
+ * main loop; 0 = 128x128 tiles whose threads load the addends and store straight from their accumulator registers (A/B
+ * reference, bit-identical).  With 1, a tensor whose base is not 16-byte aligned selects the register stores. */
+void d3r_set_conv_store(int32_t store);
 
 /* Selects the attention kernel: 3 (default) = wgmma kernel (64 query rows per warpgroup, 128-key blocks) with P kept in
  * registers (A-from-registers wgmma); 2 = the same dataflow with P through shared memory (A/B reference). */
