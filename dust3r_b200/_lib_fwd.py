@@ -85,6 +85,15 @@ def declare(lib):
     lib.d3r_forward_mixed_workspace_bytes.argtypes = [C.POINTER(Model), i32, i32, i32, i32, i32]
     lib.d3r_forward_pairs_mixed.restype = C.c_int
     lib.d3r_forward_pairs_mixed.argtypes = [C.POINTER(Model), vp, i32, i32, vp, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp]
+    lib.d3r_encode_workspace_bytes.restype = i64
+    lib.d3r_encode_workspace_bytes.argtypes = [C.POINTER(Model), i32, i32, i32]
+    lib.d3r_encode_images.restype = C.c_int
+    lib.d3r_encode_images.argtypes = [C.POINTER(Model), vp, i32, i32, i32, vp, vp, i64, vp]
+    lib.d3r_decode_workspace_bytes.restype = i64
+    lib.d3r_decode_workspace_bytes.argtypes = [C.POINTER(Model), i32, i32, i32, i32, i32]
+    lib.d3r_decode_pairs.restype = C.c_int
+    lib.d3r_decode_pairs.argtypes = [C.POINTER(Model), vp, i32, i32, i32, vp, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), i32,
+                                     vp, vp, vp, vp, vp, i64, vp]
     lib.d3r_forward_set_debug.restype = C.c_int
     lib.d3r_forward_set_debug.argtypes = [i32, vp, i64]
     lib.d3r_sizeof_model.restype = C.c_int

@@ -83,7 +83,9 @@ static int conv3(const Ctx& c, const void* x, const d3r_linear& w, int B, int H,
 }
 
 // ---- encoder ---------------------------------------------------------------------------------
-static int run_encoder(const Ctx& c, Arena& ar, const float* imgs, int n_enc, int H, int W, void** enc_out_bf16) {
+// The output (after enc_norm, bf16 [n_enc * N][E]) goes to *enc_out_bf16 when `caller_out` (memory the caller owns), else to
+// the arena, whose address is then stored in *enc_out_bf16.
+static int run_encoder(const Ctx& c, Arena& ar, const float* imgs, int n_enc, int H, int W, bool caller_out, void** enc_out_bf16) {
   const d3r_model& m = *c.m;
   const int E = m.enc_dim, M = n_enc * c.N, hid = E * m.mlp_ratio;
   float* x = ar.arr<float>((size_t)M * E);
@@ -91,8 +93,13 @@ static int run_encoder(const Ctx& c, Arena& ar, const float* imgs, int n_enc, in
   __nv_bfloat16* qkv = ar.arr<__nv_bfloat16>((size_t)M * 3 * E);
   __nv_bfloat16* att = ar.arr<__nv_bfloat16>((size_t)M * E);
   __nv_bfloat16* hidb = ar.arr<__nv_bfloat16>((size_t)M * hid);
-  __nv_bfloat16* eout = ar.arr<__nv_bfloat16>((size_t)M * E);
-  *enc_out_bf16 = eout;
+  __nv_bfloat16* eout;
+  if (caller_out) {
+    eout = reinterpret_cast<__nv_bfloat16*>(*enc_out_bf16);
+  } else {
+    eout = ar.arr<__nv_bfloat16>((size_t)M * E);
+    *enc_out_bf16 = eout;
+  }
   if (ar.dry) return D3R_OK;
   const int pk = 3 * m.patch * m.patch;
   RC(ew::patch_im2col16(imgs, hidb, n_enc, H, W, c.st));
@@ -356,18 +363,35 @@ static Ctx token_grid(const d3r_model* mp, cudaStream_t st, int H, int W) {
 static int run(const d3r_model* mp, const Call& c, Arena& ar, cudaStream_t st) {
   const Ctx cv[2] = {token_grid(mp, st, c.H[0], c.W[0]), token_grid(mp, st, c.H[1], c.W[1])};
   void* e[2] = {nullptr, nullptr};
-  RC(run_encoder(cv[0], ar, c.imgs[0], c.n_enc, c.H[0], c.W[0], &e[0]));
-  if (c.mixed) RC(run_encoder(cv[1], ar, c.imgs[1], c.n_enc, c.H[1], c.W[1], &e[1]));
+  RC(run_encoder(cv[0], ar, c.imgs[0], c.n_enc, c.H[0], c.W[0], false, &e[0]));
+  if (c.mixed) RC(run_encoder(cv[1], ar, c.imgs[1], c.n_enc, c.H[1], c.W[1], false, &e[1]));
   else e[1] = e[0];
   const void* enc[2] = {e[0], e[1]};
   const int32_t* maps[2] = {c.mixed ? nullptr : c.idx[0], c.mixed ? nullptr : c.idx[1]};
   return decode_heads(mp, cv, enc, maps, c.B, c.pts[0], c.conf[0], c.pts[1], c.conf[1], ar, st);
 }
 
+// encoder alone: n images of H x W -> their features in `feat` (caller-owned, bf16 [n * N][E])
+static int encode(const d3r_model* mp, const float* imgs, int n, int H, int W, void* feat, Arena& ar, cudaStream_t st) {
+  void* e = feat;
+  return run_encoder(token_grid(mp, st, H, W), ar, imgs, n, H, W, true, &e);
+}
+
+// decoder + heads alone: pair b is (feat1 image idx1[b], feat2 image idx2[b]), host index arrays
+static int decode(const d3r_model* mp, const void* feat1, int H1, int W1, const void* feat2, int H2, int W2, const int32_t* idx1,
+                  const int32_t* idx2, int B, float* pts1, float* conf1, float* pts2, float* conf2, Arena& ar, cudaStream_t st) {
+  const Ctx cv[2] = {token_grid(mp, st, H1, W1), token_grid(mp, st, H2, W2)};
+  const void* enc[2] = {feat1, feat2};
+  const int32_t* maps[2] = {idx1, idx2};
+  return decode_heads(mp, cv, enc, maps, B, pts1, conf1, pts2, conf2, ar, st);
+}
+
 }  // namespace fwd
 }  // namespace d3r
 
 using namespace d3r;
+
+static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 static int check_model(const d3r_model* m, int H, int W) {
   D3R_CHECK_ARG(m != nullptr, "forward: null model");
@@ -429,6 +453,68 @@ extern "C" int d3r_forward_pairs_mixed(const d3r_model* m, const float* imgs1_de
                                        float* conf_2, void* workspace_dev, int64_t workspace_bytes, void* stream) {
   const fwd::Call c{true, {imgs1_dev, imgs2_dev}, B, B, {H1, H2}, {W1, W2}, {}, {pts3d_1, pts3d_2}, {conf_1, conf_2}};
   return forward_call(m, c, workspace_dev, workspace_bytes, stream);
+}
+
+extern "C" int64_t d3r_encode_workspace_bytes(const d3r_model* m, int32_t n, int32_t H, int32_t W) {
+  if (check_model(m, H, W)) return -1;
+  if (n <= 0) {
+    set_error("encode: empty batch (n=%d)", n);
+    return -1;
+  }
+  fwd::Arena ar{nullptr, 0, 0, true};
+  if (fwd::encode(m, nullptr, n, H, W, nullptr, ar, 0)) return -1;
+  return (int64_t)ar.off + 4096;
+}
+
+extern "C" int d3r_encode_images(const d3r_model* m, const float* imgs_dev, int32_t n, int32_t H, int32_t W, void* feat_dev,
+                                 void* workspace_dev, int64_t workspace_bytes, void* stream) {
+  RC(check_model(m, H, W));
+  D3R_CHECK_ARG(imgs_dev && feat_dev && workspace_dev, "encode: null buffer");
+  D3R_CHECK_ARG(n > 0, "encode: empty batch (n=%d)", n);
+  D3R_CHECK_ARG(aligned16(imgs_dev) && aligned16(feat_dev), "encode: images and features must be 16-byte aligned");
+  const int64_t need = d3r_encode_workspace_bytes(m, n, H, W);
+  D3R_CHECK_ARG(need > 0 && workspace_bytes >= need, "encode: workspace of %lld bytes needed, %lld given", (long long)need,
+                (long long)workspace_bytes);
+  fwd::Arena ar{reinterpret_cast<uint8_t*>(workspace_dev), (size_t)workspace_bytes, 0, false};
+  const int rc = fwd::encode(m, imgs_dev, n, H, W, feat_dev, ar, (cudaStream_t)stream);
+  fwd::g_tap = {-1, nullptr, 0};
+  return rc;
+}
+
+extern "C" int64_t d3r_decode_workspace_bytes(const d3r_model* m, int32_t B, int32_t H1, int32_t W1, int32_t H2, int32_t W2) {
+  if (check_model(m, H1, W1) || check_model(m, H2, W2)) return -1;
+  if (B <= 0) {
+    set_error("decode: empty batch (B=%d)", B);
+    return -1;
+  }
+  fwd::Arena ar{nullptr, 0, 0, true};
+  if (fwd::decode(m, nullptr, H1, W1, nullptr, H2, W2, nullptr, nullptr, B, nullptr, nullptr, nullptr, nullptr, ar, 0)) return -1;
+  return (int64_t)ar.off + 4096;
+}
+
+extern "C" int d3r_decode_pairs(const d3r_model* m, const void* feat1_dev, int32_t n1, int32_t H1, int32_t W1, const void* feat2_dev,
+                                int32_t n2, int32_t H2, int32_t W2, const int32_t* idx1_host, const int32_t* idx2_host, int32_t B,
+                                float* pts3d_1, float* conf_1, float* pts3d_2, float* conf_2, void* workspace_dev,
+                                int64_t workspace_bytes, void* stream) {
+  RC(check_model(m, H1, W1));
+  RC(check_model(m, H2, W2));
+  D3R_CHECK_ARG(feat1_dev && feat2_dev && idx1_host && idx2_host && pts3d_1 && pts3d_2 && workspace_dev, "decode: null buffer");
+  D3R_CHECK_ARG(n1 > 0 && n2 > 0 && B > 0, "decode: empty batch (n1=%d, n2=%d, B=%d)", n1, n2, B);
+  // the features are gathered 16 bytes at a time, and the gathered copies are read by TMA
+  D3R_CHECK_ARG(aligned16(feat1_dev) && aligned16(feat2_dev), "decode: features must be 16-byte aligned");
+  D3R_CHECK_ARG(feat1_dev != feat2_dev || (n1 == n2 && H1 == H2 && W1 == W2),
+                "decode: one feature buffer given with two sizes (%d x %dx%d, %d x %dx%d)", n1, H1, W1, n2, H2, W2);
+  for (int b = 0; b < B; ++b)
+    D3R_CHECK_ARG(idx1_host[b] >= 0 && idx1_host[b] < n1 && idx2_host[b] >= 0 && idx2_host[b] < n2,
+                  "decode: pair %d indexes images (%d, %d) of (%d, %d)", b, idx1_host[b], idx2_host[b], n1, n2);
+  const int64_t need = d3r_decode_workspace_bytes(m, B, H1, W1, H2, W2);
+  D3R_CHECK_ARG(need > 0 && workspace_bytes >= need, "decode: workspace of %lld bytes needed, %lld given", (long long)need,
+                (long long)workspace_bytes);
+  fwd::Arena ar{reinterpret_cast<uint8_t*>(workspace_dev), (size_t)workspace_bytes, 0, false};
+  const int rc = fwd::decode(m, feat1_dev, H1, W1, feat2_dev, H2, W2, idx1_host, idx2_host, B, pts3d_1, conf_1, pts3d_2, conf_2, ar,
+                             (cudaStream_t)stream);
+  fwd::g_tap = {-1, nullptr, 0};
+  return rc;
 }
 
 extern "C" int d3r_sizeof_model(void) { return (int)sizeof(d3r_model); }

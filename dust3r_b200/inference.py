@@ -5,7 +5,9 @@ with every tensor ON CPU, concatenated over pairs in input order (lists when ima
 Differences are internal: each batch is one C-ABI call (d3r_forward_pairs), device->host copies of
 the predictions go through pinned staging buffers and overlap the next batch's compute, and
 `keep_on_device=True` (extension) skips the host round trip for callers that feed global_aligner next
-(SURVEY §8f rank 2)."""
+(SURVEY §8f rank 2).  Pair lists that share images (make_pairs) encode each image once (model.encode_images) and
+decode every batch from those features (model.decode_pairs); pair lists of several image sizes are decoded in
+batches of one (size, size) group each instead of one pair per call."""
 from __future__ import annotations
 
 import os
@@ -112,6 +114,104 @@ def _micro_batch(batch_size):
     return half + (half & 1)
 
 
+def _distinct_images(views):
+    """The distinct image tensors of single-image view dicts, by identity (make_pairs reuses one dict per image in many
+    pairs), in order of first use, and per view the index of each pair's image in that list."""
+    uniq, order, gidx = {}, [], ([], [])
+    for k in range(2):
+        for v in views[k]:
+            t = v['img']
+            key = (t.data_ptr(), tuple(t.shape), tuple(t.stride()))
+            if key not in uniq:
+                uniq[key] = len(order)
+                order.append(t)
+            gidx[k].append(uniq[key])
+    return order, gidx
+
+
+def _upload(ts, dev, up):
+    """One device tensor holding the images `ts` (each (1,3,H,W), one size), copied on the stream `up`; the current stream
+    waits for the copy."""
+    main = torch.cuda.current_stream(dev)
+    out = torch.empty((len(ts),) + tuple(ts[0].shape[1:]), dtype=ts[0].dtype, device=dev)
+    up.wait_stream(main)
+    with torch.cuda.stream(up):
+        if all(_uploadable(t, dev) for t in ts):
+            for j, t in enumerate(ts):
+                out[j:j + 1].copy_(t, non_blocking=True)
+        else:
+            stage = torch.empty(out.shape, dtype=out.dtype, pin_memory=True)
+            _fill_pinned(stage, ts, 0, wait=True)
+            out.copy_(stage, non_blocking=True)
+    ev = torch.cuda.Event()
+    ev.record(up)
+    main.wait_event(ev)
+    return out
+
+
+def _encode(model, imgs, chunk):
+    """Encoder features of every image of `imgs`, in calls of at most `chunk` images (what bounds the encoder's workspace:
+    a fused call of `chunk // 2` pairs encodes up to `chunk` images)."""
+    parts = [model.encode_images(imgs[c:c + chunk]) for c in range(0, int(imgs.shape[0]), chunk)]
+    return parts[0] if len(parts) == 1 else torch.cat(parts)
+
+
+def _inference_mixed(pairs, model, dev, batch_size, verbose, keep_on_device, return_images):
+    """Pair lists of more than one image size (one image per view dict, a model with landscape_only=False): every distinct
+    image is uploaded and encoded once, one size at a time, and the pairs of each (view-1 size, view-2 size) group are
+    decoded in input order, `batch_size` pairs per call.  The result is the reference's one-pair-per-call loop
+    (inference.py:60-72): lists with one entry per pair, in input order, with the same values -- a pair's output does not
+    depend on the batch it is computed in."""
+    n = len(pairs)
+    views = ([a for a, b in pairs], [b for a, b in pairs])
+    order, gidx = _distinct_images(views)
+    by_size = {}
+    for j, t in enumerate(order):
+        by_size.setdefault(tuple(t.shape[-2:]), []).append(j)
+    slot = [None] * len(order)   # distinct image -> (its size, its row in that size's feature tensor)
+    up = torch.cuda.Stream(device=dev)
+    imgs, feats = {}, {}
+    for hw, js in by_size.items():
+        for r, j in enumerate(js):
+            slot[j] = (hw, r)
+        imgs[hw] = _upload([order[j] for j in js], dev, up)
+        feats[hw] = _encode(model, imgs[hw], 2 * batch_size)
+        if not return_images:
+            del imgs[hw]
+        elif not keep_on_device:
+            imgs[hw] = imgs[hw].cpu()
+    groups = {}
+    for i in range(n):
+        groups.setdefault((slot[gidx[0][i]][0], slot[gidx[1][i]][0]), []).append(i)
+    preds = [None] * n
+    with tqdm.tqdm(total=n, disable=not verbose) as bar:
+        for (hw1, hw2), members in groups.items():
+            for c in range(0, len(members), batch_size):
+                sel = members[c:c + batch_size]
+                out = model.decode_pairs(feats[hw1], [slot[gidx[0][i]][1] for i in sel],
+                                         feats[hw2], [slot[gidx[1][i]][1] for i in sel])
+                out = out if keep_on_device else to_cpu(out)
+                for j, i in enumerate(sel):
+                    preds[i] = tuple({key: t[j:j + 1] for key, t in p.items()} for p in out)
+                bar.update(len(sel))
+    results = []
+    for i in range(n):
+        vs = []
+        for k in range(2):
+            v = collate_with_cat([views[k][i]])
+            if return_images:
+                hw, r = slot[gidx[k][i]]
+                v['img'] = imgs[hw][r:r + 1]
+            else:
+                del v['img']
+            if keep_on_device:   # where loss_of_one_batch puts the other fields of a view
+                v.update({key: t.to(dev, non_blocking=True) for key, t in v.items()
+                          if key != 'img' and key not in _IGNORE and torch.is_tensor(t)})
+            vs.append(v)
+        results.append(dict(view1=vs[0], view2=vs[1], pred1=preds[i][0], pred2=preds[i][1], loss=None))
+    return collate_with_cat(results, lists=True)
+
+
 @torch.no_grad()
 def inference(pairs, model, device, batch_size=8, verbose=True, keep_on_device=False, return_images=True):
     """inference.py:55-72.  Returns {'view1','view2','pred1','pred2','loss'}; tensors on CPU (pinned) unless
@@ -124,6 +224,9 @@ def inference(pairs, model, device, batch_size=8, verbose=True, keep_on_device=F
         print(f'>> Inference with model on {len(pairs)} image pairs')
     multiple_shapes = not check_if_same_size(pairs)
     dev = torch.device(device)
+    if (multiple_shapes and dev.type == 'cuda' and hasattr(model, 'decode_pairs') and not getattr(model, 'landscape_only', True)
+            and all(int(v['img'].shape[0]) == 1 for pair in pairs for v in pair)):
+        return _inference_mixed(pairs, model, dev, batch_size, verbose, keep_on_device, return_images)
     fused = dev.type == 'cuda' and not multiple_shapes and len(pairs) > 0
     if not fused:
         # mixed image sizes (batch size forced to 1, lists instead of stacked tensors) or non-CUDA stand-in
@@ -143,7 +246,7 @@ def inference(pairs, model, device, batch_size=8, verbose=True, keep_on_device=F
     proto = [vs[0]['img'] for vs in views]
     # pinned staging = the collated 'img' of the returned views; device copies of the whole pair list (a few MB / pair)
     img_pin = None    # allocated below, unless the caller does not want the images back and the upload does not stage through it
-    img_dev = None    # device copies of both views: only the non-deduplicated path needs them (allocated there)
+    img_dev = None    # device copies of both views: only the path without shared images needs them (allocated there)
     meta_all = [{key: collate_with_cat([v[key] for v in vs]) for key in vs[0] if key != 'img'} for vs in views]
     _mark('alloc+meta')
     outs = None
@@ -153,44 +256,24 @@ def inference(pairs, model, device, batch_size=8, verbose=True, keep_on_device=F
     mb = _micro_batch(batch_size)
     r0 = 0
     pending = []
-    # pair lists from make_pairs reuse the same image dict in many pairs (n images -> up to n(n-1) pairs): upload every
-    # distinct image once and let each batch address the ones it needs through index maps -- the encoder then runs once
-    # per distinct image of a batch instead of twice per pair (its output for an image does not depend on what else
-    # is in the batch, so results are unchanged)
-    uniq_dev, gidx = None, ([], [])
-    if hasattr(model, 'forward_indexed') and all(int(v['img'].shape[0]) == 1 for vs in views for v in vs):
-        uniq, order = {}, []
-        for k in range(2):
-            for v in views[k]:
-                t = v['img']
-                key = (t.data_ptr(), tuple(t.shape), tuple(t.stride()))
-                if key not in uniq:
-                    uniq[key] = len(order)
-                    order.append(t)
-                gidx[k].append(uniq[key])
+    # pair lists from make_pairs reuse the same image dict in many pairs (n images -> up to n(n-1) pairs): upload and encode
+    # every distinct image once, then decode each micro-batch from those features through index maps -- the encoder runs
+    # once per image of the list instead of twice per pair (its output for an image does not depend on what else is in
+    # the batch, so results are unchanged).  Encoder calls take at most 2 * mb images, as a fused call of mb pairs does.
+    feats, gidx = None, ([], [])
+    if hasattr(model, 'decode_pairs') and all(int(v['img'].shape[0]) == 1 for vs in views for v in vs):
+        order, gidx = _distinct_images(views)
         if len(order) < 2 * n:
-            uniq_dev = torch.empty((len(order),) + tuple(order[0].shape[1:]), dtype=order[0].dtype, device=dev)
-            up.wait_stream(main)
-            with torch.cuda.stream(up):
-                if all(_uploadable(t, dev) for t in order):
-                    for j, t in enumerate(order):
-                        uniq_dev[j:j + 1].copy_(t, non_blocking=True)
-                else:
-                    stage = torch.empty(uniq_dev.shape, dtype=uniq_dev.dtype, pin_memory=True)
-                    _fill_pinned(stage, order, 0, wait=True)
-                    uniq_dev.copy_(stage, non_blocking=True)
-            ev_uniq = torch.cuda.Event()
-            ev_uniq.record(up)
-            main.wait_event(ev_uniq)
+            feats = _encode(model, _upload(order, dev, up), 2 * mb)
     all_pinned = all(_uploadable(v['img'], dev) for vs in views for v in vs)
-    if return_images or not (uniq_dev is not None or all_pinned):
+    if return_images or not (feats is not None or all_pinned):
         img_pin = [torch.empty((rows[k],) + tuple(proto[k].shape[1:]), dtype=proto[k].dtype, pin_memory=True) for k in range(2)]
     for i in tqdm.trange(0, n, mb, disable=not verbose):
         chunk = (views[0][i:i + mb], views[1][i:i + mb])
         r1 = r0
         srcs = [[v['img'] for v in chunk[k]] for k in range(2)]
         direct = all(_uploadable(t, dev) for ts in srcs for t in ts)
-        indexed = uniq_dev is not None
+        indexed = feats is not None
         for k in range(2):
             # sources already in pinned memory are uploaded straight from where they are; the collated copy that the
             # caller gets back is then filled in the background, off the critical path
@@ -201,12 +284,8 @@ def inference(pairs, model, device, batch_size=8, verbose=True, keep_on_device=F
             pending.extend(futs)
         _mark('fill')
         if indexed:
-            g1, g2 = gidx[0][i:i + mb], gidx[1][i:i + mb]
-            ids = sorted(set(g1) | set(g2))
-            loc = {g: j for j, g in enumerate(ids)}
-            sel = uniq_dev if len(ids) == uniq_dev.shape[0] else uniq_dev.index_select(0, torch.tensor(ids, device=dev))
             _mark('h2d+meta')
-            pred1, pred2 = model.forward_indexed(sel, [loc[g] for g in g1], [loc[g] for g in g2])
+            pred1, pred2 = model.decode_pairs(feats, gidx[0][i:i + mb], feats, gidx[1][i:i + mb])
         else:
             # device staging: two micro-batch sized buffers per view, used alternately (the reference holds one batch on the
             # GPU at a time; a whole-pair-list copy would grow by 4.7 MB per pair at 512x384).  A buffer is reused two

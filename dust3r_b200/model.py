@@ -273,19 +273,50 @@ class AsymmetricCroCo3DStereo(nn.Module, _HubMixin, **_hub_kwargs):
                         out[k].index_copy_(0, seld, v.contiguous())
         return out1, out2
 
-    def forward_indexed(self, imgs, idx1, idx2):
-        """Extension used by inference(): `imgs` (n,3,H,W) are the DISTINCT images of a batch (CUDA), pair b is
-        (imgs[idx1[b]], imgs[idx2[b]]).  The encoder runs once per distinct image (the reference encodes every pair's
-        two images again, model.py:142-170; a symmetrised batch is the special case it shortcuts); decoder and heads
-        run per pair.  Same outputs as forward() on the expanded batch."""
+    @torch.no_grad()
+    def encode_images(self, imgs):
+        """Encoder features of (n,3,H,W) CUDA images, one image at a time: a bf16 CUDA tensor (n, H/16, W/16, enc_embed_dim),
+        the reference's `_encode_image` output (model.py:128-140, after enc_norm) rounded to bf16.  An image's features do
+        not depend on the other images of the call, so features encoded once can be kept and decoded in any pairing later
+        with decode_pairs() -- e.g. to add a view to a scene, encode only the new image and decode only its new pairs."""
+        if not torch.is_tensor(imgs) or imgs.dim() != 4 or int(imgs.shape[1]) != 3 or int(imgs.shape[0]) == 0:
+            raise ValueError(f'encode_images takes (n,3,H,W) images with n > 0, got {getattr(imgs, "shape", type(imgs))}')
         dev = imgs.device
         _lib.require_cuda_device(dev)
         self._ensure_packed(dev)
-        B = len(idx1)
-        assert len(idx2) == B and B > 0
-        H, W = int(imgs.shape[-2]), int(imgs.shape[-1])
-        return _in_other_view(self._packed.forward(imgs.float().contiguous(), np.asarray(idx1, dtype=np.int32),
-                                                   np.asarray(idx2, dtype=np.int32), B, H, W))
+        return self._packed.encode(imgs.float().contiguous())
+
+    @torch.no_grad()
+    def decode_pairs(self, feat1, idx1, feat2, idx2):
+        """Decoders and heads for the pairs (feat1[idx1[b]], feat2[idx2[b]]) of features made by encode_images().  Returns
+        (res1, res2) like forward(): res1 {'pts3d', 'conf'} in view 1's frame, res2 {'pts3d_in_other_view', 'conf'}.  The
+        image sizes are read from the features' shapes (patch 16); the two feature tensors may hold images of different
+        sizes, as forward() allows for the two views of a batch."""
+        E = self.enc_embed_dim
+        for name, f in (('feat1', feat1), ('feat2', feat2)):
+            if not torch.is_tensor(f) or f.dtype != torch.bfloat16 or f.dim() != 4 or int(f.shape[-1]) != E or int(f.shape[0]) == 0:
+                raise ValueError(f'{name} must be encode_images() output, a bf16 tensor (n, H/16, W/16, {E}) with n > 0; got '
+                                 f'{getattr(f, "dtype", type(f))} {tuple(getattr(f, "shape", ()))}')
+            if not f.is_cuda:
+                raise ValueError(f'{name} lives on {f.device}: features are CUDA tensors')
+            if self.landscape_only and int(f.shape[1]) > int(f.shape[2]):
+                raise ValueError(f'{name}: portrait features on a landscape_only model (forward() would reject the images)')
+        if feat1.device != feat2.device:
+            raise ValueError(f'feat1 on {feat1.device}, feat2 on {feat2.device}')
+        idx = []
+        for name, ix, f in (('idx1', idx1, feat1), ('idx2', idx2, feat2)):
+            ix = torch.as_tensor(ix).reshape(-1).cpu()
+            if ix.dtype.is_floating_point or ix.dtype.is_complex or ix.dtype == torch.bool:
+                raise ValueError(f'{name} must hold integer indices, got {ix.dtype}')
+            if ix.numel() and (int(ix.min()) < 0 or int(ix.max()) >= int(f.shape[0])):
+                raise ValueError(f'{name} indexes outside [0, {int(f.shape[0])})')
+            idx.append(ix.to(torch.int32).numpy())
+        if len(idx[0]) != len(idx[1]) or len(idx[0]) == 0:
+            raise ValueError(f'idx1 and idx2 must have the same, non-zero length ({len(idx[0])} vs {len(idx[1])})')
+        dev = feat1.device
+        _lib.require_cuda_device(dev)
+        self._ensure_packed(dev)
+        return _in_other_view(self._packed.decode(feat1.contiguous(), idx[0], feat2.contiguous(), idx[1]))
 
 
 def _in_other_view(res):
@@ -422,31 +453,67 @@ class _PackedModel:
             m.lin_head[0] = lin('downstream_head1.proj')
             m.lin_head[1] = lin('downstream_head2.proj')
         self.cmodel = m
-        self._ws = None
-        self._ws_key = None
+        self._ws = {}   # kind of call -> (shape key, workspace)
 
-    def _run(self, launch, query, dims, inputs, B, sizes, debug=None):
-        """One call of d3r_forward_pairs / d3r_forward_pairs_mixed (`launch`): the workspace, sized by `query` on the
-        call's shape `dims` and kept while the shape stays the same, and one ({'pts3d','conf'}) dict per view."""
+    def _workspace(self, kind, query, dims):
+        """The device workspace of one kind of call ('forward' for both fused calls, 'encode', 'decode'), sized by `query` on
+        the call's shape `dims` and kept while that shape stays the same.  Each kind keeps its own, so alternating encode and
+        decode calls do not reallocate."""
         key = (query.__name__,) + dims
-        if self._ws_key != key:
+        cur = self._ws.get(kind)
+        if cur is None or cur[0] != key:
             need = query(C.byref(self.cmodel), *dims)
             if need <= 0:
                 _lib.check(-1)
-            self._ws = None   # free the old one first
-            self._ws = torch.empty((need,), dtype=torch.uint8, device=self.device)
-            self._ws_key = key
+            self._ws.pop(kind, None)   # free the old one first
+            cur = self._ws[kind] = (key, torch.empty((need,), dtype=torch.uint8, device=self.device))
+        return cur[1]
+
+    def _outputs(self, B, sizes):
+        """One ({'pts3d', 'conf'}) dict of fp32 CUDA tensors per view; `conf` only with a confidence channel."""
         dev = self.device
         res = tuple({'pts3d': torch.empty((B, H, W, 3), dtype=torch.float32, device=dev)} for H, W in sizes)
         if self.cmodel.nch > 3:
             for r, (H, W) in zip(res, sizes):
                 r['conf'] = torch.empty((B, H, W), dtype=torch.float32, device=dev)
+        return res
+
+    def _run(self, launch, query, dims, inputs, B, sizes, debug=None):
+        """One call of d3r_forward_pairs / d3r_forward_pairs_mixed (`launch`) into fresh outputs."""
+        ws = self._workspace('forward', query, dims)
+        res = self._outputs(B, sizes)
         if debug is not None:
             stage, buf = debug
             _lib.check(self.lib.d3r_forward_set_debug(stage, buf.data_ptr(), buf.numel()))
         outs = [r[k].data_ptr() if k in r else None for r in res for k in ('pts3d', 'conf')]
-        with torch.cuda.device(dev):
-            _lib.check(launch(C.byref(self.cmodel), *inputs, *outs, self._ws.data_ptr(), self._ws.numel(), _lib.stream_ptr()))
+        with torch.cuda.device(self.device):
+            _lib.check(launch(C.byref(self.cmodel), *inputs, *outs, ws.data_ptr(), ws.numel(), _lib.stream_ptr()))
+        return res
+
+    def encode(self, imgs):
+        """imgs (n,3,H,W) fp32 CUDA -> features (n, H/16, W/16, enc_dim) bf16 CUDA (d3r_encode_images)."""
+        n, H, W = int(imgs.shape[0]), int(imgs.shape[-2]), int(imgs.shape[-1])
+        p = self.cfg.patch_size
+        ws = self._workspace('encode', self.lib.d3r_encode_workspace_bytes, (n, H, W))
+        feat = torch.empty((n, H // p, W // p, self.cfg.enc_embed_dim), dtype=torch.bfloat16, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.d3r_encode_images(C.byref(self.cmodel), imgs.data_ptr(), n, H, W, feat.data_ptr(), ws.data_ptr(),
+                                                  ws.numel(), _lib.stream_ptr()))
+        return feat
+
+    def decode(self, feat1, idx1, feat2, idx2):
+        """Pairs (feat1[idx1[b]], feat2[idx2[b]]) of (n, H/16, W/16, enc_dim) bf16 CUDA features, idx int32 host arrays ->
+        ({'pts3d','conf'}, {'pts3d','conf'}) (d3r_decode_pairs)."""
+        p, B = self.cfg.patch_size, len(idx1)
+        (n1, H1, W1), (n2, H2, W2) = [(int(f.shape[0]), int(f.shape[1]) * p, int(f.shape[2]) * p) for f in (feat1, feat2)]
+        ws = self._workspace('decode', self.lib.d3r_decode_workspace_bytes, (B, H1, W1, H2, W2))
+        res = self._outputs(B, ((H1, W1), (H2, W2)))
+        outs = [r[k].data_ptr() if k in r else None for r in res for k in ('pts3d', 'conf')]
+        i1 = (C.c_int32 * B)(*[int(v) for v in idx1])
+        i2 = (C.c_int32 * B)(*[int(v) for v in idx2])
+        with torch.cuda.device(self.device):
+            _lib.check(self.lib.d3r_decode_pairs(C.byref(self.cmodel), feat1.data_ptr(), n1, H1, W1, feat2.data_ptr(), n2, H2, W2,
+                                                 i1, i2, B, *outs, ws.data_ptr(), ws.numel(), _lib.stream_ptr()))
         return res
 
     def forward_mixed(self, imgs1, imgs2):

@@ -446,6 +446,23 @@ int d3r_forward_pairs_mixed(const d3r_model* m, const float* imgs1_dev, int32_t 
                             int32_t H2, int32_t W2, int32_t B, float* pts3d_1, float* conf_1, float* pts3d_2,
                             float* conf_2, void* workspace_dev, int64_t workspace_bytes, void* stream);
 
+/* The two halves of d3r_forward_pairs, for callers that keep encoder features between calls (each image of a
+ * multi-view scene encoded once, however many pairs it appears in; pairs of two image sizes batched).
+ * d3r_encode_images: imgs (n,3,H,W) fp32 in [-1,1] -> feat (n, H/16, W/16, enc_dim) bf16, caller-owned: the
+ * encoder's output after enc_norm (model.py:128-140), the tensor the decoder and DPT hook 0 read.
+ * d3r_decode_pairs: decoders + heads for B pairs; pair b is (image idx1[b] of feat1, image idx2[b] of feat2),
+ * idx HOST int32[B], indices in [0, n1) / [0, n2).  feat1 and feat2 may be the same buffer when the sizes are equal.
+ * Features must be 16-byte aligned.  Outputs as d3r_forward_pairs_mixed (sizes H1 x W1 for view 1, H2 x W2 for
+ * view 2).  Debug taps 1-4 apply to the encode call, 5 and up to the decode call. */
+int64_t d3r_encode_workspace_bytes(const d3r_model* m, int32_t n, int32_t H, int32_t W);
+int d3r_encode_images(const d3r_model* m, const float* imgs_dev, int32_t n, int32_t H, int32_t W, void* feat_dev,
+                      void* workspace_dev, int64_t workspace_bytes, void* stream);
+int64_t d3r_decode_workspace_bytes(const d3r_model* m, int32_t B, int32_t H1, int32_t W1, int32_t H2, int32_t W2);
+int d3r_decode_pairs(const d3r_model* m, const void* feat1_dev, int32_t n1, int32_t H1, int32_t W1, const void* feat2_dev,
+                     int32_t n2, int32_t H2, int32_t W2, const int32_t* idx1_host, const int32_t* idx2_host, int32_t B,
+                     float* pts3d_1, float* conf_1, float* pts3d_2, float* conf_2, void* workspace_dev,
+                     int64_t workspace_bytes, void* stream);
+
 /* Optional taps for the parity tests: when non-NULL, fp32 copies of intermediate stages are written.
  * (set with d3r_forward_set_debug before a call; cleared after it).  stage ids in DESIGN.md. */
 int d3r_forward_set_debug(int32_t stage_id, float* out_dev, int64_t capacity_floats);

@@ -42,7 +42,7 @@ def forward(Bp):
         idx1, idx2 = np.arange(B, dtype=np.int32), B + np.arange(B, dtype=np.int32)
         ms = timeit(lambda: packed.forward(imgs, idx1, idx2, B, H, W), warm=2, rep=3)
         print(json.dumps(dict(kind='forward', B=B, ms=ms, pairs_per_s=B / ms * 1e3, tflops_alg=B * 1856.8 / ms)), flush=True)
-        packed._ws = None; packed._ws_key = None
+        packed._ws.clear()
 
 if __name__ == '__main__':
     lib = _lib.get_lib()
