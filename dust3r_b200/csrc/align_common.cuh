@@ -81,6 +81,11 @@ __device__ __forceinline__ float fix_get(const long long* src, int& bad) {
 __device__ __forceinline__ void fix_report(int bad, int* overflow_flag) {
   if (bad) *overflow_flag = 1;
 }
+// A launch whose sums left the range (or met a NaN / Inf) reports NaN instead of a finite loss and gradient: fix_add
+// turns a NaN partial into an ordinary integer, so the sums themselves no longer show it.  The last CTA reads the flag
+// with ld.global.cg after the grid ticket, like the accumulators, and ORs it with its own range checks.
+__device__ __forceinline__ int overflow_seen(const Workspace& ws) { return __ldcg(ws.flags); }
+__device__ __forceinline__ float nan_if(bool poison, float v) { return poison ? __int_as_float(0x7fffffff) : v; }
 
 // Grid ticket: release this CTA's accumulations / log-depth updates and acquire everybody else's in ONE operation by one
 // thread (the CTA barrier before / after it extends both to the other threads by cumulativity).  What the last CTA then reads
@@ -371,10 +376,9 @@ static __device__ __noinline__ void small_param_step(const d3r_align_desc& D, co
 
   // phase 0: loss (fixed order over entries), one barrier
   float lpart = 0.f;
-  int bad = 0;
+  int bad = threadIdx.x == 0 ? overflow_seen(ws) : 0;
   for (int k = threadIdx.x; k < 2 * E; k += blockDim.x) lpart += fix_get(ws.ent_acc + k * kEntVals + 12, bad);
   const float loss = block_sum8(lpart, s_red);
-  if (threadIdx.x == 0) D.loss_out[it] = loss;
   D3R_TSTAMP(0);
 
   // phase 1: gradients -> ws.grad.  edges on low thread ids, images on high thread ids (different warps).
@@ -397,6 +401,8 @@ static __device__ __noinline__ void small_param_step(const d3r_align_desc& D, co
     }
   }
   fix_report(bad, ws.flags);
+  const bool poison = __syncthreads_or(bad);
+  if (threadIdx.x == 0) D.loss_out[it] = nan_if(poison, loss);
   D3R_TSTAMP(1);
   // zero the accumulators for the next launch (everything has been read above; barrier inside block_sum8)
   const float coupling = block_sum8(coupl, s_red + 16) / float(E);
@@ -437,10 +443,9 @@ static __device__ __noinline__ void small_grad_step(const d3r_align_desc& D, con
   const int n = D.n_imgs, E = D.n_edges;
   const SmallLayout L(n, E);
   float lpart = 0.f;
-  int bad = 0;
+  int bad = threadIdx.x == 0 ? overflow_seen(ws) : 0;
   for (int k = threadIdx.x; k < 2 * E; k += blockDim.x) lpart += fix_get(ws.ent_acc + k * kEntVals + 12, bad);
   const float loss = block_sum8(lpart, s_red);
-  if (threadIdx.x == 0) D.loss_out[0] = loss;
 
   float coupl = 0.f;
   for (int e = threadIdx.x; e < E; e += blockDim.x) {
@@ -463,10 +468,17 @@ static __device__ __noinline__ void small_grad_step(const d3r_align_desc& D, con
     image_grad(D, L, i, S, c, go.small_grad);
   }
   fix_report(bad, ws.flags);
+  const bool poison = __syncthreads_or(bad);
+  if (threadIdx.x == 0) D.loss_out[0] = nan_if(poison, loss);
   // every accumulator has been read (barrier inside block_sum8): fold in the coupling, clear for the next launch
   const float coupling = block_sum8(coupl, s_red + 16) / float(E);
-  if (D.norm_pw_scale)
+  if (poison) {            // every gradient and entry loss of the launch is NaN (the barriers above ordered the writes)
+    for (int k = threadIdx.x; k < L.total; k += blockDim.x) go.small_grad[k] = nan_if(true, 0.f);
+    if (go.entry_loss)
+      for (int k = threadIdx.x; k < 2 * E; k += blockDim.x) go.entry_loss[k] = nan_if(true, 0.f);
+  } else if (D.norm_pw_scale) {
     for (int e = threadIdx.x; e < E; e += blockDim.x) go.small_grad[L.pw + e * 8 + 7] -= coupling;   // written by this thread above
+  }
   for (int k = threadIdx.x; k < 2 * E * kEntVals; k += blockDim.x) ws.ent_acc[k] = 0;
   for (int k = threadIdx.x; k < n * kImgVals; k += blockDim.x) ws.img_acc[k] = 0;
 }
@@ -508,7 +520,7 @@ static __device__ __forceinline__ void small_param_step_fast(const d3r_align_des
 
   // ---- stage A
   float lpart = 0.f, coupl = 0.f;
-  int bad = 0;
+  int bad = tid == 0 ? overflow_seen(ws) : 0;
   if (has_e) {
     const int ei = D.edge_ent[e * 2 + 0], ej = D.edge_ent[e * 2 + 1];
     float c[kGeomE];
@@ -536,12 +548,12 @@ static __device__ __forceinline__ void small_param_step_fast(const d3r_align_des
   coupl = warp_sum(coupl);
   if ((tid & 31) == 0) { s_red[tid >> 5] = lpart; s_red[8 + (tid >> 5)] = coupl; }
   D3R_TSTAMP(0);
-  __syncthreads();
+  const bool poison = __syncthreads_or(bad);
   float loss = 0.f, coupling = 0.f;
 #pragma unroll
   for (int w = 0; w < kWarps; ++w) { loss += s_red[w]; coupling += s_red[8 + w]; }
   coupling /= float(E);
-  if (tid == 0) D.loss_out[it] = loss;
+  if (tid == 0) D.loss_out[it] = nan_if(poison, loss);
   D3R_TSTAMP(1);
 
   // ---- stage B: Adam, one thread per parameter

@@ -173,11 +173,14 @@ int d3r_align_run(const d3r_align_desc* desc, int32_t it_begin, int32_t it_end, 
  * not written: pass a zeroed buffer).  small_grad [11n+10E]: dL/d(raw parameter) in the `small` layout, complete: log-scale
  * mean coupling and adaptor mean removal folded in; with tied focals both focal slots hold the full dL/dfocal.  Gradients of
  * every parameter, whatever small_trainable says.  entry_loss (may be NULL) [E][2]: coefficient-weighted loss of (edge, side).
- * Sets the overflow flag like a run; leaves the accumulators cleared, so a following d3r_align_run is unaffected. */
+ * Sets the overflow flag like a run; leaves the accumulators cleared, so a following d3r_align_run is unaffected.  When the
+ * flag is set (a NaN / Inf observation, or a sum out of the fixed-point range), loss_out[0], every element of small_grad and
+ * of entry_loss are NaN, so that an out-of-range scene never returns a finite objective without a host check. */
 int d3r_align_loss_grad(const d3r_align_desc* desc, float* logd_grad, float* small_grad, float* entry_loss, void* stream);
 /* Cross-CTA sums use order-independent 2^40 fixed-point integer atomics (bit-reproducible).  *host_out = 1 when a
  * partial sum (|x| >= 2^18) or a total (|x| >= 2^22) left the supported range (unreasonably scaled scene, NaN / Inf input)
- * since iteration 0 of the current d3r_align_run batch. */
+ * since iteration 0 of the current d3r_align_run batch, or during the last d3r_align_loss_grad.  Every iteration from the one
+ * that set it writes NaN to loss_out (eval_only runs included). */
 int d3r_align_overflow_flag(const d3r_align_desc* desc, int32_t* host_out, void* stream);
 /* World-frame pointmaps X[i] = R_i * unproject(depth_i) + T_i for every image
  * (PointCloudOptimizer.depth_to_pts3d, optimizer.py:170-180).  out: [sum P_i][3] float. */

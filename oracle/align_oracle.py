@@ -140,7 +140,8 @@ def unproject(prob, im_depthmaps, im_poses, im_focals, im_pp):
     out = []
     for i, (H, W) in enumerate(prob.imshapes):
         d = im_depthmaps[i].exp()
-        v, u = torch.meshgrid(torch.arange(H, dtype=torch.float32), torch.arange(W, dtype=torch.float32), indexing='ij')
+        dt = d.dtype               # float32 for the oracle itself; float64 when the float64 tests evaluate it
+        v, u = torch.meshgrid(torch.arange(H, dtype=dt), torch.arange(W, dtype=dt), indexing='ij')
         cx = W / 2 + 10 * im_pp[i, 0]
         cy = H / 2 + 10 * im_pp[i, 1]
         fx, fy = f[i, 0], f[i, -1]
