@@ -76,15 +76,6 @@ def declare(lib):
     lib.d3r_set_conv_store.argtypes = [i32]
     lib.d3r_set_attention_impl.restype = None
     lib.d3r_set_attention_impl.argtypes = [i32]
-    lib.d3r_forward_workspace_bytes.restype = i64
-    lib.d3r_forward_workspace_bytes.argtypes = [C.POINTER(Model), i32, i32, i32, i32]
-    lib.d3r_forward_pairs.restype = C.c_int
-    lib.d3r_forward_pairs.argtypes = [C.POINTER(Model), vp, i32, C.POINTER(i32), C.POINTER(i32), i32, i32, i32,
-                                      vp, vp, vp, vp, vp, i64, vp]
-    lib.d3r_forward_mixed_workspace_bytes.restype = i64
-    lib.d3r_forward_mixed_workspace_bytes.argtypes = [C.POINTER(Model), i32, i32, i32, i32, i32]
-    lib.d3r_forward_pairs_mixed.restype = C.c_int
-    lib.d3r_forward_pairs_mixed.argtypes = [C.POINTER(Model), vp, i32, i32, vp, i32, i32, i32, vp, vp, vp, vp, vp, i64, vp]
     lib.d3r_encode_workspace_bytes.restype = i64
     lib.d3r_encode_workspace_bytes.argtypes = [C.POINTER(Model), i32, i32, i32]
     lib.d3r_encode_images.restype = C.c_int

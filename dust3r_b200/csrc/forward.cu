@@ -1,5 +1,6 @@
 // Pairwise forward orchestration (host side, C++): replaces AsymmetricCroCo3DStereo.forward
-// (dust3r/model.py:199-211) for one batch of same-sized pairs with a fixed launch sequence on ONE stream:
+// (dust3r/model.py:199-211) with two calls, each a fixed launch sequence on ONE stream: d3r_encode_images (encoder,
+// output in caller memory) and d3r_decode_pairs (decoders + heads for pairs addressed by index maps into the features):
 //
 //   encoder   patch im2col -> GEMM(+bias)->x(f32) ; 24 x { LN -> GEMM(qkv,+bias,+RoPE) -> attention ->
 //             GEMM(proj,+bias,+=x) -> LN -> GEMM(fc1,+bias,GELU) -> GEMM(fc2,+bias,+=x) } ; LN(enc_norm)
@@ -83,25 +84,17 @@ static int conv3(const Ctx& c, const void* x, const d3r_linear& w, int B, int H,
 }
 
 // ---- encoder ---------------------------------------------------------------------------------
-// The output (after enc_norm, bf16 [n_enc * N][E]) goes to *enc_out_bf16 when `caller_out` (memory the caller owns), else to
-// the arena, whose address is then stored in *enc_out_bf16.
-static int run_encoder(const Ctx& c, Arena& ar, const float* imgs, int n_enc, int H, int W, bool caller_out, void** enc_out_bf16) {
+// The output (after enc_norm, bf16 [n_enc * N][E]) goes to `eout`, memory the caller owns.
+static int run_encoder(const Ctx& c, Arena& ar, const float* imgs, int n_enc, int H, int W, __nv_bfloat16* eout) {
   const d3r_model& m = *c.m;
-  const int E = m.enc_dim, M = n_enc * c.N, hid = E * m.mlp_ratio;
+  const int E = m.enc_dim, M = n_enc * c.N, hid = E * m.mlp_ratio, pk = 3 * m.patch * m.patch;
   float* x = ar.arr<float>((size_t)M * E);
   __nv_bfloat16* ln = ar.arr<__nv_bfloat16>((size_t)M * E);
   __nv_bfloat16* qkv = ar.arr<__nv_bfloat16>((size_t)M * 3 * E);
   __nv_bfloat16* att = ar.arr<__nv_bfloat16>((size_t)M * E);
-  __nv_bfloat16* hidb = ar.arr<__nv_bfloat16>((size_t)M * hid);
-  __nv_bfloat16* eout;
-  if (caller_out) {
-    eout = reinterpret_cast<__nv_bfloat16*>(*enc_out_bf16);
-  } else {
-    eout = ar.arr<__nv_bfloat16>((size_t)M * E);
-    *enc_out_bf16 = eout;
-  }
+  // hidb holds the patch im2col [M][pk] first, the MLP hidden [M][hid] after: pk > hid for a narrow encoder (E < 192)
+  __nv_bfloat16* hidb = ar.arr<__nv_bfloat16>((size_t)M * (hid > pk ? hid : pk));
   if (ar.dry) return D3R_OK;
-  const int pk = 3 * m.patch * m.patch;
   RC(ew::patch_im2col16(imgs, hidb, n_enc, H, W, c.st));
   RC(linear(c, hidb, pk, m.patch_embed, M, E, pk, x, gemm::F_OUT_F32));
   tap_f32(1, x, (size_t)M * E, c.st);
@@ -238,7 +231,7 @@ static int run_dpt(const Ctx& c, Arena& ar, const d3r_dpt_head& hd, const void* 
 }
 
 // decoder + heads.  cv[br]: token grid of view br; enc[br]: encoder output holding view br's images; maps_host[br]: image
-// index of each pair inside enc[br] (nullptr = identity, pair b uses image b).
+// index of each pair inside enc[br] (host array).
 static int decode_heads(const d3r_model* mp, const Ctx cv[2], const void* const enc[2], const int32_t* const maps_host[2], int B,
                         float* pts1, float* conf1, float* pts2, float* conf2, Arena& ar, cudaStream_t st) {
   const d3r_model& m = *mp;
@@ -289,12 +282,8 @@ static int decode_heads(const d3r_model* mp, const Ctx cv[2], const void* const 
   }
 
   for (int br = 0; br < 2; ++br) {
-    if (maps_host[br]) {
-      D3R_CUDA(cudaMemcpyAsync(maps + br * B, maps_host[br], sizeof(int) * B, cudaMemcpyHostToDevice, st));
-      RC(ew::gather_images_bf16(enc[br], f[br], maps + br * B, B, cv[br].N, E, st));
-    } else {
-      D3R_CUDA(cudaMemcpyAsync(f[br], enc[br], sizeof(bf) * (size_t)Md[br] * E, cudaMemcpyDeviceToDevice, st));
-    }
+    D3R_CUDA(cudaMemcpyAsync(maps + br * B, maps_host[br], sizeof(int) * B, cudaMemcpyHostToDevice, st));
+    RC(ew::gather_images_bf16(enc[br], f[br], maps + br * B, B, cv[br].N, E, st));
   }
 
   // decoder (model.py:172-191)
@@ -343,38 +332,13 @@ static int decode_heads(const d3r_model* mp, const Ctx cv[2], const void* const 
   return D3R_OK;
 }
 
-// One forward call.  Same-size (!mixed): imgs[0] holds n_enc images of H[0] x W[0] (H[1], W[1] equal), and pair b is
-// (image idx[0][b], image idx[1][b]), host arrays.  Mixed (two image sizes): imgs[br] holds the n_enc = B views br of
-// H[br] x W[br]; the reference encodes them separately (model.py:147-151) and the decoder cross-attends between the two
-// token grids.  Null pointers throughout for a dry (size-only) pass.
-struct Call {
-  bool mixed;
-  const float* imgs[2];
-  int n_enc, B, H[2], W[2];
-  const int32_t* idx[2];
-  float *pts[2], *conf[2];
-};
-
 static Ctx token_grid(const d3r_model* mp, cudaStream_t st, int H, int W) {
   return Ctx{mp, st, H / mp->patch, W / mp->patch, (H / mp->patch) * (W / mp->patch)};
 }
 
-// same-size: one encoder pass over the n_enc distinct images, index gathers; mixed: one encoder pass per view, identity copies
-static int run(const d3r_model* mp, const Call& c, Arena& ar, cudaStream_t st) {
-  const Ctx cv[2] = {token_grid(mp, st, c.H[0], c.W[0]), token_grid(mp, st, c.H[1], c.W[1])};
-  void* e[2] = {nullptr, nullptr};
-  RC(run_encoder(cv[0], ar, c.imgs[0], c.n_enc, c.H[0], c.W[0], false, &e[0]));
-  if (c.mixed) RC(run_encoder(cv[1], ar, c.imgs[1], c.n_enc, c.H[1], c.W[1], false, &e[1]));
-  else e[1] = e[0];
-  const void* enc[2] = {e[0], e[1]};
-  const int32_t* maps[2] = {c.mixed ? nullptr : c.idx[0], c.mixed ? nullptr : c.idx[1]};
-  return decode_heads(mp, cv, enc, maps, c.B, c.pts[0], c.conf[0], c.pts[1], c.conf[1], ar, st);
-}
-
 // encoder alone: n images of H x W -> their features in `feat` (caller-owned, bf16 [n * N][E])
 static int encode(const d3r_model* mp, const float* imgs, int n, int H, int W, void* feat, Arena& ar, cudaStream_t st) {
-  void* e = feat;
-  return run_encoder(token_grid(mp, st, H, W), ar, imgs, n, H, W, true, &e);
+  return run_encoder(token_grid(mp, st, H, W), ar, imgs, n, H, W, reinterpret_cast<__nv_bfloat16*>(feat));
 }
 
 // decoder + heads alone: pair b is (feat1 image idx1[b], feat2 image idx2[b]), host index arrays
@@ -403,56 +367,6 @@ static int check_model(const d3r_model* m, int H, int W) {
   D3R_CHECK_ARG(m->head_type == 0 || m->head_type == 1, "forward: bad head type");
   D3R_CHECK_ARG(m->head_type == 0 || (m->enc_dim % 32 == 0 && m->dpt[0] && m->dpt[1]), "forward: missing DPT weights");
   return D3R_OK;
-}
-
-static int check_sizes(const d3r_model* m, const fwd::Call& c) {
-  RC(check_model(m, c.H[0], c.W[0]));
-  return c.mixed ? check_model(m, c.H[1], c.W[1]) : D3R_OK;
-}
-
-static int64_t workspace_bytes(const d3r_model* m, const fwd::Call& c) {
-  if (check_sizes(m, c)) return -1;
-  fwd::Arena ar{nullptr, 0, 0, true};
-  if (fwd::run(m, c, ar, 0)) return -1;
-  return (int64_t)ar.off + 4096;
-}
-
-static int forward_call(const d3r_model* m, const fwd::Call& c, void* workspace_dev, int64_t workspace_bytes_given, void* stream) {
-  RC(check_sizes(m, c));
-  D3R_CHECK_ARG(c.imgs[0] && c.imgs[1] && (c.mixed || (c.idx[0] && c.idx[1])) && c.pts[0] && c.pts[1] && workspace_dev,
-                "forward: null buffer");
-  D3R_CHECK_ARG(c.n_enc > 0 && c.B > 0, "forward: empty batch");
-  for (int b = 0; !c.mixed && b < c.B; ++b)
-    D3R_CHECK_ARG(c.idx[0][b] >= 0 && c.idx[0][b] < c.n_enc && c.idx[1][b] >= 0 && c.idx[1][b] < c.n_enc, "forward: pair index out of range");
-  const int64_t need = workspace_bytes(m, c);
-  D3R_CHECK_ARG(need > 0 && workspace_bytes_given >= need, "forward: workspace of %lld bytes needed, %lld given", (long long)need,
-                (long long)workspace_bytes_given);
-  fwd::Arena ar{reinterpret_cast<uint8_t*>(workspace_dev), (size_t)workspace_bytes_given, 0, false};
-  const int rc = fwd::run(m, c, ar, (cudaStream_t)stream);
-  fwd::g_tap = {-1, nullptr, 0};
-  return rc;
-}
-
-extern "C" int64_t d3r_forward_workspace_bytes(const d3r_model* m, int32_t n_enc, int32_t B, int32_t H, int32_t W) {
-  return workspace_bytes(m, fwd::Call{false, {}, n_enc, B, {H, H}, {W, W}, {}, {}, {}});
-}
-
-extern "C" int d3r_forward_pairs(const d3r_model* m, const float* imgs_dev, int32_t n_enc, const int32_t* idx1_host,
-                                 const int32_t* idx2_host, int32_t B, int32_t H, int32_t W, float* pts3d_1, float* conf_1,
-                                 float* pts3d_2, float* conf_2, void* workspace_dev, int64_t workspace_bytes, void* stream) {
-  const fwd::Call c{false, {imgs_dev, imgs_dev}, n_enc, B, {H, H}, {W, W}, {idx1_host, idx2_host}, {pts3d_1, pts3d_2}, {conf_1, conf_2}};
-  return forward_call(m, c, workspace_dev, workspace_bytes, stream);
-}
-
-extern "C" int64_t d3r_forward_mixed_workspace_bytes(const d3r_model* m, int32_t B, int32_t H1, int32_t W1, int32_t H2, int32_t W2) {
-  return workspace_bytes(m, fwd::Call{true, {}, B, B, {H1, H2}, {W1, W2}, {}, {}, {}});
-}
-
-extern "C" int d3r_forward_pairs_mixed(const d3r_model* m, const float* imgs1_dev, int32_t H1, int32_t W1, const float* imgs2_dev,
-                                       int32_t H2, int32_t W2, int32_t B, float* pts3d_1, float* conf_1, float* pts3d_2,
-                                       float* conf_2, void* workspace_dev, int64_t workspace_bytes, void* stream) {
-  const fwd::Call c{true, {imgs1_dev, imgs2_dev}, B, B, {H1, H2}, {W1, W2}, {}, {pts3d_1, pts3d_2}, {conf_1, conf_2}};
-  return forward_call(m, c, workspace_dev, workspace_bytes, stream);
 }
 
 extern "C" int64_t d3r_encode_workspace_bytes(const d3r_model* m, int32_t n, int32_t H, int32_t W) {

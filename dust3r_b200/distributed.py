@@ -74,7 +74,7 @@ class PairOutputGather:
         off = 0
         for which, key, w, _ in self.cols:
             if w and preds[which] is not None:
-                # the fused forward names view 2's pointmap 'pts3d' until model.forward() renames it (model.py:199-211)
+                # the packed model's forward names view 2's pointmap 'pts3d' until model.forward() renames it (model.py:199-211)
                 t = preds[which][key] if key in preds[which] else preds[which]['pts3d']
                 send[:t.shape[0], off:off + w].copy_(t.reshape(t.shape[0], w), non_blocking=True)
             off += w

@@ -2,8 +2,8 @@
 
 Same contract as the reference: takes the `make_pairs` list, returns {'view1','view2','pred1','pred2','loss'}
 with every tensor ON CPU, concatenated over pairs in input order (lists when image sizes are mixed).
-Differences are internal: each batch is one C-ABI call (d3r_forward_pairs), device->host copies of
-the predictions go through pinned staging buffers and overlap the next batch's compute, and
+Differences are internal: each batch runs as C-ABI encode and decode calls (d3r_encode_images, d3r_decode_pairs),
+device->host copies of the predictions go through pinned staging buffers and overlap the next batch's compute, and
 `keep_on_device=True` (extension) skips the host round trip for callers that feed global_aligner next
 (SURVEY §8f rank 2).  Pair lists that share images (make_pairs) encode each image once (model.encode_images) and
 decode every batch from those features (model.decode_pairs); pair lists of several image sizes are decoded in
@@ -105,7 +105,7 @@ def _uploadable(t, dev):
 
 
 def _micro_batch(batch_size):
-    """Pairs per fused forward call.  A user batch of >= 16 pairs is run as two halves so that the host-side
+    """Pairs per forward call.  A user batch of >= 16 pairs is run as two halves so that the host-side
     staging + H2D of one half and the D2H of the other overlap the GPU compute (per-pair results do not depend on
     the batch they are computed in); halves stay even so symmetrised (a,b),(b,a) neighbours are kept together."""
     if batch_size < 16:
@@ -151,7 +151,7 @@ def _upload(ts, dev, up):
 
 def _encode(model, imgs, chunk):
     """Encoder features of every image of `imgs`, in calls of at most `chunk` images (what bounds the encoder's workspace:
-    a fused call of `chunk // 2` pairs encodes up to `chunk` images)."""
+    forward() on `chunk // 2` pairs encodes up to `chunk` images)."""
     parts = [model.encode_images(imgs[c:c + chunk]) for c in range(0, int(imgs.shape[0]), chunk)]
     return parts[0] if len(parts) == 1 else torch.cat(parts)
 
@@ -217,7 +217,7 @@ def inference(pairs, model, device, batch_size=8, verbose=True, keep_on_device=F
     """inference.py:55-72.  Returns {'view1','view2','pred1','pred2','loss'}; tensors on CPU (pinned) unless
     keep_on_device.  Software pipeline over micro-batches: images are gathered into pinned host memory (which is
     also the returned, collated view; return_images=False -- extension -- leaves 'img' out of the returned views and skips
-    that copy where the upload does not need it), uploaded on a copy stream, run through one fused forward call, and the
+    that copy where the upload does not need it), uploaded on a copy stream, run through one forward call, and the
     predictions are copied D2H on a second side stream into the final (whole pair list) pinned output -- the
     upload of batch k+1 and the download of batch k-1 overlap the compute of batch k."""
     if verbose:
@@ -259,7 +259,7 @@ def inference(pairs, model, device, batch_size=8, verbose=True, keep_on_device=F
     # pair lists from make_pairs reuse the same image dict in many pairs (n images -> up to n(n-1) pairs): upload and encode
     # every distinct image once, then decode each micro-batch from those features through index maps -- the encoder runs
     # once per image of the list instead of twice per pair (its output for an image does not depend on what else is in
-    # the batch, so results are unchanged).  Encoder calls take at most 2 * mb images, as a fused call of mb pairs does.
+    # the batch, so results are unchanged).  Encoder calls take at most 2 * mb images, as forward() on mb pairs does.
     feats, gidx = None, ([], [])
     if hasattr(model, 'decode_pairs') and all(int(v['img'].shape[0]) == 1 for vs in views for v in vs):
         order, gidx = _distinct_images(views)

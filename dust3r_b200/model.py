@@ -226,7 +226,9 @@ class AsymmetricCroCo3DStereo(nn.Module, _HubMixin, **_hub_kwargs):
                 raise AssertionError(f'true_shape {(h, w)} does not match the image tensor {(Hv, Wv)}')
         if (H, W) != (H2, W2):
             # model.py:147-151: the two views are encoded separately; the decoder cross-attends between the two grids
-            return _in_other_view(self._packed.forward_mixed(img1.float().contiguous(), img2.float().contiguous()))
+            feat1, feat2 = (self._packed.encode(img.float().contiguous()) for img in (img1, img2))
+            idx = np.arange(B, dtype=np.int32)
+            return _in_other_view(self._packed.decode(feat1, idx, feat2, idx))
         # model.py:153-170: a batch [(a,b),(b,a),...] only encodes its even half
         if is_symmetrized(view1, view2):
             imgs = torch.cat((img1[::2], img2[::2]), dim=0)
@@ -453,21 +455,19 @@ class _PackedModel:
             m.lin_head[0] = lin('downstream_head1.proj')
             m.lin_head[1] = lin('downstream_head2.proj')
         self.cmodel = m
-        self._ws = {}   # kind of call -> (shape key, workspace)
+        self._ws = {}   # kind of call ('encode', 'decode') -> workspace
 
-    def _workspace(self, kind, query, dims):
-        """The device workspace of one kind of call ('forward' for both fused calls, 'encode', 'decode'), sized by `query` on
-        the call's shape `dims` and kept while that shape stays the same.  Each kind keeps its own, so alternating encode and
-        decode calls do not reallocate."""
-        key = (query.__name__,) + dims
+    def _workspace(self, kind, need):
+        """The device workspace of one kind of call ('encode' or 'decode') for a call that needs `need` bytes (its size
+        query's answer): the cached one whenever it is at least that large, else a new one.  Each kind keeps its own, so
+        alternating encode and decode calls, and calls of smaller shapes, do not reallocate."""
+        if need <= 0:
+            _lib.check(-1)
         cur = self._ws.get(kind)
-        if cur is None or cur[0] != key:
-            need = query(C.byref(self.cmodel), *dims)
-            if need <= 0:
-                _lib.check(-1)
+        if cur is None or cur.numel() < need:
             self._ws.pop(kind, None)   # free the old one first
-            cur = self._ws[kind] = (key, torch.empty((need,), dtype=torch.uint8, device=self.device))
-        return cur[1]
+            cur = self._ws[kind] = torch.empty((need,), dtype=torch.uint8, device=self.device)
+        return cur
 
     def _outputs(self, B, sizes):
         """One ({'pts3d', 'conf'}) dict of fp32 CUDA tensors per view; `conf` only with a confidence channel."""
@@ -478,23 +478,11 @@ class _PackedModel:
                 r['conf'] = torch.empty((B, H, W), dtype=torch.float32, device=dev)
         return res
 
-    def _run(self, launch, query, dims, inputs, B, sizes, debug=None):
-        """One call of d3r_forward_pairs / d3r_forward_pairs_mixed (`launch`) into fresh outputs."""
-        ws = self._workspace('forward', query, dims)
-        res = self._outputs(B, sizes)
-        if debug is not None:
-            stage, buf = debug
-            _lib.check(self.lib.d3r_forward_set_debug(stage, buf.data_ptr(), buf.numel()))
-        outs = [r[k].data_ptr() if k in r else None for r in res for k in ('pts3d', 'conf')]
-        with torch.cuda.device(self.device):
-            _lib.check(launch(C.byref(self.cmodel), *inputs, *outs, ws.data_ptr(), ws.numel(), _lib.stream_ptr()))
-        return res
-
     def encode(self, imgs):
         """imgs (n,3,H,W) fp32 CUDA -> features (n, H/16, W/16, enc_dim) bf16 CUDA (d3r_encode_images)."""
         n, H, W = int(imgs.shape[0]), int(imgs.shape[-2]), int(imgs.shape[-1])
         p = self.cfg.patch_size
-        ws = self._workspace('encode', self.lib.d3r_encode_workspace_bytes, (n, H, W))
+        ws = self._workspace('encode', self.lib.d3r_encode_workspace_bytes(C.byref(self.cmodel), n, H, W))
         feat = torch.empty((n, H // p, W // p, self.cfg.enc_embed_dim), dtype=torch.bfloat16, device=self.device)
         with torch.cuda.device(self.device):
             _lib.check(self.lib.d3r_encode_images(C.byref(self.cmodel), imgs.data_ptr(), n, H, W, feat.data_ptr(), ws.data_ptr(),
@@ -506,7 +494,7 @@ class _PackedModel:
         ({'pts3d','conf'}, {'pts3d','conf'}) (d3r_decode_pairs)."""
         p, B = self.cfg.patch_size, len(idx1)
         (n1, H1, W1), (n2, H2, W2) = [(int(f.shape[0]), int(f.shape[1]) * p, int(f.shape[2]) * p) for f in (feat1, feat2)]
-        ws = self._workspace('decode', self.lib.d3r_decode_workspace_bytes, (B, H1, W1, H2, W2))
+        ws = self._workspace('decode', self.lib.d3r_decode_workspace_bytes(C.byref(self.cmodel), B, H1, W1, H2, W2))
         res = self._outputs(B, ((H1, W1), (H2, W2)))
         outs = [r[k].data_ptr() if k in r else None for r in res for k in ('pts3d', 'conf')]
         i1 = (C.c_int32 * B)(*[int(v) for v in idx1])
@@ -516,18 +504,17 @@ class _PackedModel:
                                                  i1, i2, B, *outs, ws.data_ptr(), ws.numel(), _lib.stream_ptr()))
         return res
 
-    def forward_mixed(self, imgs1, imgs2):
-        """imgs1 (B,3,H1,W1), imgs2 (B,3,H2,W2) fp32 CUDA with different sizes -> ({'pts3d','conf'}, {'pts3d','conf'})."""
-        B = int(imgs1.shape[0])
-        assert int(imgs2.shape[0]) == B
-        H1, W1, H2, W2 = int(imgs1.shape[-2]), int(imgs1.shape[-1]), int(imgs2.shape[-2]), int(imgs2.shape[-1])
-        return self._run(self.lib.d3r_forward_pairs_mixed, self.lib.d3r_forward_mixed_workspace_bytes, (B, H1, W1, H2, W2),
-                         (imgs1.data_ptr(), H1, W1, imgs2.data_ptr(), H2, W2, B), B, ((H1, W1), (H2, W2)))
-
     def forward(self, imgs, idx1, idx2, B, H, W, debug=None):
-        """imgs: (n_enc,3,H,W) fp32 CUDA.  Returns ({'pts3d','conf'}, {'pts3d','conf'}) CUDA fp32 tensors."""
-        n_enc = int(imgs.shape[0])
-        i1 = (C.c_int32 * B)(*[int(v) for v in idx1])
-        i2 = (C.c_int32 * B)(*[int(v) for v in idx2])
-        return self._run(self.lib.d3r_forward_pairs, self.lib.d3r_forward_workspace_bytes, (n_enc, B, H, W),
-                         (imgs.data_ptr(), n_enc, i1, i2, B, H, W), B, ((H, W), (H, W)), debug)
+        """imgs: (n_enc,3,H,W) fp32 CUDA; pair b is (image idx1[b], image idx2[b]).  Returns ({'pts3d','conf'}, {'pts3d','conf'})
+        CUDA fp32 tensors.  debug=(stage, buf) taps one intermediate stage into the fp32 tensor `buf` (d3r_forward_set_debug,
+        armed before the call that owns the stage: 1-4 the encode call, 5 and up the decode call)."""
+        assert len(idx1) == len(idx2) == B and tuple(imgs.shape[-2:]) == (H, W)
+        if debug is not None and debug[0] <= 4:
+            self._tap(*debug)
+        feat = self.encode(imgs)
+        if debug is not None and debug[0] > 4:
+            self._tap(*debug)
+        return self.decode(feat, idx1, feat, idx2)
+
+    def _tap(self, stage, buf):
+        _lib.check(self.lib.d3r_forward_set_debug(stage, buf.data_ptr(), buf.numel()))

@@ -1,9 +1,9 @@
 """Small host-side helpers of the forward path.
 
-Only `is_symmetrized` carries reference semantics that the fused forward depends on (dust3r/utils/misc.py:32-40
+Only `is_symmetrized` carries reference semantics that the forward depends on (dust3r/utils/misc.py:32-40
 decides, from the `instance` strings of a batch, whether it has the layout [(a,b),(b,a),(c,d),(d,c),...] whose
 encoder work can be halved).  The head wrappers of the reference (`transpose_to_landscape`) have no counterpart here:
-token-grid handling lives inside the fused C call (`d3r_forward_pairs`)."""
+token-grid handling lives inside the C calls (`d3r_encode_images`, `d3r_decode_pairs`)."""
 from __future__ import annotations
 
 import inspect

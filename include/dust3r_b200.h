@@ -216,7 +216,7 @@ int d3r_align_pack_entries(const d3r_pack_entry* table_dev, int32_t n_entries, i
 
 /* ------------------------------------------------------------------------------------------
  * Path 1 building blocks — exported so the parity tests can exercise each kernel in isolation.
- * Integrators use d3r_forward_* below; these are the ops it is composed of.
+ * Integrators use d3r_encode_images / d3r_decode_pairs below; these are the ops they are composed of.
  * ------------------------------------------------------------------------------------------ */
 
 /* epilogue flags of d3r_gemm_bf16 / d3r_conv3x3_bf16 */
@@ -366,8 +366,8 @@ int d3r_segment_sky(int32_t n_imgs, const int32_t* hw_dev, const int64_t* off_de
 
 /* ------------------------------------------------------------------------------------------
  * Path 1 — pairwise forward: replaces AsymmetricCroCo3DStereo.forward (dust3r/model.py:199-211 =
- * _encode_symmetrized :153-170, _decoder :172-191, downstream heads :193-208) for one batch of
- * same-sized pairs.  Weights are caller-owned device buffers, repacked once by the host side
+ * _encode_symmetrized :153-170, _decoder :172-191, downstream heads :193-208) as an encode call and a
+ * decode call.  Weights are caller-owned device buffers, repacked once by the host side
  * (dust3r_b200/model.py: bf16 GEMM operands, fp32 biases / LayerNorm parameters).
  * ------------------------------------------------------------------------------------------ */
 typedef struct d3r_linear { const void* w; const float* b; } d3r_linear;  /* w: bf16 [out][in]; b may be NULL */
@@ -428,35 +428,19 @@ typedef struct d3r_model {
 /* sizeof(d3r_model) as compiled into the library (binding self-check). */
 int d3r_sizeof_model(void);
 
-/* Bytes of device workspace d3r_forward_pairs needs for (n_enc images to encode, B pairs, HxW). */
-int64_t d3r_forward_workspace_bytes(const d3r_model* m, int32_t n_enc, int32_t B, int32_t H, int32_t W);
-
-/* imgs: (n_enc,3,H,W) fp32 in [-1,1] — the images the encoder runs on (model.py:142-170 decides which:
- * cat(img1,img2), or only the even halves for a symmetrised batch).  idx1/idx2: HOST int32[B], the
- * encoded image acting as view1 / view2 of pair b.  Outputs (fp32, device):
- * pts3d_1 (B,H,W,3), conf_1 (B,H,W) in view1's frame for view1; pts3d_2 / conf_2 for view2
- * ('pts3d_in_other_view').  conf pointers may be NULL when the model has no confidence channel. */
-int d3r_forward_pairs(const d3r_model* m, const float* imgs_dev, int32_t n_enc, const int32_t* idx1_host,
-                      const int32_t* idx2_host, int32_t B, int32_t H, int32_t W, float* pts3d_1, float* conf_1,
-                      float* pts3d_2, float* conf_2, void* workspace_dev, int64_t workspace_bytes, void* stream);
-
-/* Pairs whose two images differ in size (the reference encodes them separately, dust3r/model.py:147-151, and
- * inference() then runs one pair per call, dust3r/inference.py:60-64): imgs1 (B,3,H1,W1) are the first views,
- * imgs2 (B,3,H2,W2) the second views; outputs pts3d_1 (B,H1,W1,3), conf_1 (B,H1,W1), pts3d_2 (B,H2,W2,3),
- * conf_2 (B,H2,W2).  No symmetrisation shortcut on this path. */
-int64_t d3r_forward_mixed_workspace_bytes(const d3r_model* m, int32_t B, int32_t H1, int32_t W1, int32_t H2, int32_t W2);
-int d3r_forward_pairs_mixed(const d3r_model* m, const float* imgs1_dev, int32_t H1, int32_t W1, const float* imgs2_dev,
-                            int32_t H2, int32_t W2, int32_t B, float* pts3d_1, float* conf_1, float* pts3d_2,
-                            float* conf_2, void* workspace_dev, int64_t workspace_bytes, void* stream);
-
-/* The two halves of d3r_forward_pairs, for callers that keep encoder features between calls (each image of a
- * multi-view scene encoded once, however many pairs it appears in; pairs of two image sizes batched).
+/* The forward is two calls on one stream.
  * d3r_encode_images: imgs (n,3,H,W) fp32 in [-1,1] -> feat (n, H/16, W/16, enc_dim) bf16, caller-owned: the
- * encoder's output after enc_norm (model.py:128-140), the tensor the decoder and DPT hook 0 read.
+ * encoder's output after enc_norm (model.py:128-140), the tensor the decoder and DPT hook 0 read.  A symmetrised batch
+ * (model.py:153-170) encodes only its even half; two views of different sizes (model.py:147-151) are encoded by one
+ * call each.
  * d3r_decode_pairs: decoders + heads for B pairs; pair b is (image idx1[b] of feat1, image idx2[b] of feat2),
  * idx HOST int32[B], indices in [0, n1) / [0, n2).  feat1 and feat2 may be the same buffer when the sizes are equal.
- * Features must be 16-byte aligned.  Outputs as d3r_forward_pairs_mixed (sizes H1 x W1 for view 1, H2 x W2 for
- * view 2).  Debug taps 1-4 apply to the encode call, 5 and up to the decode call. */
+ * Features must be 16-byte aligned.  Outputs (fp32, device): pts3d_1 (B,H1,W1,3), conf_1 (B,H1,W1) in view1's frame
+ * for view1; pts3d_2 (B,H2,W2,3) / conf_2 (B,H2,W2) for view2 ('pts3d_in_other_view').  conf pointers may be NULL
+ * when the model has no confidence channel.
+ * Each image's features, and each pair's outputs, are independent of the rest of their call, so features can be kept
+ * between calls (each image of a multi-view scene encoded once, however many pairs it appears in).  Debug taps 1-4
+ * apply to the encode call, 5 and up to the decode call. */
 int64_t d3r_encode_workspace_bytes(const d3r_model* m, int32_t n, int32_t H, int32_t W);
 int d3r_encode_images(const d3r_model* m, const float* imgs_dev, int32_t n, int32_t H, int32_t W, void* feat_dev,
                       void* workspace_dev, int64_t workspace_bytes, void* stream);

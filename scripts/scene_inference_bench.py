@@ -39,22 +39,17 @@ def views(n_land, n_port, seed=21):
 
 
 class EncoderCounter:
-    """Counts the images every library call encodes: fused calls (both builds) and encode calls (where they exist)."""
+    """Counts the images every encode call of the library encodes (every forward runs through `_PackedModel.encode`)."""
 
     def __init__(self):
         from dust3r_b200.model import _PackedModel
         self.n = 0
-        for name, count in (('forward', lambda a, k: int(a[0].shape[0])), ('forward_mixed', lambda a, k: 2 * int(a[0].shape[0])),
-                            ('encode', lambda a, k: int(a[0].shape[0]))):
-            fn = getattr(_PackedModel, name, None)
-            if fn is not None:
-                setattr(_PackedModel, name, self._wrap(fn, count))
+        encode = _PackedModel.encode
 
-    def _wrap(self, fn, count):
-        def run(packed, *a, **k):
-            self.n += count(a, k)
-            return fn(packed, *a, **k)
-        return run
+        def counted(packed, imgs):
+            self.n += int(imgs.shape[0])
+            return encode(packed, imgs)
+        _PackedModel.encode = counted
 
 
 def sample(out):

@@ -128,7 +128,7 @@ def test_forward_matches_oracle_and_reference_golden(cuda_device, name):
 @pytest.mark.parametrize('name', ['small_dpt', 'small_linear'])
 def test_forward_mixed_sizes_matches_reference_golden(cuda_device, name):
     """Three images of three sizes, all ordered pairs: inference() returns lists (inference.py:60-72) and every pair
-    runs through d3r_forward_pairs_mixed (separate encoder passes, cross-attention between two token grids)."""
+    runs through one encode call per size and d3r_decode_pairs (cross-attention between two token grids)."""
     from dust3r_b200.inference import inference
     cfg, H, W = _small_cfgs()[name]
     net, sd = _build(cfg, 11, cuda_device)
@@ -177,7 +177,7 @@ def test_inference_pipelined_micro_batches_bit_identical(cuda_device):
 
 @pytest.mark.timeout(900)
 def test_forward_stages_against_oracle(cuda_device):
-    """Stage taps of the fused path vs the oracle's intermediate tensors (small DPT model, 2 pairs)."""
+    """Stage taps of the forward vs the oracle's intermediate tensors (small DPT model, 2 pairs)."""
     from oracle.forward_oracle import forward_oracle
     cfg, H, W = _small_cfgs()['small_dpt']
     net, sd = _build(cfg, 11, cuda_device)

@@ -1,5 +1,5 @@
 """Two-GPU test of the product multi-GPU path (`-m gpu`; skipped on a single-GPU box): inference_sharded() over NCCL -- every
-rank runs its slice of the pair list through the fused forward, ONE all_gather_into_tensor rebuilds the full result on every
+rank runs its slice of the pair list through the forward, ONE all_gather_into_tensor rebuilds the full result on every
 rank (device resident), and it must equal single-GPU inference() of the whole list."""
 import os
 import sys

@@ -2,7 +2,7 @@
 inference() paths built on them, against the paths that existed before them.
 
 Every comparison is bit for bit: each kernel computes an image (or a token row) independently of the rest of its launch, so
-encoding an image once and decoding its pairs in any batch gives the bits of the fused forward on that pair."""
+encoding an image once and decoding its pairs in any batch gives the bits of forward() on that pair."""
 import ctypes as C
 
 import numpy as np
@@ -73,7 +73,7 @@ def _patch_embed_rows(records, E):
 @pytest.mark.parametrize('name', ['small_dpt', 'small_linear'])
 def test_same_size_scene_equals_private_copies(cuda_device, name):
     """A make_pairs list shares one image dict between many pairs: inference() encodes every image once and decodes each
-    micro-batch from those features.  The same list with private copies of every image takes the fused all-distinct path
+    micro-batch from those features.  The same list with private copies of every image takes the all-distinct path
     (both images of every pair encoded in the batch): the two must agree bit for bit, for every graph and batch size."""
     from dust3r_b200.inference import inference
     cfg, H, W = _small_cfgs()[name]
@@ -138,9 +138,9 @@ def test_mixed_sizes_equal_the_per_pair_loop(cuda_device, name):
 
 # ---- the public API ------------------------------------------------------------------------------------------------------
 @pytest.mark.timeout(900)
-def test_encode_images_is_the_fused_encoder_output(cuda_device):
-    """encode_images == debug tap 4 (enc_norm output) of the fused forward, bit for bit, and the oracle's enc_norm stage within
-    the stage tolerance; the decoder taps (5 and up) of decode_pairs equal the fused forward's."""
+def test_encode_images_is_the_forward_encoder_output(cuda_device):
+    """encode_images == debug tap 4 (enc_norm output) of the packed model's forward, bit for bit, and the oracle's enc_norm
+    stage within the stage tolerance."""
     from oracle.forward_oracle import forward_oracle
     cfg, H, W = _small_cfgs()['small_dpt']
     net, sd = _net(cfg, cuda_device)
@@ -161,14 +161,6 @@ def test_encode_images_is_the_fused_encoder_output(cuda_device):
     assert torch.equal(feat.float().reshape(-1), tap)
     ref = st['enc_norm'].reshape(-1)
     assert float((feat.float().cpu().reshape(-1) - ref).norm() / ref.norm()) < 2e-2
-    for stage, n in ((5, 2 * N * cfg.dec_embed_dim), (7, 2 * N * cfg.dec_embed_dim)):
-        fused = torch.zeros((n,), dtype=torch.float32, device=cuda_device)
-        packed.forward(x, idx1, idx2, 2, H, W, debug=(stage, fused))
-        split = torch.zeros_like(fused)
-        _lib.check(packed.lib.d3r_forward_set_debug(stage, split.data_ptr(), split.numel()))
-        packed.decode(feat, idx1, feat, idx2)
-        torch.cuda.synchronize()
-        assert torch.equal(fused, split) and bool(fused.abs().sum() > 0), stage
 
 
 @pytest.mark.timeout(900)
@@ -198,7 +190,7 @@ def test_add_a_view_to_a_scene(cuda_device, name):
 
 @pytest.mark.timeout(900)
 def test_decode_two_sizes_equals_forward(cuda_device):
-    """decode_pairs over a landscape and a portrait feature set == model.forward() on the same pairs (two-size fused call)."""
+    """decode_pairs over a landscape and a portrait feature set == model.forward() on the same pairs (two-size batch)."""
     cfg, H, W = _small_cfgs()['small_dpt']
     net, _ = _net(cfg, cuda_device)
     a = torch.cat([v['img'] for v in synth_images(3, H, W, seed=70)]).to(cuda_device)
@@ -268,6 +260,33 @@ def test_rejected_arguments_launch_nothing(cuda_device):
     assert all(rc != 0 for rc in rcs), rcs
     assert _lib.launch_count() == before
     assert lib.d3r_encode_workspace_bytes(m, 0, H, W) < 0 and lib.d3r_decode_workspace_bytes(m, 0, H, W, H, W) < 0
+
+
+@pytest.mark.timeout(600)
+@pytest.mark.parametrize('name', ['small_dpt', 'small_linear'])
+def test_calls_write_only_inside_their_buffers(cuda_device, name):
+    """An encode call writes nothing past the workspace size its query returns or past the features, and a decode call
+    nothing past its workspace: sentinel bytes behind each buffer stay as they were.  The small DPT model's encoder is
+    narrower than a patch (4 x 128 < 3 x 16 x 16), so its patch im2col is wider than its MLP hidden layer."""
+    cfg, H, W = _small_cfgs()[name]
+    net, _ = _net(cfg, cuda_device)
+    x = torch.cat([v['img'] for v in synth_images(3, H, W, seed=95)]).to(cuda_device)
+    packed, lib = net.repack(), net._packed.lib
+    m, st, tail = C.byref(packed.cmodel), _lib.stream_ptr(), 1 << 20
+    n_feat = 3 * (H // 16) * (W // 16) * cfg.enc_embed_dim * 2
+    need_e, need_d = lib.d3r_encode_workspace_bytes(m, 3, H, W), lib.d3r_decode_workspace_bytes(m, 2, H, W, H, W)
+    ws_e, feat, ws_d = [torch.full((n + tail,), 0xA5, dtype=torch.uint8, device=cuda_device) for n in (need_e, n_feat, need_d)]
+    out = [torch.empty((2, H, W, 3), device=cuda_device) for _ in range(2)]
+    conf = [torch.empty((2, H, W), device=cuda_device) for _ in range(2)]
+    assert lib.d3r_encode_images(m, x.data_ptr(), 3, H, W, feat.data_ptr(), ws_e.data_ptr(), need_e, st) == 0
+    i1, i2 = (C.c_int32 * 2)(0, 1), (C.c_int32 * 2)(2, 0)
+    assert lib.d3r_decode_pairs(m, feat.data_ptr(), 3, H, W, feat.data_ptr(), 3, H, W, i1, i2, 2, out[0].data_ptr(),
+                                conf[0].data_ptr(), out[1].data_ptr(), conf[1].data_ptr(), ws_d.data_ptr(), need_d, st) == 0
+    torch.cuda.synchronize()
+    for what, buf, n in (('encode workspace', ws_e, need_e), ('features', feat, n_feat), ('decode workspace', ws_d, need_d)):
+        assert bool((buf[n:] == 0xA5).all()), what
+    ref = net.encode_images(x)
+    assert torch.equal(feat[:n_feat].view(torch.bfloat16).reshape(ref.shape), ref)
 
 
 # ---- the published model -------------------------------------------------------------------------------------------------
