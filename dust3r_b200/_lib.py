@@ -62,6 +62,11 @@ def _declare(lib):
         getattr(lib, name).argtypes = [C.POINTER(AlignDesc), vp]
     lib.d3r_align_run.restype = C.c_int
     lib.d3r_align_run.argtypes = [C.POINTER(AlignDesc), i32, i32, vp]
+    for name in ('d3r_align_pixel_pass', 'd3r_align_small_step'):
+        getattr(lib, name).restype = C.c_int
+        getattr(lib, name).argtypes = [C.POINTER(AlignDesc), i32, vp]
+    lib.d3r_align_reduce_block.restype = C.c_int
+    lib.d3r_align_reduce_block.argtypes = [i32, i32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
     lib.d3r_align_loss_grad.restype = C.c_int
     lib.d3r_align_loss_grad.argtypes = [C.POINTER(AlignDesc), vp, vp, vp, vp]
     lib.d3r_align_overflow_flag.restype = C.c_int

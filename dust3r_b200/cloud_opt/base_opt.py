@@ -250,8 +250,10 @@ class BasePCOptimizer(nn.Module):
         return None
 
     def _build_engine(self):
+        """The scene's AlignEngine; a scene from distributed.global_aligner_sharded gets the engine of this rank's images."""
         dev = self.device
         keys = self.str_edges
+        shard = self.__dict__.get('_align_shard')
         self._engine = AlignEngine(
             self.edges, self.imshapes,
             [self.pred_i[k] for k in keys], [self.pred_j[k] for k in keys],
@@ -259,7 +261,8 @@ class BasePCOptimizer(nn.Module):
             device=dev, conf_mode=self.conf_mode, dist=self.dist, variant=self._engine_variant(), pix_stride=self._engine_pix_stride(),
             base_scale=self.base_scale, pw_break=self.pw_break,
             focal_break=getattr(self, 'focal_break', getattr(self, 'focal_brake', 20)),
-            kernel=getattr(self, 'align_kernel', 'auto'))
+            kernel=getattr(self, 'align_kernel', 'auto'),
+            shards=shard.shards if shard is not None else None, group=shard.group if shard is not None else None)
         return self._engine
 
     def _engine_push(self, eng):

@@ -7,6 +7,10 @@ HBM layout (all fp32, owned by torch):
              while its pixels' world points stay in registers.  32*E*P bytes, read once / iteration.
   logd       float[ sum_i stride_i ]            log-depth (+ exp_avg, exp_avg_sq): 24*n*P bytes r+w.
   small      float[ 7n + 2n + 2n + 8E + 2E ]    poses / focals / pp / pairwise poses / adaptors.
+
+Sharded over the ranks of a process group (`shards=`), each rank packs and streams only its own images' entries and runs
+every iteration as pixel pass -> one all-reduce of the fixed-point accumulator block -> small step (d3r_align_pixel_pass /
+d3r_align_small_step), so that every rank computes the same small parameters; `logd` keeps its global layout.
 """
 from __future__ import annotations
 
@@ -17,6 +21,7 @@ from typing import List, Sequence, Tuple
 
 import numpy as np
 import torch
+import torch.distributed as tdist
 
 from .. import _lib
 from .commons import cosine_schedule, linear_schedule
@@ -30,6 +35,12 @@ ITEM = np.dtype([('img', np.int32), ('slot0', np.int32), ('nslots', np.int32), (
                  ('v0', np.int32), ('inv_w', np.float32), ('pix0', np.int64), ('obs0', np.int64),
                  ('slab_units', np.int32), ('reserved', np.int32)])
 SLOT_PX = 64          # pixels per slot of the streaming layout (32 pixel pairs)
+PIXEL_COST = 3        # streaming cost of a slot = entries of its image + PIXEL_COST (unprojection, depth Adam, item set-up)
+
+
+def stream_cost(slots, degrees):
+    """Streaming cost of every image (or slot): slots x (entries of the image + fixed per-pixel work)."""
+    return np.asarray(slots, dtype=np.float64) * (np.asarray(degrees, dtype=np.float64) + PIXEL_COST)
 
 
 def build_stream_items(imshapes, pix_off, ent_ptr, ent_obs_off, slots, ppt, warps_per_cta, max_ctas):
@@ -46,7 +57,7 @@ def build_stream_items(imshapes, pix_off, ent_ptr, ent_obs_off, slots, ppt, warp
     img_first = np.concatenate([[0], np.cumsum(slots)])            # first global slot of every image
     total = int(img_first[-1])
     slot_img = np.repeat(np.arange(n), slots)                      # image of every slot, global slot order
-    cost = (deg[slot_img] + 3).astype(np.float64)
+    cost = stream_cost(1, deg[slot_img])
     cum = np.concatenate([[0.0], np.cumsum(cost)])
     n_warps = int(min(max_ctas * warps_per_cta, total))
     grid = (n_warps + warps_per_cta - 1) // warps_per_cta
@@ -84,13 +95,17 @@ class AlignEngine:
     """pred_i / pred_j: per-edge (H, W, 3) pointmaps; conf_i / conf_j: per-edge RAW confidences (H, W) -- the
     confidence transform `conf_mode` (commons.py:73-80) is applied by the packing kernel.  Tensors already on
     `device` (e.g. views of inference(keep_on_device=True) / all-gather output) are read in place; everything is
-    packed by ONE launch (d3r_align_pack_entries)."""
+    packed by ONE launch (d3r_align_pack_entries).
+
+    shards: optional list of contiguous image ranges [lo, hi), one per rank of `group` (distributed.shard_images); this
+    rank packs and streams only the entries of its own range, and run() / evaluate_loss() exchange the accumulators with
+    one all-reduce per iteration.  Streaming kernel only."""
 
     def __init__(self, edges: Sequence[Tuple[int, int]], imshapes: Sequence[Tuple[int, int]],
                  pred_i: Sequence[torch.Tensor], pred_j: Sequence[torch.Tensor],
                  conf_i: Sequence[torch.Tensor], conf_j: Sequence[torch.Tensor],
                  device, conf_mode='log', dist='l1', variant='stacked', pix_stride=None,
-                 base_scale=0.5, pw_break=20.0, focal_break=20.0, kernel='auto', reverse_odd='auto'):
+                 base_scale=0.5, pw_break=20.0, focal_break=20.0, kernel='auto', reverse_odd='auto', shards=None, group=None):
         self.device = _lib.require_cuda_device(device)
         self.lib = _lib.get_lib()
         self.edges = [(int(i), int(j)) for i, j in edges]
@@ -120,6 +135,17 @@ class AlignEngine:
         assert kernel in ('stream', 'general')
         self.kernel = kernel
         stream = kernel == 'stream'
+        self.group, self.shards = group, None
+        lo, hi = 0, n
+        if shards is not None:
+            if not stream:
+                raise ValueError('the sharded alignment runs on the streaming kernel only (every image needs H*W and its pixel '
+                                 'stride to be multiples of 4)')
+            self.shards = [(int(a), int(b)) for a, b in shards]
+            if len(self.shards) != tdist.get_world_size(group):
+                raise ValueError(f'{len(self.shards)} image ranges for a group of {tdist.get_world_size(group)} ranks')
+            lo, hi = self.shards[tdist.get_rank(group)]
+        self.owned = (lo, hi)
         if reverse_odd == 'auto':     # D3R_ALIGN_REVERSE=0: every iteration walks the items in the same order (A/B switch)
             reverse_odd = os.environ.get('D3R_ALIGN_REVERSE', '1') != '0'
         self.reverse_odd = bool(reverse_odd)
@@ -164,6 +190,9 @@ class AlignEngine:
                 else:                # base_opt.py:262-270: mean over pixels, then / n_edges
                     ent_coef[k] = 1.0 / (areas[img] * E)
                 edge_ent[e, side] = k
+                if not lo <= img < hi:      # another rank's image: its observations are not packed here
+                    k += 1
+                    continue
                 pts = on_dev((pred_i if side == 0 else pred_j)[e], 3)
                 cf = on_dev((conf_i if side == 0 else conf_j)[e], 1)
                 assert pts.shape[0] >= areas[img] and cf.shape[0] >= areas[img]
@@ -186,17 +215,27 @@ class AlignEngine:
         self.max_chunks = int(max(nchunks))
         self.max_deg = int(max(len(l) for l in ent_lists))
         # observations: one launch for every entry, confidence transform and (streaming layout) loss coefficient fused
-        self.obs = torch.empty((self.total_obs, 4), dtype=torch.float32, device=dev)
-        table_dev = torch.from_numpy(table.view(np.uint8)).to(dev)
-        with torch.cuda.device(dev):
-            _lib.check(self.lib.d3r_align_pack_entries(table_dev.data_ptr(), 2 * E, int(max(areas)), _CONF_MODES[conf_mode],
-                                                       1 if stream else 0, self.obs.data_ptr(), self._stream()))
+        self.obs = torch.empty((max(self.total_obs, 1), 4), dtype=torch.float32, device=dev)   # >= 1 row: a rank without images
+        k0, k1 = int(ent_ptr[lo]), int(ent_ptr[hi])      # entries of the packed images (all of them unless sharded)
+        table_dev = torch.from_numpy(np.ascontiguousarray(table[k0:k1]).view(np.uint8)).to(dev)
+        if k1 > k0:
+            with torch.cuda.device(dev):
+                _lib.check(self.lib.d3r_align_pack_entries(table_dev.data_ptr(), k1 - k0, int(max(areas[lo:hi])), _CONF_MODES[conf_mode],
+                                                           1 if stream else 0, self.obs.data_ptr(), self._stream()))
         if keep:
             torch.cuda.current_stream(dev).synchronize()     # the staged copies may be freed after this point
         del keep, table_dev
-        self._build_items(ent_ptr, ent_obs_off, slots) if stream else self._no_items()
+        if stream:
+            self._build_items(ent_ptr, ent_obs_off, [s if lo <= i < hi else 0 for i, s in enumerate(slots)])
+        else:
+            self._no_items()
         nws = self.lib.d3r_align_workspace_floats(n, E)
         self.workspace = torch.zeros((nws,), dtype=torch.float32, device=dev)
+        if self.shards is not None:     # the int64 block [ent_acc | img_acc | overflow word] the ranks all-reduce
+            off, words = C.c_int64(0), C.c_int64(0)
+            _lib.check(self.lib.d3r_align_reduce_block(n, E, C.byref(off), C.byref(words)))
+            self.reduce_block = (int(off.value), int(words.value))
+            self._reduce = self.workspace[off.value:off.value + 2 * words.value].view(torch.int64)
         self.counters = torch.zeros((n + 2,), dtype=torch.int32, device=dev)
         self.n_small = 11 * n + 10 * E
         self.small = torch.zeros((self.n_small,), dtype=torch.float32, device=dev)
@@ -224,10 +263,18 @@ class AlignEngine:
         self._items = self._warp_item_ptr = self._items_rev = self._warp_item_ptr_rev = None
 
     def _build_items(self, ent_ptr, ent_obs_off, slots):
+        """Work items over the images with slots > 0 (a sharded engine zeroes the slots of other ranks' images).  The entry
+        window follows the whole graph, so that every rank's small step runs the same version."""
         lib = self.lib
         ppt = int(lib.d3r_align_stream_slots_per_item())
         wpc = int(lib.d3r_align_stream_warps_per_cta())
         sms = torch.cuda.get_device_properties(self.device).multi_processor_count
+        deg_max = int(np.diff(ent_ptr).max())
+        window = int(min(max(deg_max, 1), lib.d3r_align_stream_max_window()))
+        if sum(slots) == 0:         # a rank without images: no pixel pass, but the same small step as every other rank
+            self._no_items()
+            self.stream_ppt, self.stream_window = ppt, window
+            return
         arr, warp_ptr, grid = build_stream_items(self.imshapes, self.pix_off, ent_ptr, ent_obs_off, slots, ppt, wpc, 2 * sms)
         assert arr.dtype.itemsize == 64 == lib.d3r_sizeof_align_item()
         dev = self.device
@@ -243,8 +290,7 @@ class AlignEngine:
             self._items_rev = torch.from_numpy(arr_rev.view(np.uint8)).to(dev)
             self._warp_item_ptr_rev = torch.from_numpy(np.ascontiguousarray(warp_ptr_rev)).to(dev)
         self.stream_grid, self.stream_ppt = grid, ppt
-        deg_max = int(np.diff(ent_ptr).max())
-        self.stream_window = int(min(max(deg_max, 1), lib.d3r_align_stream_max_window()))
+        self.stream_window = window
 
     def _pick_chunk_px(self, areas):
         """Pixels per CTA: the largest size <= the kernel's maximum for which the grid is (close to) a whole
@@ -362,7 +408,7 @@ class AlignEngine:
         d.counters = self.counters.data_ptr()
         d.stream_kernel = 1 if self.kernel == 'stream' else 0
         d.stream_grid, d.stream_ppt, d.stream_window, d.n_items = self.stream_grid, self.stream_ppt, self.stream_window, self.n_items
-        if self.kernel == 'stream':
+        if self.n_items:
             d.items, d.warp_item_ptr = self._items.data_ptr(), self._warp_item_ptr.data_ptr()
             if self._items_rev is not None:
                 d.items_rev, d.warp_item_ptr_rev = self._items_rev.data_ptr(), self._warp_item_ptr_rev.data_ptr()
@@ -400,11 +446,48 @@ class AlignEngine:
             return torch.zeros((0,), dtype=torch.float32, device=self.device)
         self.sched = torch.from_numpy(self.make_schedule(niter, lr, schedule, lr_min)).to(self.device)
         self.loss_out = torch.zeros((niter,), dtype=torch.float32, device=self.device)
+        if self.shards is not None:
+            with torch.cuda.device(self.device):
+                self._sync_start()
+                self.prepare()
+                d = self._desc()
+                for it in range(niter):
+                    self._split_iteration(d, it)
+                self._sync_end()
+            return self.loss_out
         if not getattr(self, '_prepared', False):
             self.prepare()
         d = self._desc()
         self._call(self.lib.d3r_align_run, C.byref(d), 0, niter)
         return self.loss_out
+
+    # ------------------------------------------------------------------ sharded iterations
+    def _src(self, r):
+        """Global rank of rank r of the engine's group."""
+        return tdist.get_global_rank(self.group, r) if self.group is not None else r
+
+    def _sync_start(self):
+        """One broadcast of rank 0's log-depths and small parameters: every rank starts from the same parameters, whatever
+        its own initialisation drew."""
+        nl = self.logd.numel()
+        buf = torch.cat((self.logd, self.small))
+        tdist.broadcast(buf, src=self._src(0), group=self.group)
+        self.logd.copy_(buf[:nl])
+        self.small.copy_(buf[nl:])
+
+    def _split_iteration(self, d, it):
+        """Pixel pass over this rank's items, the exact integer all-reduce of the accumulators, the small step: all three on
+        the engine's stream, nothing waits on the host."""
+        if self.n_items:
+            self._call(self.lib.d3r_align_pixel_pass, C.byref(d), it)
+        tdist.all_reduce(self._reduce, op=tdist.ReduceOp.SUM, group=self.group)
+        self._call(self.lib.d3r_align_small_step, C.byref(d), it)
+
+    def _sync_end(self):
+        """Every owner broadcasts its images' log-depths, so that every rank holds the whole scene."""
+        for r, (a, b) in enumerate(self.shards):
+            if b > a:
+                tdist.broadcast(self.logd[int(self.pix_off[a]):int(self.pix_off[b])], src=self._src(r), group=self.group)
 
     def check_overflow(self):
         """Raises if a fixed-point accumulator left its range (host sync)."""
@@ -419,6 +502,12 @@ class AlignEngine:
         """net.forward(): the objective at the current parameters, nothing updated."""
         self.sched = torch.zeros((1, 4), dtype=torch.float32, device=self.device)
         self.loss_out = torch.zeros((1,), dtype=torch.float32, device=self.device)
+        if self.shards is not None:     # sharded: the objective at rank 0's parameters, the same value on every rank
+            with torch.cuda.device(self.device):
+                self._sync_start()
+                self.prepare()
+                self._split_iteration(self._desc(eval_only=True), 0)
+            return self.loss_out[0]
         self.prepare()
         d = self._desc(eval_only=True)
         self._call(self.lib.d3r_align_run, C.byref(d), 0, 1)
@@ -430,6 +519,9 @@ class AlignEngine:
         (0 on padding pixels), dL/d(raw parameter) in the `small` layout (split it with split_small) and, when asked
         for, the (E, 2) coefficient-weighted loss of every (edge, side), else None.  Every tensor is freshly allocated,
         so results of two calls never alias."""
+        if self.shards is not None:
+            raise NotImplementedError('the differentiable objective (loss.backward(), ret_details=True) is not available on a '
+                                      'sharded alignment scene; use global_aligner for it')
         dev = self.device
         loss = torch.zeros((), dtype=torch.float32, device=dev)
         logd_grad = torch.zeros_like(self.logd)

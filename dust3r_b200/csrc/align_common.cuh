@@ -24,6 +24,8 @@ struct Workspace {
   float* imgT;           // [n][16]
   long long* ent_acc;    // [2E][13]  fixed-point (2^40) accumulators, zero between launches
   long long* img_acc;    // [n][12]
+  long long* ovf;        // [1]       split iteration: partial-range overflow seen by the pixel pass (directly after img_acc, so
+                         //           [ent_acc | img_acc | ovf] is one contiguous block that one all-reduce(SUM) carries)
   float* grad;           // [11n + 10E] multi-pass small-step scratch: raw gradients in the flat parameter layout
   int* flags;            // [4]       [0] = fixed-point overflow seen
   float* entT;           // [2E][12]  streaming kernel: -M (9), -t (3) of the entry's edge, indexed by entry (no indirection)
@@ -41,6 +43,7 @@ __host__ __device__ inline Workspace carve(float* ws, int n, int E) {
   w.imgT = ws + o;     o += align4(int64_t(n) * kImgT);
   w.ent_acc = reinterpret_cast<long long*>(ws + o); o += align4(int64_t(2) * E * kEntVals * 2);
   w.img_acc = reinterpret_cast<long long*>(ws + o); o += align4(int64_t(n) * kImgVals * 2);
+  w.ovf = reinterpret_cast<long long*>(ws + o); o += 4;
   w.grad = ws + o;     o += align4(int64_t(n) * 11 + int64_t(E) * 10);
   w.flags = reinterpret_cast<int*>(ws + o); o += 4;
   w.entT = ws + o;     o += align4(int64_t(2) * E * kEdgeT);
@@ -49,9 +52,16 @@ __host__ __device__ inline Workspace carve(float* ws, int n, int E) {
   return w;
 }
 
+// Where the block [ent_acc | img_acc | ovf] sits in the workspace (in floats) and how many int64 words it holds: what a
+// multi-GPU caller all-reduces between the pixel pass and the small step of a split iteration.
+inline void reduce_block(int n, int E, int64_t* offset_floats, int64_t* n_words) {
+  *offset_floats = align4(int64_t(E) * kEdgeT) + align4(int64_t(n) * kImgT);
+  *n_words = int64_t(2) * E * kEntVals + int64_t(n) * kImgVals + 1;
+}
+
 inline int64_t workspace_floats(int n, int E) {
   return align4(int64_t(E) * kEdgeT) + align4(int64_t(n) * kImgT) + align4(int64_t(2) * E * kEntVals * 2) +
-         align4(int64_t(n) * kImgVals * 2) + align4(int64_t(n) * 11 + int64_t(E) * 10) + 4 +
+         align4(int64_t(n) * kImgVals * 2) + 4 + align4(int64_t(n) * 11 + int64_t(E) * 10) + 4 +
          align4(int64_t(2) * E * kEdgeT) + align4(int64_t(E) * 24) + align4(int64_t(n) * 20);
 }
 

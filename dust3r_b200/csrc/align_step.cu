@@ -339,6 +339,7 @@ __global__ void __launch_bounds__(kThreads) pts3d_kernel(const __grid_constant__
 
 namespace d3r { namespace align {
 int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, const GradOut* go, cudaStream_t st);
+int launch_stream_split(const d3r_align_desc* desc, int it, bool pixel, cudaStream_t st);
 int stream_set_debug(unsigned long long* p);
 } }
 
@@ -406,6 +407,32 @@ extern "C" int d3r_align_run(const d3r_align_desc* desc, int32_t it_begin, int32
   if (desc->stream_kernel) return launch_stream(desc, it_begin, it_end, nullptr, (cudaStream_t)stream);
   return desc->dist_l2 ? launch_ppt<true>(desc, it_begin, it_end, nullptr, (cudaStream_t)stream)
                        : launch_ppt<false>(desc, it_begin, it_end, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_align_pixel_pass(const d3r_align_desc* desc, int32_t it, void* stream) {
+  int rc = validate(desc);
+  if (rc) return rc;
+  D3R_CHECK_ARG(it >= 0, "d3r_align_pixel_pass: bad iteration %d", it);
+  prof::Scope scope("align_pixel", (cudaStream_t)stream, 0.0, 0.0, 1);
+  return launch_stream_split(desc, it, true, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_align_small_step(const d3r_align_desc* desc, int32_t it, void* stream) {
+  int rc = validate(desc);
+  if (rc) return rc;
+  D3R_CHECK_ARG(it >= 0, "d3r_align_small_step: bad iteration %d", it);
+  if (it == 0) {   // the overflow flag reports on the run that starts here (only the small step writes it in a split iteration)
+    const Workspace ws0 = carve(desc->workspace, desc->n_imgs, desc->n_edges);
+    D3R_CUDA(cudaMemsetAsync(ws0.flags, 0, sizeof(int), (cudaStream_t)stream));
+  }
+  prof::Scope scope("align_small", (cudaStream_t)stream, 0.0, 0.0, 1);
+  return launch_stream_split(desc, it, false, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_align_reduce_block(int32_t n_imgs, int32_t n_edges, int64_t* offset_floats, int64_t* n_words) {
+  D3R_CHECK_ARG(n_imgs > 0 && n_edges > 0 && offset_floats && n_words, "d3r_align_reduce_block: bad arguments");
+  reduce_block(n_imgs, n_edges, offset_floats, n_words);
+  return D3R_OK;
 }
 
 extern "C" int d3r_align_loss_grad(const d3r_align_desc* desc, float* logd_grad, float* small_grad, float* entry_loss, void* stream) {

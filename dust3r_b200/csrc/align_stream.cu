@@ -21,7 +21,9 @@
 //     atomics (order independent -> bit-reproducible), exactly like the general kernel;
 //   * sqrt / reciprocal / exp of the per-pixel Adam update and unprojection use the MUFU approximations (<= 2 ulp).
 //
-// The last CTA of the grid (ticket) runs the same small-parameter step as the general kernel (align_common.cuh).
+// The last CTA of the grid (ticket) runs the same small-parameter step as the general kernel (align_common.cuh).  A split
+// iteration (align_stream_pixel_kernel + align_small_step_kernel) runs the same two halves as two launches, so that a
+// multi-GPU caller can all-reduce the accumulators between them.
 #include "align_common.cuh"
 
 namespace d3r {
@@ -274,10 +276,12 @@ __device__ __forceinline__ void adam_slots(const d3r_align_desc& D, const uint8_
   for (int v = 0; v < kImgVals; ++v) { float lo, hi; unpack2(S[v], lo, hi); s12[v] = lo + hi; }
 }
 
-// Body of both instantiation families: kGrad = false is the training iteration (align_stream_kernel), kGrad = true the
+// Body of all three instantiation families: kGrad = false is the training iteration (align_stream_kernel), kGrad = true the
 // gradient export (align_stream_grad_kernel): its MV stage brings only the image row, writes dL/dlog-depth to go.logd_grad
-// and still forms the image sums; the last CTA runs small_grad_step.
-template <bool kGrad, bool kL2, int PPT, int NST>
+// and still forms the image sums; the last CTA runs small_grad_step.  kSplit (align_stream_pixel_kernel) is the training
+// iteration's pixel pass alone: partial-range overflow goes to ws.ovf, which travels with the sums, and every CTA leaves
+// where the grid ticket would be taken -- align_small_step_kernel runs the small step.
+template <bool kGrad, bool kL2, int PPT, int NST, bool kSplit>
 __device__ __forceinline__ void stream_body(const d3r_align_desc& D, int it, const GradOut& go) {
   static_assert(PPT == 3, "the per-slot specialisations below are written for 3 slots per item");
   constexpr int kStage = kHdrBytes + PPT * kSlotBytes;
@@ -298,6 +302,7 @@ __device__ __forceinline__ void stream_body(const d3r_align_desc& D, int it, con
   float* s_img = s_acc + Wn * kEntVals;                           // [12] image sums
   uint64_t* full = s_full[warp];
   ProdState* ps = &s_prod[warp];
+  int* const ovf_flag = kSplit ? reinterpret_cast<int*>(ws.ovf) : ws.flags;   // low half of the word (little endian)
 
   // odd iterations walk the reversed item table when the host provides one (L2 reuse across iterations)
   const bool rev = (it & 1) && D.items_rev != nullptr;
@@ -336,7 +341,7 @@ __device__ __forceinline__ void stream_body(const d3r_align_desc& D, int it, con
       for (int idx = lane; idx < acc_cnt * kEntVals; idx += 32) {
         const float v = s_acc[idx];
         s_acc[idx] = 0.f;
-        fix_add(ws.ent_acc + int64_t(acc_e0) * kEntVals + idx, v, ws.flags);
+        fix_add(ws.ent_acc + int64_t(acc_e0) * kEntVals + idx, v, ovf_flag);
       }
       __syncwarp();
     }
@@ -344,7 +349,7 @@ __device__ __forceinline__ void stream_body(const d3r_align_desc& D, int it, con
   };
   auto flush_image = [&]() {
     if (simg >= 0 && lane < kImgVals) {
-      fix_add(ws.img_acc + int64_t(simg) * kImgVals + lane, s_img[lane], ws.flags);
+      fix_add(ws.img_acc + int64_t(simg) * kImgVals + lane, s_img[lane], ovf_flag);
       s_img[lane] = 0.f;
     }
     __syncwarp();
@@ -418,6 +423,7 @@ __device__ __forceinline__ void stream_body(const d3r_align_desc& D, int it, con
   if (dbg && lane == 0) dbg[2] = gtime();
   const int scr_floats = int(size_t(kSWarps) * per_warp / 4);
   if (!kGrad && warp == 0) prefetch_small_step_inputs(D, ws, it, scr_floats, lane, 32);
+  if (kSplit) return;
 
   // ---- grid ticket: the last CTA to finish runs the small-parameter step ----
   __syncthreads();
@@ -437,13 +443,39 @@ __device__ __forceinline__ void stream_body(const d3r_align_desc& D, int it, con
 template <bool kL2, int PPT, int NST>
 __global__ void __launch_bounds__(kSThreads, 2)
 align_stream_kernel(const __grid_constant__ d3r_align_desc D, int it) {
-  stream_body<false, kL2, PPT, NST>(D, it, GradOut{});
+  stream_body<false, kL2, PPT, NST, false>(D, it, GradOut{});
+}
+
+template <bool kL2, int PPT, int NST>
+__global__ void __launch_bounds__(kSThreads, 2)
+align_stream_pixel_kernel(const __grid_constant__ d3r_align_desc D, int it) {
+  stream_body<false, kL2, PPT, NST, true>(D, it, GradOut{});
+}
+
+// Second half of a split iteration: one CTA with the blockDim and dynamic shared memory of a streaming CTA, so that
+// small_step picks the same version the fused launch's last CTA does, runs it on the (all-reduced) accumulators.  The
+// pixel passes' overflow word joins the flag before any total is read; the word is cleared with the accumulators.
+template <int PPT, int NST>
+__global__ void __launch_bounds__(kSThreads, 2)
+align_small_step_kernel(const __grid_constant__ d3r_align_desc D, int it) {
+  constexpr int kStage = kHdrBytes + PPT * kSlotBytes;
+  extern __shared__ __align__(128) uint8_t s_dyn[];
+  __shared__ float s_red[40];
+  const Workspace ws = carve(D.workspace, D.n_imgs, D.n_edges);
+  const int acc_floats = (D.stream_window * kEntVals + 16 + 31) & ~31;
+  const int scr_floats = int(size_t(kSWarps) * (size_t(NST) * kStage + size_t(acc_floats) * 4) / 4);
+  // everything below reads what the pixel pass and the reduction wrote
+  pdl::sync_with_predecessor();
+  if (threadIdx.x == 0 && __ldcg(ws.ovf) != 0) *ws.flags = 1;
+  __syncthreads();
+  small_step(D, ws, it, s_red, reinterpret_cast<float*>(s_dyn), scr_floats);
+  if (threadIdx.x == 0) *ws.ovf = 0;
 }
 
 template <bool kL2, int PPT, int NST>
 __global__ void __launch_bounds__(kSThreads, 2)
 align_stream_grad_kernel(const __grid_constant__ d3r_align_desc D, GradOut go) {
-  stream_body<true, kL2, PPT, NST>(D, 0, go);
+  stream_body<true, kL2, PPT, NST, false>(D, 0, go);
 }
 
 // ---- one launch packs every entry (device-resident forward output -> observation layout) ----------------------
@@ -496,18 +528,26 @@ size_t stream_smem_bytes(int ppt, int nst, int window) {
   return size_t(kSWarps) * (size_t(nst) * (kHdrBytes + ppt * kSlotBytes) + size_t(acc_floats) * 4);
 }
 
+// Ring depth of the streaming CTA: 4 stages while the entry window leaves room for two CTAs per SM, else 3.  Returns 0 and
+// sets the error when the window does not fit at all.
+static int stream_depth(const d3r_align_desc* desc, const char* op) {
+  const size_t budget = 113 * 1024;
+  if (stream_smem_bytes(3, 4, desc->stream_window) <= budget) return 4;
+  if (stream_smem_bytes(3, 3, desc->stream_window) <= budget) return 3;
+  set_error("%s: stream_window=%d does not fit shared memory", op, desc->stream_window);
+  return 0;
+}
+
 // go == nullptr: iterations [it_begin, it_end); otherwise one gradient launch
 int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, const GradOut* go, cudaStream_t st) {
   D3R_CHECK_ARG(desc->items && desc->warp_item_ptr && desc->n_items > 0 && desc->stream_grid > 0,
                 "d3r_align_run: streaming kernel selected without a work-item table");
   D3R_CHECK_ARG(desc->stream_ppt == 3, "d3r_align_run: stream_ppt=%d is not built (3)", desc->stream_ppt);
   D3R_CHECK_ARG(desc->stream_window >= 1, "d3r_align_run: stream_window must be >= 1");
-  // ring depth: 4 stages while the entry window leaves room for two CTAs per SM, else 3
-  const size_t budget = 113 * 1024;
-  const bool deep = stream_smem_bytes(3, 4, desc->stream_window) <= budget;
-  D3R_CHECK_ARG(deep || stream_smem_bytes(3, 3, desc->stream_window) <= budget, "d3r_align_run: stream_window=%d does not fit shared memory",
-                desc->stream_window);
-  const size_t smem = stream_smem_bytes(3, deep ? 4 : 3, desc->stream_window);
+  const int depth = stream_depth(desc, "d3r_align_run");
+  if (!depth) return D3R_ERR_INVALID;
+  const bool deep = depth == 4;
+  const size_t smem = stream_smem_bytes(3, depth, desc->stream_window);
   if (go) {
     void (*kernel)(d3r_align_desc, GradOut) = desc->dist_l2 ? (deep ? align_stream_grad_kernel<true, 3, 4> : align_stream_grad_kernel<true, 3, 3>)
                                                             : (deep ? align_stream_grad_kernel<false, 3, 4> : align_stream_grad_kernel<false, 3, 3>);
@@ -516,6 +556,28 @@ int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, const Gr
   void (*kernel)(d3r_align_desc, int) = desc->dist_l2 ? (deep ? align_stream_kernel<true, 3, 4> : align_stream_kernel<true, 3, 3>)
                                                       : (deep ? align_stream_kernel<false, 3, 4> : align_stream_kernel<false, 3, 3>);
   return launch_iterations(kernel, desc, desc->stream_grid, kSThreads, smem, it_begin, it_end, st);
+}
+
+// One half of split iteration `it`: the pixel pass over this descriptor's items (none: nothing to launch), or the
+// one-CTA small step.
+int launch_stream_split(const d3r_align_desc* desc, int it, bool pixel, cudaStream_t st) {
+  const char* op = pixel ? "d3r_align_pixel_pass" : "d3r_align_small_step";
+  D3R_CHECK_ARG(desc->stream_kernel, "%s: the split iteration runs on the streaming kernel only", op);
+  D3R_CHECK_ARG(desc->stream_ppt == 3, "%s: stream_ppt=%d is not built (3)", op, desc->stream_ppt);
+  D3R_CHECK_ARG(desc->stream_window >= 1, "%s: stream_window must be >= 1", op);
+  const int depth = stream_depth(desc, op);
+  if (!depth) return D3R_ERR_INVALID;
+  const bool deep = depth == 4;
+  const size_t smem = stream_smem_bytes(3, depth, desc->stream_window);
+  if (!pixel) {
+    void (*kernel)(d3r_align_desc, int) = deep ? align_small_step_kernel<3, 4> : align_small_step_kernel<3, 3>;
+    return launch_iterations(kernel, desc, 1, kSThreads, smem, it, it + 1, st);
+  }
+  if (desc->n_items == 0) return D3R_OK;
+  D3R_CHECK_ARG(desc->items && desc->warp_item_ptr && desc->stream_grid > 0, "%s: no work-item table", op);
+  void (*kernel)(d3r_align_desc, int) = desc->dist_l2 ? (deep ? align_stream_pixel_kernel<true, 3, 4> : align_stream_pixel_kernel<true, 3, 3>)
+                                                      : (deep ? align_stream_pixel_kernel<false, 3, 4> : align_stream_pixel_kernel<false, 3, 3>);
+  return launch_iterations(kernel, desc, desc->stream_grid, kSThreads, smem, it, it + 1, st);
 }
 
 }  // namespace align

@@ -11,9 +11,14 @@ The collective is a single `all_gather_into_tensor` of one packed fp32 buffer: r
 tensors handed to the caller are VIEWS of the gathered buffer (no unpacking copy when the pair count divides
 the world size; one row gather otherwise).  `PairOutputGather` is the object both `inference_sharded` and
 `bench.py --gpus N` use; with `async_op=True` it double-buffers so that the gather of step k overlaps the
-forward of step k+1.  Works with backend 'nccl' (GPU) and 'gloo' (CPU tests)."""
+forward of step k+1.  Works with backend 'nccl' (GPU) and 'gloo' (CPU tests).
+
+Global alignment shards the other way round: `global_aligner_sharded` gives every rank a contiguous range of images
+(`shard_images`); each rank streams only those images' observations and the ranks exchange the fixed-point accumulator
+block with one all-reduce per iteration (cloud_opt/engine.py)."""
 from __future__ import annotations
 
+import numpy as np
 import torch
 import torch.distributed as dist
 
@@ -26,6 +31,63 @@ def shard_bounds(n_items: int, world: int, rank: int):
     base, extra = divmod(n_items, world)
     start = rank * base + min(rank, extra)
     return start, start + base + (1 if rank < extra else 0)
+
+
+def shard_images(imshapes, degrees, world):
+    """Contiguous image ranges [lo, hi), one per rank, balanced by the alignment kernel's streaming cost: 64-pixel slots x
+    (entries of the image + fixed per-pixel work), the cost build_stream_items balances its warps by.  Every boundary is
+    the image boundary closest to an even split, so each rank's cost is within one image's cost of total / world.  With
+    fewer images than ranks some ranges are empty; those ranks still take part in every collective."""
+    from .cloud_opt.engine import SLOT_PX, stream_cost
+    slots = [(h * w + SLOT_PX - 1) // SLOT_PX for h, w in imshapes]
+    cum = np.concatenate([[0.0], np.cumsum(stream_cost(slots, degrees))])
+    n, world = len(imshapes), int(world)
+    bounds = [0]
+    for r in range(1, world):
+        target = cum[-1] * r / world
+        b = int(np.searchsorted(cum, target, side='left'))      # first boundary at or past the target
+        if b > 0 and target - cum[b - 1] <= cum[b] - target:    # the one before it is closer
+            b -= 1
+        bounds.append(min(max(b, bounds[-1]), n))
+    bounds.append(n)
+    return [(bounds[r], bounds[r + 1]) for r in range(world)]
+
+
+class _AlignShard:
+    """What a sharded scene's engine needs: the image range of every rank and the process group.  Shared, not copied, by
+    deepcopy (mask_sky copies the scene; a process group cannot be copied)."""
+
+    def __init__(self, shards, group):
+        self.shards, self.group = shards, group
+
+    def __deepcopy__(self, memo):
+        return self
+
+
+def global_aligner_sharded(dust3r_output, device, mode=None, group=None, **optim_kw):
+    """global_aligner() whose alignment loop runs on every rank of `group` (default: the whole default group), each rank
+    streaming the observations of its own contiguous range of images (shard_images) and all ranks combining the exact
+    fixed-point sums with one all-reduce per iteration.  Every rank passes the same full `dust3r_output` (inference_sharded
+    returns it on every rank) and ends with the same aligned scene.
+
+    Without an initialised process group, or in a group of one rank, this is global_aligner().  PairViewer has no loop
+    and is returned as global_aligner builds it.  On the returned scene compute_global_alignment (every init=), scene()
+    under no_grad, the getters, clean_pointcloud and mask_sky behave as on one GPU; the differentiable objective
+    (loss.backward(), ret_details=True) raises NotImplementedError.  The predictions still live whole on every rank: only
+    the packed observations and the per-pixel Adam state are divided."""
+    from .cloud_opt import GlobalAlignerMode, global_aligner
+    mode = GlobalAlignerMode.PointCloudOptimizer if mode is None else mode
+    scene = global_aligner(dust3r_output, device, mode=mode, **optim_kw)
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return scene
+    if mode is GlobalAlignerMode.PairViewer:
+        return scene
+    degrees = [0] * scene.n_imgs
+    for i, j in scene.edges:
+        degrees[i] += 1
+        degrees[j] += 1
+    scene._align_shard = _AlignShard(shard_images(scene.imshapes, degrees, dist.get_world_size(group)), group)
+    return scene
 
 
 class PairOutputGather:

@@ -166,6 +166,21 @@ int64_t d3r_align_workspace_floats(int32_t n_imgs, int32_t n_edges);
 int d3r_align_prepare(const d3r_align_desc* desc, void* stream);
 /* Runs iterations [it_begin, it_end) (indices into sched / loss_out).  Asynchronous. */
 int d3r_align_run(const d3r_align_desc* desc, int32_t it_begin, int32_t it_end, void* stream);
+/* One iteration as two launches, so that a caller can combine the cross-CTA sums of several GPUs in between:
+ *   d3r_align_pixel_pass(desc, it)   the streaming kernel's per-pixel work over desc's items (unprojection, residuals,
+ *                                    dL/dlog-depth, the depth Adam step) -- nothing is launched when n_items == 0;
+ *   all-reduce(SUM) of the int64 block that d3r_align_reduce_block locates in `workspace` (optional: one GPU needs none);
+ *   d3r_align_small_step(desc, it)   the small-parameter step of d3r_align_run's last CTA on the (reduced) sums: loss_out[it],
+ *                                    Adam on `small`, the derived transforms; with desc->eval_only only loss_out[it].
+ * Streaming kernel only (stream_kernel = 1).  On one GPU the pair gives the same bits as d3r_align_run(desc, it, it + 1).
+ * Every GPU runs the small step on the same reduced block and so computes the same `small`; each GPU's pixel pass updates
+ * only the log-depths of its own items' images.  The block is [ent_acc | img_acc | overflow word]: the fixed-point sums
+ * (integers, so the all-reduce is exact and order-independent) and a word the pixel pass makes non-zero when a partial sum
+ * left the range or met a NaN / Inf, which the small step turns into the overflow flag.  Asynchronous. */
+int d3r_align_pixel_pass(const d3r_align_desc* desc, int32_t it, void* stream);
+int d3r_align_small_step(const d3r_align_desc* desc, int32_t it, void* stream);
+/* *offset_floats: where the all-reduce block starts in `workspace` (in floats, 16-byte aligned); *n_words: its length in int64. */
+int d3r_align_reduce_block(int32_t n_imgs, int32_t n_edges, int64_t* offset_floats, int64_t* n_words);
 /* Objective and its gradient at the current parameters (net.forward() + loss.backward()): one launch of the pixel kernel
  * the descriptor selects + the last-CTA small step.  Updates no parameter or Adam moment; reads neither sched nor the moments
  * (logd_m, logd_v, small_m, small_v, small_trainable and sched may be NULL).  Call d3r_align_prepare first when `small` changed.
@@ -179,7 +194,7 @@ int d3r_align_run(const d3r_align_desc* desc, int32_t it_begin, int32_t it_end, 
 int d3r_align_loss_grad(const d3r_align_desc* desc, float* logd_grad, float* small_grad, float* entry_loss, void* stream);
 /* Cross-CTA sums use order-independent 2^40 fixed-point integer atomics (bit-reproducible).  *host_out = 1 when a
  * partial sum (|x| >= 2^18) or a total (|x| >= 2^22) left the supported range (unreasonably scaled scene, NaN / Inf input)
- * since iteration 0 of the current d3r_align_run batch, or during the last d3r_align_loss_grad.  Every iteration from the one
+ * since iteration 0 of the current d3r_align_run batch (or of the split iterations), or during the last d3r_align_loss_grad.  Every iteration from the one
  * that set it writes NaN to loss_out (eval_only runs included). */
 int d3r_align_overflow_flag(const d3r_align_desc* desc, int32_t* host_out, void* stream);
 /* World-frame pointmaps X[i] = R_i * unproject(depth_i) + T_i for every image
