@@ -2,12 +2,11 @@
 
 Same contract as the reference: takes the `make_pairs` list, returns {'view1','view2','pred1','pred2','loss'}
 with every tensor ON CPU, concatenated over pairs in input order (lists when image sizes are mixed).
-Differences are internal: each batch runs as C-ABI encode and decode calls (d3r_encode_images, d3r_decode_pairs),
-device->host copies of the predictions go through pinned staging buffers and overlap the next batch's compute, and
-`keep_on_device=True` (extension) skips the host round trip for callers that feed global_aligner next
-(SURVEY §8f rank 2).  Pair lists that share images (make_pairs) encode each image once (model.encode_images) and
-decode every batch from those features (model.decode_pairs); pair lists of several image sizes are decoded in
-batches of one (size, size) group each instead of one pair per call."""
+Differences are internal: the list runs as C-ABI encode and decode calls (model.encode_images / model.decode_pairs:
+d3r_encode_images, d3r_decode_pairs) that encode each distinct image once and decode pairs from those features, in
+batches of one (size, size) group each when sizes are mixed; device->host copies of the predictions go through pinned
+buffers and overlap the next calls' compute, and `keep_on_device=True` (extension) skips the host round trip for callers
+that feed global_aligner next (SURVEY §8f rank 2)."""
 from __future__ import annotations
 
 import os
@@ -62,13 +61,6 @@ def check_if_same_size(pairs):
 
 
 _POOL = None
-_TRACE = None   # set to a list to collect (label, perf_counter) host timestamps of the pipeline (diagnostics)
-
-
-def _mark(label):
-    if _TRACE is not None:
-        import time
-        _TRACE.append((label, time.perf_counter()))
 
 
 def _copy_pool():
@@ -79,21 +71,16 @@ def _copy_pool():
     return _POOL
 
 
-def _fill_pinned(dst, tensors, row0, wait=True):
-    """Copy each view's image rows into the pinned staging tensor `dst` starting at row `row0` (memcpy on a small
-    thread pool: Tensor.copy_ releases the GIL, one thread saturates only ~10 GB/s of host bandwidth).
-    Returns (next row, futures); with wait=False the copies are left running in the background."""
-    jobs, r = [], row0
-    for t in tensors:
-        k = int(t.shape[0])
-        jobs.append((dst[r:r + k], t))
-        r += k
+def _fill_pinned(jobs, wait=True):
+    """Run each (pinned destination, source) copy of `jobs` on a small thread pool (Tensor.copy_ releases the GIL, one
+    thread saturates only ~10 GB/s of host bandwidth).  With wait=False the copies are left running in the background and
+    their futures returned."""
     futs = [_copy_pool().submit(d.copy_, t) for d, t in jobs]
-    if wait:
-        for f in futs:
-            f.result()
-        futs = []
-    return r, futs
+    if not wait:
+        return futs
+    for f in futs:
+        f.result()
+    return []
 
 
 def _uploadable(t, dev):
@@ -114,94 +101,174 @@ def _micro_batch(batch_size):
     return half + (half & 1)
 
 
-def _distinct_images(views):
-    """The distinct image tensors of single-image view dicts, by identity (make_pairs reuses one dict per image in many
-    pairs), in order of first use, and per view the index of each pair's image in that list."""
-    uniq, order, gidx = {}, [], ([], [])
+def _distinct_images(rows):
+    """The distinct images of the rows of both views, by storage identity (make_pairs reuses one view dict per image in
+    many pairs), in order of first use; the (view, row) of each one's first use; per view the index of each row's image."""
+    uniq, first, gidx = {}, [], ([], [])
     for k in range(2):
-        for v in views[k]:
-            t = v['img']
+        for i, t in enumerate(rows[k]):
             key = (t.data_ptr(), tuple(t.shape), tuple(t.stride()))
             if key not in uniq:
-                uniq[key] = len(order)
-                order.append(t)
+                uniq[key] = len(first)
+                first.append((k, i))
             gidx[k].append(uniq[key])
-    return order, gidx
+    return [rows[k][i] for k, i in first], first, gidx
 
 
-def _upload(ts, dev, up):
-    """One device tensor holding the images `ts` (each (1,3,H,W), one size), copied on the stream `up`; the current stream
-    waits for the copy."""
+def _groups(gidx, mb):
+    """Rows of the pipeline's groups: the list is cut into the shortest runs of consecutive rows that share no image with
+    another run, and consecutive runs are joined while the group stays within `mb` rows (a longer run is a group alone)."""
+    last = [0] * (1 + max(max(ix) for ix in gidx))
+    for ix in gidx:
+        for i, j in enumerate(ix):
+            last[j] = max(last[j], i)
+    groups, start, end = [], 0, 0
+    for i in range(len(gidx[0])):
+        end = max(end, last[gidx[0][i]], last[gidx[1][i]])
+        if i == end:
+            if groups and i + 1 - groups[-1].start <= mb:
+                groups[-1] = range(groups[-1].start, i + 1)
+            else:
+                groups.append(range(start, i + 1))
+            start = i + 1
+    return groups
+
+
+def _takes_pipeline(pairs, model, dev):
+    """Whether inference() runs `pairs` as encode / decode calls.  The rest -- ManyAR batches of a landscape_only model,
+    a true_shape other than its tensor's size, view dicts of several images in a list of several sizes, CPU stand-ins and
+    models without encode_images / decode_pairs -- runs the reference's loop, where forward() checks and handles it."""
+    if dev.type != 'cuda' or not (hasattr(model, 'encode_images') and hasattr(model, 'decode_pairs')) or not pairs:
+        return False
+    views = {id(v): v for pair in pairs for v in pair}.values()
+    for v in views:
+        hw = tuple(int(s) for s in v['img'].shape[-2:])
+        ts = v.get('true_shape')
+        if ts is not None and any(tuple(s) != hw for s in torch.as_tensor(ts).reshape(-1, 2).tolist()):
+            return False
+        if getattr(model, 'landscape_only', True) and hw[0] > hw[1]:
+            return False
+    return check_if_same_size(pairs) or all(int(v['img'].shape[0]) == 1 for v in views)
+
+
+def _pipeline(pairs, model, dev, mb, verbose, keep_on_device, return_images):
+    """inference() as encode / decode calls, group by group (_groups): the group's distinct images are uploaded on a copy
+    stream and encoded once, one size at a time, in calls of at most 2 * mb images (what forward() on mb pairs encodes);
+    its pairs are decoded per (view-1 size, view-2 size) in input order, at most mb per call, and the predictions copied out
+    on a second side stream -- so the upload of the next group and the download of the last overlap the compute."""
+    rows = ([], [])   # one (1,3,H,W) image per row: a view dict of k images is k pairs
+    for a, b in pairs:
+        k = int(a['img'].shape[0])
+        assert int(b['img'].shape[0]) == k, 'both views of a pair must hold the same number of images'
+        for r, v in zip(rows, (a, b)):
+            r.extend([v['img']] if k == 1 else v['img'].split(1))
+    n = len(rows[0])
+    single = check_if_same_size(pairs)
+    order, first, gidx = _distinct_images(rows)
+    # An image that is neither pinned nor on the GPU goes up from a pinned copy: with one size and images returned, its first
+    # row in the returned views (the other rows are filled in the background, call by call); with several sizes and host
+    # images returned, a pinned copy kept for the returned views; otherwise a staging buffer of one encode call's images.
+    img_pin = [torch.empty((n,) + tuple(r[0].shape[1:]), dtype=r[0].dtype, pin_memory=True) for r in rows] \
+        if single and return_images else None
+    keep_host = return_images and not single and not keep_on_device
+    returned = {}   # several sizes, images returned: image -> its pinned (or, keep_on_device, device) copy
     main = torch.cuda.current_stream(dev)
-    out = torch.empty((len(ts),) + tuple(ts[0].shape[1:]), dtype=ts[0].dtype, device=dev)
-    up.wait_stream(main)
-    with torch.cuda.stream(up):
-        if all(_uploadable(t, dev) for t in ts):
-            for j, t in enumerate(ts):
-                out[j:j + 1].copy_(t, non_blocking=True)
-        else:
-            stage = torch.empty(out.shape, dtype=out.dtype, pin_memory=True)
-            _fill_pinned(stage, ts, 0, wait=True)
-            out.copy_(stage, non_blocking=True)
-    ev = torch.cuda.Event()
-    ev.record(up)
-    main.wait_event(ev)
-    return out
-
-
-def _encode(model, imgs, chunk):
-    """Encoder features of every image of `imgs`, in calls of at most `chunk` images (what bounds the encoder's workspace:
-    forward() on `chunk // 2` pairs encodes up to `chunk` images)."""
-    parts = [model.encode_images(imgs[c:c + chunk]) for c in range(0, int(imgs.shape[0]), chunk)]
-    return parts[0] if len(parts) == 1 else torch.cat(parts)
-
-
-def _inference_mixed(pairs, model, dev, batch_size, verbose, keep_on_device, return_images):
-    """Pair lists of more than one image size (one image per view dict, a model with landscape_only=False): every distinct
-    image is uploaded and encoded once, one size at a time, and the pairs of each (view-1 size, view-2 size) group are
-    decoded in input order, `batch_size` pairs per call.  The result is the reference's one-pair-per-call loop
-    (inference.py:60-72): lists with one entry per pair, in input order, with the same values -- a pair's output does not
-    depend on the batch it is computed in."""
-    n = len(pairs)
-    views = ([a for a, b in pairs], [b for a, b in pairs])
-    order, gidx = _distinct_images(views)
-    by_size = {}
-    for j, t in enumerate(order):
-        by_size.setdefault(tuple(t.shape[-2:]), []).append(j)
-    slot = [None] * len(order)   # distinct image -> (its size, its row in that size's feature tensor)
-    up = torch.cuda.Stream(device=dev)
-    imgs, feats = {}, {}
-    for hw, js in by_size.items():
-        for r, j in enumerate(js):
-            slot[j] = (hw, r)
-        imgs[hw] = _upload([order[j] for j in js], dev, up)
-        feats[hw] = _encode(model, imgs[hw], 2 * batch_size)
-        if not return_images:
-            del imgs[hw]
-        elif not keep_on_device:
-            imgs[hw] = imgs[hw].cpu()
-    groups = {}
-    for i in range(n):
-        groups.setdefault((slot[gidx[0][i]][0], slot[gidx[1][i]][0]), []).append(i)
-    preds = [None] * n
+    up, side = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
+    up.wait_stream(main)   # images written on the device before the call
+    outs, preds, pending = None, [None] * n, []
     with tqdm.tqdm(total=n, disable=not verbose) as bar:
-        for (hw1, hw2), members in groups.items():
-            for c in range(0, len(members), batch_size):
-                sel = members[c:c + batch_size]
-                out = model.decode_pairs(feats[hw1], [slot[gidx[0][i]][1] for i in sel],
-                                         feats[hw2], [slot[gidx[1][i]][1] for i in sel])
-                out = out if keep_on_device else to_cpu(out)
-                for j, i in enumerate(sel):
-                    preds[i] = tuple({key: t[j:j + 1] for key, t in p.items()} for p in out)
-                bar.update(len(sel))
+        for g in _groups(gidx, mb):
+            js = sorted({ix[i] for ix in gidx for i in g})
+            src = {}   # image -> the pinned copy it is uploaded from
+            if img_pin is not None:
+                src = {j: img_pin[k][i:i + 1] for j in js if not _uploadable(order[j], dev) for k, i in [first[j]]}
+                _fill_pinned([(src[j], order[j]) for j in src])
+                filled = {first[j] for j in src}
+            by_size, feats, at = {}, {}, {}   # at: image -> (its size, its row in that size's features)
+            for j in js:
+                by_size.setdefault(tuple(order[j].shape[-2:]), []).append(j)
+            for hw, sj in by_size.items():
+                parts = []
+                for c in range(0, len(sj), 2 * mb):
+                    chunk = sj[c:c + 2 * mb]
+                    shape, dtype = (len(chunk),) + tuple(order[chunk[0]].shape[1:]), order[chunk[0]].dtype
+                    staged = [j for j in chunk if j not in src and (keep_host or not _uploadable(order[j], dev))]
+                    if staged:
+                        stage = torch.empty((len(staged),) + shape[1:], dtype=dtype, pin_memory=True)
+                        src.update((j, stage[r:r + 1]) for r, j in enumerate(staged))
+                        _fill_pinned([(src[j], order[j]) for j in staged])
+                    # allocated on the copy stream and recorded on the main one: the memory is reused once the encode
+                    # that reads it has run, without making the next upload wait for this group's compute
+                    with torch.cuda.stream(up):
+                        img = torch.empty(shape, dtype=dtype, device=dev)
+                        for r, j in enumerate(chunk):
+                            img[r:r + 1].copy_(src.get(j, order[j]), non_blocking=True)
+                    ev = torch.cuda.Event()
+                    ev.record(up)
+                    main.wait_event(ev)
+                    img.record_stream(main)
+                    parts.append(model.encode_images(img))
+                    if return_images and not single:
+                        returned.update((j, img[r:r + 1] if keep_on_device else src[j]) for r, j in enumerate(chunk))
+                feats[hw] = parts[0] if len(parts) == 1 else torch.cat(parts)
+                at.update((j, (hw, r)) for r, j in enumerate(sj))
+            calls = {}
+            for i in g:
+                calls.setdefault((at[gidx[0][i]][0], at[gidx[1][i]][0]), []).append(i)
+            for (hw1, hw2), members in calls.items():
+                for c in range(0, len(members), mb):
+                    sel = members[c:c + mb]
+                    if img_pin is not None:
+                        pending += _fill_pinned([(img_pin[k][i:i + 1], rows[k][i]) for k in range(2) for i in sel
+                                                 if (k, i) not in filled], wait=False)
+                    pred1, pred2 = model.decode_pairs(feats[hw1], [at[gidx[0][i]][1] for i in sel],
+                                                      feats[hw2], [at[gidx[1][i]][1] for i in sel])
+                    flat = {('pred1', key): t for key, t in pred1.items()}
+                    flat.update({('pred2', key): t for key, t in pred2.items()})
+                    if single:   # one stacked result; a group's rows are consecutive
+                        if outs is None:
+                            outs = {key: torch.empty((n,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev if keep_on_device else None,
+                                                     pin_memory=not keep_on_device) for key, t in flat.items()}
+                        dst = {key: outs[key][sel[0]:sel[0] + len(sel)] for key in flat}
+                    elif keep_on_device:
+                        dst = flat
+                    else:
+                        dst = {key: torch.empty(t.shape, dtype=t.dtype, pin_memory=True) for key, t in flat.items()}
+                    if dst is not flat:
+                        ev = torch.cuda.Event()
+                        ev.record(main)
+                        side.wait_event(ev)
+                        with torch.cuda.stream(side):
+                            for key, t in flat.items():
+                                dst[key].copy_(t, non_blocking=True)
+                                t.record_stream(side)
+                    if not single:
+                        for r, i in enumerate(sel):
+                            preds[i] = tuple({key: t[r:r + 1] for (w, key), t in dst.items() if w == which}
+                                             for which in ('pred1', 'pred2'))
+                    bar.update(len(sel))
+            del feats
+    side.synchronize()
+    for f in pending:
+        f.result()
+    views = ([a for a, b in pairs], [b for a, b in pairs])
+    if single:
+        vs = [{key: collate_with_cat([v[key] for v in views[k]]) for key in views[k][0] if key != 'img'} for k in range(2)]
+        if return_images:
+            for k in range(2):
+                vs[k]['img'] = img_pin[k]
+        res = dict(view1=vs[0], view2=vs[1], pred1={}, pred2={}, loss=None)
+        for (which, key), t in outs.items():
+            res[which][key] = t
+        return res
+    # several sizes: the reference's one-pair-per-call loop (inference.py:60-72), lists with one entry per pair
     results = []
     for i in range(n):
         vs = []
         for k in range(2):
             v = collate_with_cat([views[k][i]])
             if return_images:
-                hw, r = slot[gidx[k][i]]
-                v['img'] = imgs[hw][r:r + 1]
+                v['img'] = returned[gidx[k][i]]
             else:
                 del v['img']
             if keep_on_device:   # where loss_of_one_batch puts the other fields of a view
@@ -215,135 +282,23 @@ def _inference_mixed(pairs, model, dev, batch_size, verbose, keep_on_device, ret
 @torch.no_grad()
 def inference(pairs, model, device, batch_size=8, verbose=True, keep_on_device=False, return_images=True):
     """inference.py:55-72.  Returns {'view1','view2','pred1','pred2','loss'}; tensors on CPU (pinned) unless
-    keep_on_device.  Software pipeline over micro-batches: images are gathered into pinned host memory (which is
-    also the returned, collated view; return_images=False -- extension -- leaves 'img' out of the returned views and skips
-    that copy where the upload does not need it), uploaded on a copy stream, run through one forward call, and the
-    predictions are copied D2H on a second side stream into the final (whole pair list) pinned output -- the
-    upload of batch k+1 and the download of batch k-1 overlap the compute of batch k."""
+    keep_on_device; lists with one entry per pair when the image sizes are mixed.  return_images=False (extension) leaves
+    'img' out of the returned views and skips the host copy behind them where the upload does not need it.
+
+    On a CUDA device, a model with encode_images / decode_pairs runs every list _takes_pipeline accepts as one pipeline
+    (_pipeline): each distinct image of the list (by storage: make_pairs shares one view dict between many pairs) is
+    uploaded and encoded once, and its pairs are decoded from those features in calls of at most one micro-batch
+    (_micro_batch), overlapped with the upload of the next images and the download of the last predictions.  Every other
+    list runs the reference's loop of forward() calls."""
     if verbose:
         print(f'>> Inference with model on {len(pairs)} image pairs')
-    multiple_shapes = not check_if_same_size(pairs)
     dev = torch.device(device)
-    if (multiple_shapes and dev.type == 'cuda' and hasattr(model, 'decode_pairs') and not getattr(model, 'landscape_only', True)
-            and all(int(v['img'].shape[0]) == 1 for pair in pairs for v in pair)):
-        return _inference_mixed(pairs, model, dev, batch_size, verbose, keep_on_device, return_images)
-    fused = dev.type == 'cuda' and not multiple_shapes and len(pairs) > 0
-    if not fused:
-        # mixed image sizes (batch size forced to 1, lists instead of stacked tensors) or non-CUDA stand-in
-        # models used by host-side tests: plain reference control flow
-        result = []
-        bs = 1 if multiple_shapes else batch_size
-        for i in tqdm.trange(0, len(pairs), bs, disable=not verbose):
-            res = loss_of_one_batch(collate_with_cat(pairs[i:i + bs]), model, None, device)
-            result.append(res if keep_on_device else to_cpu(res))
-        return collate_with_cat(result, lists=multiple_shapes)
-
-    _mark('begin')
-    n = len(pairs)
-    views = ([a for a, b in pairs], [b for a, b in pairs])
-    rows = [sum(int(v['img'].shape[0]) for v in vs) for vs in views]
-    assert rows[0] == rows[1], 'both views of a pair must hold the same number of images'
-    proto = [vs[0]['img'] for vs in views]
-    # pinned staging = the collated 'img' of the returned views; device copies of the whole pair list (a few MB / pair)
-    img_pin = None    # allocated below, unless the caller does not want the images back and the upload does not stage through it
-    img_dev = None    # device copies of both views: only the path without shared images needs them (allocated there)
-    meta_all = [{key: collate_with_cat([v[key] for v in vs]) for key in vs[0] if key != 'img'} for vs in views]
-    _mark('alloc+meta')
-    outs = None
-    main = torch.cuda.current_stream(dev)
-    up, side = torch.cuda.Stream(device=dev), torch.cuda.Stream(device=dev)
-    up.wait_stream(main)
-    mb = _micro_batch(batch_size)
-    r0 = 0
-    pending = []
-    # pair lists from make_pairs reuse the same image dict in many pairs (n images -> up to n(n-1) pairs): upload and encode
-    # every distinct image once, then decode each micro-batch from those features through index maps -- the encoder runs
-    # once per image of the list instead of twice per pair (its output for an image does not depend on what else is in
-    # the batch, so results are unchanged).  Encoder calls take at most 2 * mb images, as forward() on mb pairs does.
-    feats, gidx = None, ([], [])
-    if hasattr(model, 'decode_pairs') and all(int(v['img'].shape[0]) == 1 for vs in views for v in vs):
-        order, gidx = _distinct_images(views)
-        if len(order) < 2 * n:
-            feats = _encode(model, _upload(order, dev, up), 2 * mb)
-    all_pinned = all(_uploadable(v['img'], dev) for vs in views for v in vs)
-    if return_images or not (feats is not None or all_pinned):
-        img_pin = [torch.empty((rows[k],) + tuple(proto[k].shape[1:]), dtype=proto[k].dtype, pin_memory=True) for k in range(2)]
-    for i in tqdm.trange(0, n, mb, disable=not verbose):
-        chunk = (views[0][i:i + mb], views[1][i:i + mb])
-        r1 = r0
-        srcs = [[v['img'] for v in chunk[k]] for k in range(2)]
-        direct = all(_uploadable(t, dev) for ts in srcs for t in ts)
-        indexed = feats is not None
-        for k in range(2):
-            # sources already in pinned memory are uploaded straight from where they are; the collated copy that the
-            # caller gets back is then filled in the background, off the critical path
-            if img_pin is None:
-                r1 = r0 + sum(int(t.shape[0]) for t in srcs[k])
-                continue
-            r1, futs = _fill_pinned(img_pin[k], srcs[k], r0, wait=not (direct or indexed))
-            pending.extend(futs)
-        _mark('fill')
-        if indexed:
-            _mark('h2d+meta')
-            pred1, pred2 = model.decode_pairs(feats, gidx[0][i:i + mb], feats, gidx[1][i:i + mb])
-        else:
-            # device staging: two micro-batch sized buffers per view, used alternately (the reference holds one batch on the
-            # GPU at a time; a whole-pair-list copy would grow by 4.7 MB per pair at 512x384).  A buffer is reused two
-            # micro-batches later: the upload stream first waits for the forward that last read it.
-            if img_dev is None:
-                per_item = [int(v['img'].shape[0]) for v in views[0]]
-                cap = max(sum(per_item[c:c + mb]) for c in range(0, n, mb))
-                img_dev = [[torch.empty((cap,) + tuple(proto[k].shape[1:]), dtype=proto[k].dtype, device=dev) for k in range(2)]
-                           for _ in range(2)]
-                dev_free = [None, None]
-            slot = (i // mb) & 1
-            nrow = r1 - r0
-            with torch.cuda.stream(up):
-                if dev_free[slot] is not None:
-                    up.wait_event(dev_free[slot])
-                for k in range(2):
-                    if direct:
-                        r = 0
-                        for t in srcs[k]:
-                            img_dev[slot][k][r:r + int(t.shape[0])].copy_(t, non_blocking=True)
-                            r += int(t.shape[0])
-                    else:
-                        img_dev[slot][k][:nrow].copy_(img_pin[k][r0:r1], non_blocking=True)
-            ev_up = torch.cuda.Event()
-            ev_up.record(up)
-            main.wait_event(ev_up)
-            d = [dict({key: collate_with_cat([v[key] for v in chunk[k]]) for key in chunk[k][0] if key != 'img'},
-                      img=img_dev[slot][k][:nrow]) for k in range(2)]
-            _mark('h2d+meta')
-            pred1, pred2 = model(d[0], d[1])
-            dev_free[slot] = torch.cuda.Event()
-            dev_free[slot].record(main)
-        _mark('forward-enqueued')
-        flat = {('pred1', k): v for k, v in pred1.items()}
-        flat.update({('pred2', k): v for k, v in pred2.items()})
-        if outs is None:
-            if keep_on_device:
-                outs = {key: torch.empty((rows[0],) + tuple(t.shape[1:]), dtype=t.dtype, device=dev) for key, t in flat.items()}
-            else:
-                outs = {key: torch.empty((rows[0],) + tuple(t.shape[1:]), dtype=t.dtype, pin_memory=True) for key, t in flat.items()}
-        ev = torch.cuda.Event()
-        ev.record(main)
-        with torch.cuda.stream(side):
-            side.wait_event(ev)
-            for key, t in flat.items():
-                outs[key][r0:r1].copy_(t, non_blocking=True)
-                t.record_stream(side)
-        _mark('d2h-enqueued')
-        r0 = r1
-    side.synchronize()
-    for f in pending:
-        f.result()
-    _mark('synced')
-    main.wait_stream(up)
-    if return_images:
-        res = dict(view1=dict(meta_all[0], img=img_pin[0]), view2=dict(meta_all[1], img=img_pin[1]), pred1={}, pred2={}, loss=None)
-    else:
-        res = dict(view1=dict(meta_all[0]), view2=dict(meta_all[1]), pred1={}, pred2={}, loss=None)
-    for (which, k), t in outs.items():
-        res[which][k] = t
-    return res
+    if _takes_pipeline(pairs, model, dev):
+        return _pipeline(pairs, model, dev, _micro_batch(batch_size), verbose, keep_on_device, return_images)
+    multiple_shapes = not check_if_same_size(pairs)
+    result = []
+    bs = 1 if multiple_shapes else batch_size
+    for i in tqdm.trange(0, len(pairs), bs, disable=not verbose):
+        res = loss_of_one_batch(collate_with_cat(pairs[i:i + bs]), model, None, device)
+        result.append(res if keep_on_device else to_cpu(res))
+    return collate_with_cat(result, lists=multiple_shapes)

@@ -2,8 +2,9 @@
 encode_images / decode_pairs / forward whose "features" and "pointmaps" are plain functions of each image's pixels, and the
 torch.cuda stream / event entry points inference() touches are no-ops, so everything it hands to the model can be inspected:
 each distinct image is encoded once, in calls within the workspace bound; each pair is decoded once, in its (size, size)
-group, in batches of at most batch_size; results land in input order with the structure of the reference's loop; and the
-lists that must keep today's paths never reach encode / decode.  No kernel runs; the numerics are the `-m gpu` tests' job."""
+group, in batches of at most one micro-batch; results land in input order with the structure of the reference's loop; and
+the lists forward() has to check or handle never reach encode / decode.  No kernel runs; the numerics are the `-m gpu`
+tests' job."""
 import contextlib
 import types
 
@@ -43,7 +44,7 @@ class _Model:
         return _feat(imgs)
 
     def decode_pairs(self, feat1, idx1, feat2, idx2):
-        self.decoded.append((tuple(feat1.shape), list(idx1), tuple(feat2.shape), list(idx2)))
+        self.decoded.append((feat1, list(idx1), feat2, list(idx2)))
         return _heads(feat1[list(idx1)], feat2[list(idx2)])
 
     def __call__(self, view1, view2):
@@ -65,13 +66,21 @@ class _Stream:
         pass
 
 
+PINNED = []   # shapes of the pinned buffers allocated under fake_cuda
+
+
 @pytest.fixture()
 def fake_cuda(monkeypatch):
-    """'cuda' tensors are CPU tensors, pinned memory is pageable memory, streams and events do nothing."""
+    """'cuda' tensors are CPU tensors, pinned memory is pageable memory (its allocations recorded in PINNED), streams and
+    events do nothing."""
     real_empty = torch.empty
+    PINNED.clear()
 
     def empty(*a, pin_memory=False, device=None, **k):
-        return real_empty(*a, **k)
+        t = real_empty(*a, **k)
+        if pin_memory:
+            PINNED.append(tuple(t.shape))
+        return t
 
     monkeypatch.setattr(torch, 'empty', empty)
     monkeypatch.setattr(torch.cuda, 'Stream', _Stream)
@@ -124,6 +133,16 @@ def _assert_same(a, b, path='out'):
         assert a == b, (path, a, b)
 
 
+def _staged_images(chunk):
+    """Pinned image buffers (n,3,H,W) allocated so far hold at most one encode call's images."""
+    assert all(s[0] <= chunk for s in PINNED if len(s) == 4 and s[1] == 3), PINNED
+
+
+def _positions(feat, imgs):
+    """Position in `imgs` of the image behind each row of the stand-in features `feat`."""
+    return [next(k for k, v in enumerate(imgs) if torch.equal(_feat(v['img'])[0], f)) for f in feat]
+
+
 def _check_encoded_once(model, distinct, chunk):
     assert all(0 < int(t.shape[0]) <= chunk for t in model.encoded), [int(t.shape[0]) for t in model.encoded]
     got = [e for t in model.encoded for e in t]
@@ -142,23 +161,24 @@ def test_mixed_sizes_group_decode_and_keep_the_loop_structure(fake_cuda, batch_s
     pairs = make_pairs(imgs, scene_graph='complete', prefilter=None, symmetrize=symmetrize)
     model = _Model()
     out = inf.inference(pairs, model, fake_cuda, batch_size=batch_size, verbose=False)
+    mb = inf._micro_batch(batch_size)
     assert not model.forwarded
-    _check_encoded_once(model, [v['img'] for v in imgs], 2 * batch_size)
-    # every pair decoded once, in the group of its two sizes, batches of at most batch_size, in input order within a group
+    _check_encoded_once(model, [v['img'] for v in imgs], 2 * mb)
+    # every pair decoded once, in the group of its two sizes, batches of at most mb, in input order within a group
     size_of = {id(v['img']): tuple(v['img'].shape[-2:]) for v in imgs}
     seen = []
-    for s1, i1, s2, i2 in model.decoded:
-        assert 0 < len(i1) == len(i2) <= batch_size
-        seen.extend(((s1[1] * 16, s1[2] * 16), (s2[1] * 16, s2[2] * 16)) for _ in i1)
+    for f1, i1, f2, i2 in model.decoded:
+        assert 0 < len(i1) == len(i2) <= mb
+        seen.extend(((f1.shape[1] * 16, f1.shape[2] * 16), (f2.shape[1] * 16, f2.shape[2] * 16)) for _ in i1)
     assert len(seen) == len(pairs)
     want = [(size_of[id(a['img'])], size_of[id(b['img'])]) for a, b in pairs]
     assert sorted(seen) == sorted(want)
     # each group's batches are full except its last one
     groups = {}
-    for s1, i1, s2, i2 in model.decoded:
-        groups.setdefault((s1, s2), []).append(len(i1))
+    for f1, i1, f2, i2 in model.decoded:
+        groups.setdefault((f1.shape, f2.shape), []).append(len(i1))
     for sizes in groups.values():
-        assert all(s == batch_size for s in sizes[:-1])
+        assert all(s == mb for s in sizes[:-1])
     _assert_same(out, _loop_reference(pairs, _Model(), fake_cuda))
 
 
@@ -172,57 +192,100 @@ def test_mixed_sizes_options(fake_cuda, keep_on_device, return_images):
     if not return_images:
         for view in ('view1', 'view2'):
             del ref[view]['img']
+        _staged_images(2 * inf._micro_batch(4))
     _assert_same(out, ref)
+
+
+KEYS = (('pred1', 'pts3d'), ('pred1', 'conf'), ('pred2', 'pts3d_in_other_view'), ('pred2', 'conf'))
 
 
 @pytest.mark.parametrize('batch_size', [1, 4, 16, 18])
 @pytest.mark.parametrize('graph,symmetrize', [('complete', True), ('complete', False), ('swin-2', True), ('oneref-1', True)])
-def test_same_size_scene_encodes_each_image_once(fake_cuda, batch_size, graph, symmetrize):
-    imgs = _views([(64, 96)] * 7, seed=batch_size)
-    pairs = make_pairs(imgs, scene_graph=graph, prefilter=None, symmetrize=symmetrize)
+@pytest.mark.parametrize('scenes', [1, 2])
+def test_same_size_scene_encodes_each_image_once(fake_cuda, batch_size, graph, symmetrize, scenes):
+    # with two scenes the list is the pairs of one followed by those of the other, which shares no image with it
+    imgs = [_views([(64, 96)] * 7, seed=batch_size + 100 * s) for s in range(scenes)]
+    per_scene = [make_pairs(v, scene_graph=graph, prefilter=None, symmetrize=symmetrize) for v in imgs]
+    imgs, pairs = sum(imgs, []), sum(per_scene, [])
     model = _Model()
     out = inf.inference(pairs, model, fake_cuda, batch_size=batch_size, verbose=False)
     mb = inf._micro_batch(batch_size)
     assert not model.forwarded
     _check_encoded_once(model, [v['img'] for v in imgs], 2 * mb)
-    # one decode call per micro-batch, in input order: the concatenated index lists are the pairs' images
+    # each scene is decoded in calls of one micro-batch, in input order: the concatenated index lists are the pairs' images
     pos = {id(v['img']): k for k, v in enumerate(imgs)}
-    assert [len(i1) for _, i1, _, _ in model.decoded] == [min(mb, len(pairs) - c) for c in range(0, len(pairs), mb)]
-    i1 = [i for _, ix, _, _ in model.decoded for i in ix]
-    i2 = [i for _, _, _, ix in model.decoded for i in ix]
-    enc_order = [next(k for k, v in enumerate(imgs) if torch.equal(v['img'], e[None])) for t in model.encoded for e in t]
-    assert [enc_order[i] for i in i1] == [pos[id(a['img'])] for a, b in pairs]
-    assert [enc_order[i] for i in i2] == [pos[id(b['img'])] for a, b in pairs]
+    assert [len(i1) for _, i1, _, _ in model.decoded] == [min(mb, len(p) - c) for p in per_scene for c in range(0, len(p), mb)]
+    assert [k for f, ix, _, _ in model.decoded for k in _positions(f[ix], imgs)] == [pos[id(a['img'])] for a, b in pairs]
+    assert [k for _, _, f, ix in model.decoded for k in _positions(f[ix], imgs)] == [pos[id(b['img'])] for a, b in pairs]
+    # no encode call, and no feature tensor handed to a decode call, holds images of both scenes
+    for t in model.encoded:
+        assert len({k // 7 for k in _positions(_feat(t), imgs)}) == 1
+    for f1, _, f2, _ in model.decoded:
+        assert len({k // 7 for k in _positions(torch.cat((f1, f2)), imgs)}) == 1
     # the stacked result equals the one-batch-per-call reference, row by row
     ref = collate_with_cat([to_cpu(inf.loss_of_one_batch(collate_with_cat(pairs[c:c + 1]), _Model(), None, fake_cuda))
                             for c in range(len(pairs))])
-    for which, key in (('pred1', 'pts3d'), ('pred1', 'conf'), ('pred2', 'pts3d_in_other_view'), ('pred2', 'conf')):
+    for which, key in KEYS:
         assert torch.equal(out[which][key], ref[which][key]), (which, key)
     assert torch.equal(out['view1']['img'], ref['view1']['img']) and out['view2']['idx'] == ref['view2']['idx']
+    # without the images in the result, pageable images are staged one encode call at a time
+    PINNED.clear()
+    bare = inf.inference(pairs, _Model(), fake_cuda, batch_size=batch_size, verbose=False, return_images=False)
+    _staged_images(2 * mb)
+    assert 'img' not in bare['view1'] and all(torch.equal(bare[which][key], out[which][key]) for which, key in KEYS)
 
 
-def test_all_distinct_and_landscape_only_lists_keep_their_paths(fake_cuda, monkeypatch):
-    # private copies of every image: the pipelined fused path, no encode / decode
+@pytest.mark.parametrize('batch_size', [4, 18])
+def test_private_copies_are_encoded_a_micro_batch_at_a_time(fake_cuda, batch_size):
+    """Private copies of every image share nothing, so every group is mb pairs: one encode call of its view-1 then view-2
+    images and one decode call -- the calls forward() makes on a micro-batch -- with the result of the shared list."""
     imgs = _views([(64, 96)] * 4)
     pairs = make_pairs(imgs, scene_graph='complete', prefilter=None, symmetrize=True)
     private = [(dict(a, img=a['img'].clone()), dict(b, img=b['img'].clone())) for a, b in pairs]
     model = _Model()
-    a = inf.inference(private, model, fake_cuda, batch_size=4, verbose=False)
-    assert model.forwarded and not model.encoded and not model.decoded
-    b = inf.inference(pairs, _Model(), fake_cuda, batch_size=4, verbose=False)
-    for which, key in (('pred1', 'pts3d'), ('pred2', 'pts3d_in_other_view'), ('pred2', 'conf')):
-        assert torch.equal(a[which][key], b[which][key])
-    # landscape_only=True with mixed sizes, and view dicts of two images: today's one-call-per-batch loop
+    a = inf.inference(private, model, fake_cuda, batch_size=batch_size, verbose=False)
+    mb, n = inf._micro_batch(batch_size), len(private)
+    assert not model.forwarded
+    assert [len(i1) for _, i1, _, _ in model.decoded] == [min(mb, n - c) for c in range(0, n, mb)]
+    assert len(model.encoded) == len(model.decoded)
+    for t, c in zip(model.encoded, range(0, n, mb)):
+        assert torch.equal(t, torch.cat([p[0]['img'] for p in private[c:c + mb]] + [p[1]['img'] for p in private[c:c + mb]]))
+    _assert_same(a, inf.inference(pairs, _Model(), fake_cuda, batch_size=batch_size, verbose=False))
+
+
+def test_view_dicts_of_several_images_are_taken_row_by_row(fake_cuda):
+    v = _views([(64, 96)] * 6, seed=5)
+    d = [collate_with_cat(v[c:c + 2]) for c in range(0, 6, 2)]
+    pairs = [(d[a], d[b]) for a in range(3) for b in range(3) if a != b]
+    model = _Model()
+    out = inf.inference(pairs, model, fake_cuda, batch_size=4, verbose=False)
+    assert not model.forwarded
+    _check_encoded_once(model, [x['img'] for x in v], 2 * inf._micro_batch(4))
+    ref = collate_with_cat([to_cpu(inf.loss_of_one_batch(collate_with_cat([p]), _Model(), None, fake_cuda)) for p in pairs])
+    for which, key in KEYS:
+        assert torch.equal(out[which][key], ref[which][key]), (which, key)
+    for view in ('view1', 'view2'):
+        assert torch.equal(out[view]['img'], ref[view]['img']) and out[view]['idx'] == ref[view]['idx']
+
+
+@pytest.mark.parametrize('case', ['landscape_only_mixed', 'two_image_mixed', 'landscape_only_portrait_true_shape'])
+def test_lists_forward_has_to_handle_take_the_loop(fake_cuda, monkeypatch, case):
+    """landscape_only=True with a portrait tensor, view dicts of two images in a list of several sizes, and a shared-image
+    list whose true_shape says portrait on a landscape_only=True model (a ManyAR batch): the reference's loop of forward()
+    calls, one pair per call when sizes are mixed."""
     calls = []
     real = inf.loss_of_one_batch
     monkeypatch.setattr(inf, 'loss_of_one_batch', lambda batch, m, *a, **k: calls.append(1) or real(batch, m, *a, **k))
-    mixed = make_pairs(_views(MIXED[:3]), scene_graph='complete', prefilter=None, symmetrize=True)
-    model = _Model(landscape_only=True)
-    inf.inference(mixed, model, fake_cuda, batch_size=4, verbose=False)
-    assert len(calls) == len(mixed) and not model.encoded and not model.decoded
-    calls.clear()
-    v = _views(MIXED)
-    two = [(collate_with_cat([v[0], v[4]]), collate_with_cat([v[4], v[0]])), (collate_with_cat([v[1], v[5]]), collate_with_cat([v[0], v[4]]))]
-    model = _Model()
-    inf.inference(two, model, fake_cuda, batch_size=4, verbose=False)
-    assert len(calls) == len(two) and not model.encoded and not model.decoded
+    model = _Model(landscape_only=case.startswith('landscape_only'))
+    if case == 'landscape_only_mixed':
+        pairs = make_pairs(_views(MIXED[:3]), scene_graph='complete', prefilter=None, symmetrize=True)
+    elif case == 'two_image_mixed':
+        v = _views(MIXED)
+        pairs = [(collate_with_cat([v[0], v[4]]), collate_with_cat([v[4], v[0]])),
+                 (collate_with_cat([v[1], v[5]]), collate_with_cat([v[0], v[4]]))]
+    else:
+        portrait = [dict(v, true_shape=torch.tensor([[96, 64]], dtype=torch.int32)) for v in _views([(64, 96)] * 4)]
+        pairs = make_pairs(portrait, scene_graph='complete', prefilter=None, symmetrize=True)
+    inf.inference(pairs, model, fake_cuda, batch_size=4, verbose=False)
+    assert len(calls) == (len(pairs) if case.endswith('mixed') else -(-len(pairs) // 4))
+    assert model.forwarded and not model.encoded and not model.decoded
