@@ -29,6 +29,9 @@ def global_aligner(dust3r_output, device, mode=GlobalAlignerMode.PointCloudOptim
     inference(keep_on_device=True) feeds, bit-identical results."""
     if not isinstance(mode, GlobalAlignerMode):
         raise NotImplementedError(f'Unknown mode {mode}')
+    if dust3r_output.get('owned') is not None:
+        raise ValueError("this output holds only the rows one rank keeps (inference_sharded(keep='owned')): align it with "
+                         'distributed.global_aligner_sharded over the same process group')
     early = optim_kw.pop('early_upload', os.environ.get('D3R_ALIGN_EARLY_UPLOAD', '0') == '1')
     pred1, pred2 = dust3r_output['pred1'], dust3r_output['pred2']
     if early and mode is not GlobalAlignerMode.PairViewer and torch.device(device).type == 'cuda':

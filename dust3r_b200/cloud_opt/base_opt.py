@@ -45,9 +45,13 @@ class BasePCOptimizer(nn.Module):
     def _init_from_views(self, view1, view2, pred1, pred2,
                          dist='l1', conf='log', min_conf_thr=3, base_scale=0.5,
                          allow_pw_adaptors=False, pw_break=20, rand_pose=torch.randn,
-                         iterationsCount=None, verbose=True, kernel='auto'):
+                         iterationsCount=None, verbose=True, kernel='auto', imshapes=None):
         """Scene graph from the output of inference(): view*['idx'] give the image ids of every pair, pred1 / pred2 the
-        two pointmaps (+ confidences) of every pair, both expressed in the first image's camera frame."""
+        two pointmaps (+ confidences) of every pair, both expressed in the first image's camera frame.
+
+        imshapes (extension): (H, W) of every image, for the rows of inference_sharded(keep='owned'), where pred1 / pred2
+        hold None for the pairs (or view-2 halves) this rank does not keep.  The per-edge dictionaries then hold only the
+        kept entries, and im_conf only this rank's maxima until distributed.global_aligner_sharded shares it."""
         super().__init__()
         if dist not in ALL_DISTS:
             raise KeyError(dist)
@@ -65,7 +69,7 @@ class BasePCOptimizer(nn.Module):
 
         # ---- observations, one entry per directed pair "i_j"
         def per_edge(stacked):
-            return NoGradParamDict({key: stacked[e] for e, key in enumerate(self.str_edges)})
+            return NoGradParamDict({key: stacked[e] for e, key in enumerate(self.str_edges) if stacked[e] is not None})
         pts_i, pts_j = pred1['pts3d'], pred2['pts3d_in_other_view']
         # equal-size scenes arrive as 4 stacked tensors: remember them so that .to(device) moves 4 buffers (one H2D
         # copy each, or none at all when inference(keep_on_device=True) / the all-gather left them in HBM) and the
@@ -73,7 +77,7 @@ class BasePCOptimizer(nn.Module):
         stacks = (pts_i, pts_j, pred1['conf'], pred2['conf'])
         self._obs_stacks = stacks if all(torch.is_tensor(t) for t in stacks) else None
         self.pred_i, self.pred_j = per_edge(pts_i), per_edge(pts_j)
-        self.imshapes = get_imshapes(self.edges, pts_i, pts_j)
+        self.imshapes = [tuple(hw) for hw in imshapes] if imshapes is not None else get_imshapes(self.edges, pts_i, pts_j)
         self.min_conf_thr = min_conf_thr
         self.conf_mode, self.conf_trf = conf, get_conf_trf(conf)
         self.conf_i, self.conf_j = per_edge(pred1['conf']), per_edge(pred2['conf'])
@@ -151,10 +155,15 @@ class BasePCOptimizer(nn.Module):
 
     @torch.no_grad()
     def _compute_img_conf(self, pred1_conf, pred2_conf):
-        im_conf = nn.ParameterList([torch.zeros(hw, device=pred1_conf[0].device) for hw in self.imshapes])
+        """Per-image maximum of the confidences of its entries (entries this rank does not keep are None and skipped)."""
+        first = next((c for confs in (pred1_conf, pred2_conf) for c in confs if c is not None), None)
+        dev = first.device if first is not None else None
+        im_conf = nn.ParameterList([torch.zeros(hw, device=dev) for hw in self.imshapes])
         for e, (i, j) in enumerate(self.edges):
-            im_conf[i] = torch.maximum(im_conf[i], pred1_conf[e])
-            im_conf[j] = torch.maximum(im_conf[j], pred2_conf[e])
+            if pred1_conf[e] is not None:
+                im_conf[i] = torch.maximum(im_conf[i], pred1_conf[e])
+            if pred2_conf[e] is not None:
+                im_conf[j] = torch.maximum(im_conf[j], pred2_conf[e])
         return im_conf
 
     # ---------------------------------------------------------------- pairwise poses
@@ -254,10 +263,11 @@ class BasePCOptimizer(nn.Module):
         dev = self.device
         keys = self.str_edges
         shard = self.__dict__.get('_align_shard')
+        # a scene of kept rows (inference_sharded(keep='owned')) lacks the entries of other ranks' images: the engine
+        # packs only its own images' entries and never reads those
         self._engine = AlignEngine(
             self.edges, self.imshapes,
-            [self.pred_i[k] for k in keys], [self.pred_j[k] for k in keys],
-            [self.conf_i[k] for k in keys], [self.conf_j[k] for k in keys],
+            *([obs.get(k) for k in keys] for obs in (self.pred_i, self.pred_j, self.conf_i, self.conf_j)),
             device=dev, conf_mode=self.conf_mode, dist=self.dist, variant=self._engine_variant(), pix_stride=self._engine_pix_stride(),
             base_scale=self.base_scale, pw_break=self.pw_break,
             focal_break=getattr(self, 'focal_break', getattr(self, 'focal_brake', 20)),

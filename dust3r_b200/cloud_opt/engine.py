@@ -99,7 +99,8 @@ class AlignEngine:
 
     shards: optional list of contiguous image ranges [lo, hi), one per rank of `group` (distributed.shard_images); this
     rank packs and streams only the entries of its own range, and run() / evaluate_loss() exchange the accumulators with
-    one all-reduce per iteration.  Streaming kernel only."""
+    one all-reduce per iteration.  Streaming kernel only.  The inputs of entries outside the range are never read and may
+    be None (a scene of the rows inference_sharded(keep='owned') kept)."""
 
     def __init__(self, edges: Sequence[Tuple[int, int]], imshapes: Sequence[Tuple[int, int]],
                  pred_i: Sequence[torch.Tensor], pred_j: Sequence[torch.Tensor],
@@ -193,8 +194,10 @@ class AlignEngine:
                 if not lo <= img < hi:      # another rank's image: its observations are not packed here
                     k += 1
                     continue
-                pts = on_dev((pred_i if side == 0 else pred_j)[e], 3)
-                cf = on_dev((conf_i if side == 0 else conf_j)[e], 1)
+                pts, cf = (pred_i[e], conf_i[e]) if side == 0 else (pred_j[e], conf_j[e])
+                if pts is None or cf is None:
+                    raise ValueError(f'entry ({e}, side {side}) of image {img}, an image of this rank, was not given')
+                pts, cf = on_dev(pts, 3), on_dev(cf, 1)
                 assert pts.shape[0] >= areas[img] and cf.shape[0] >= areas[img]
                 table[k] = (pts.data_ptr(), cf.data_ptr(), off, areas[img], ent_coef[k])
                 off += slots[img] * SLOT_PX if stream else areas[img]

@@ -20,7 +20,7 @@ import torch
 from ..post_process import estimate_focal_knowing_depth
 from ..utils.device import to_numpy
 from ..utils.geometry import geotrf, inv
-from . import commons
+from . import commons, owned
 from .commons import compute_edge_scores, edge_str, i_j_ij
 
 
@@ -123,11 +123,14 @@ def dict_to_sparse_graph(dic):
 
 # ------------------------------------------------------------------------------------------------ spanning-tree growth
 def minimum_spanning_tree(imshapes, edges, pred_i, pred_j, conf_i, conf_j, im_conf, min_conf_thr, device,
-                          has_im_poses=True, niter_PnP=10, verbose=True):
-    """Returns (world pointmap per image, tree edges in attachment order, focals, cam2world poses)."""
+                          has_im_poses=True, niter_PnP=10, verbose=True, scores=None):
+    """Returns (world pointmap per image, tree edges in attachment order, focals, cam2world poses).  scores: the
+    {(i, j): score} of compute_edge_scores when already known."""
     n_imgs = len(imshapes)
+    if scores is None:
+        scores = compute_edge_scores(map(i_j_ij, edges), conf_i, conf_j)
     # scipy computes MINIMUM spanning trees: negate the confidences
-    graph = -dict_to_sparse_graph(compute_edge_scores(map(i_j_ij, edges), conf_i, conf_j))
+    graph = -dict_to_sparse_graph(scores)
     tree = sp.csgraph.minimum_spanning_tree(graph).tocoo()
     # best edge on the right; an edge that cannot be attached yet goes back to the left end (lowest priority)
     queue = deque(sorted(zip(-tree.data, tree.row, tree.col)))
@@ -213,11 +216,18 @@ def init_from_pts3d(self, pts3d, im_focals, im_poses):
         for cloud in pts3d:
             cloud[:] = geotrf(to_known, cloud)
 
-    # pairwise similarity of every pair onto the world cloud
+    # pairwise similarity of every pair onto the world cloud; a scene of kept rows registers the edges whose row it keeps
+    # and takes the others' from their keepers
+    partial = owned.shard_of(self) is not None
+    mine = owned.keeps_edge(self) if partial else None
     for e, (i, j) in enumerate(self.edges):
+        if partial and not mine[e]:
+            continue
         key = edge_str(i, j)
         s, R, T = rigid_points_registration(self.pred_i[key], pts3d[i], conf=self.conf_i[key])
         self._set_pose(self.pw_poses, e, R, T, scale=s)
+    if partial and self.pw_poses.requires_grad:
+        owned.share_edge_rows(self, self.pw_poses)
 
     # fix the scale gauge the way the objective does
     gauge = self.get_pw_norm_scale_factor()
@@ -238,9 +248,12 @@ def init_from_pts3d(self, pts3d, im_focals, im_poses):
 
 @torch.no_grad()
 def init_minimum_spanning_tree(self, **kw):
-    pts3d, _, im_focals, im_poses = minimum_spanning_tree(self.imshapes, self.edges, self.pred_i, self.pred_j, self.conf_i,
-                                                          self.conf_j, self.im_conf, self.min_conf_thr, self.device,
-                                                          has_im_poses=self.has_im_poses, verbose=self.verbose, **kw)
+    rows, scores = (self.pred_i, self.pred_j, self.conf_i, self.conf_j), None
+    if owned.shard_of(self) is not None:     # kept rows: scores from their keepers, the rows the walk reads broadcast
+        rows, scores = owned.kept_rows(self), owned.edge_scores(self)
+    pts3d, _, im_focals, im_poses = minimum_spanning_tree(self.imshapes, self.edges, *rows, self.im_conf, self.min_conf_thr,
+                                                          self.device, has_im_poses=self.has_im_poses, verbose=self.verbose,
+                                                          scores=scores, **kw)
     return init_from_pts3d(self, pts3d, im_focals, im_poses)
 
 
@@ -253,8 +266,14 @@ def init_from_known_poses(self, niter_PnP=10, min_conf_thr=3):
     n_focals, _, focals = get_known_focals(self)
     assert n_focals == self.n_imgs
     pps = self.get_principal_points()
+    # a scene of kept rows works on the edges whose row it keeps -- all the edges (i, *) of its own images i -- and takes
+    # the other pairwise poses and depth maps from their keepers
+    partial = owned.shard_of(self) is not None
+    mine = owned.keeps_edge(self) if partial else None
     best = {}        # image -> (score, pair key, scale) of its most confident pair
     for e, (i, j) in enumerate(self.edges):
+        if partial and not mine[e]:
+            continue
         key = edge_str(i, j)
         # second camera of the pair by PnP in the first camera's frame, then both onto the known cameras
         msk = self.conf_i[key] > min(min_conf_thr, self.conf_i[key].min() - 0.1)
@@ -266,5 +285,11 @@ def init_from_known_poses(self, niter_PnP=10, min_conf_thr=3):
             best[i] = (score, key, s)
     for i in range(self.n_imgs):
         assert known_msk[i]
+        if partial and not owned.owns_image(self, i):
+            continue
         _, key, s = best[i]
         self._set_depthmap(i, self.pred_i[key][:, :, 2] * s)
+    if partial:
+        if self.pw_poses.requires_grad:
+            owned.share_edge_rows(self, self.pw_poses)
+        owned.share_image_rows(self)
