@@ -90,6 +90,14 @@ def _declare(lib):
     lib.d3r_segment_sky_workspace_bytes.argtypes = [i32, i64]
     lib.d3r_segment_sky.restype = C.c_int
     lib.d3r_segment_sky.argtypes = [i32, vp, vp, i32, i64, vp, vp, vp, i64, vp]
+    lib.d3r_nanmedian_workspace_bytes.restype = i64
+    lib.d3r_nanmedian_workspace_bytes.argtypes = [i32]
+    lib.d3r_segmented_nanmedian.restype = C.c_int
+    lib.d3r_segmented_nanmedian.argtypes = [i32, i64, vp, vp, vp, i64, vp]
+    lib.d3r_criterion_workspace_bytes.restype = i64
+    lib.d3r_criterion_workspace_bytes.argtypes = [i32, i64, i64, i32]
+    lib.d3r_criterion.restype = C.c_int
+    lib.d3r_criterion.argtypes = [i32, i64, i64, i32, i32, f32, f32] + [vp] * 15 + [i64, vp]
     for name in ('d3r_sizeof_align_item', 'd3r_sizeof_pack_entry', 'd3r_align_stream_slots_per_item',
                  'd3r_align_stream_warps_per_cta', 'd3r_align_stream_max_window'):
         getattr(lib, name).restype = C.c_int

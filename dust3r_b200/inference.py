@@ -15,6 +15,7 @@ import torch
 import tqdm
 
 from .utils.device import to_cpu, collate_with_cat
+from .utils.geometry import geotrf
 
 
 def _interleave_imgs(img1, img2):
@@ -37,8 +38,30 @@ def make_batch_symmetric(batch):
 _IGNORE = {'depthmap', 'dataset', 'label', 'instance', 'idx', 'true_shape', 'rng'}
 
 
+def get_pred_pts3d(gt, pred, use_pose=False):
+    """inference.py:81-103: the predicted points of a view -- pred['pts3d'] (moved by pred['camera_pose'] when use_pose), or
+    pred['pts3d_in_other_view'] as it is (use_pose must then be set).  DUSt3R's heads never predict the depth / pseudo-focal
+    pair the reference also accepts, so that form raises."""
+    if 'depth' in pred and 'pseudo_focal' in pred:
+        raise NotImplementedError('predictions given as depth + pseudo_focal are not supported: DUSt3R heads return pts3d')
+    if 'pts3d' in pred:
+        pts3d = pred['pts3d']
+    elif 'pts3d_in_other_view' in pred:
+        assert use_pose is True
+        return pred['pts3d_in_other_view']
+    else:
+        raise KeyError('the prediction has neither pts3d nor pts3d_in_other_view')
+    if use_pose:
+        camera_pose = pred.get('camera_pose')
+        assert camera_pose is not None
+        pts3d = geotrf(camera_pose, pts3d)
+    return pts3d
+
+
 def loss_of_one_batch(batch, model, criterion, device, symmetrize_batch=False, use_amp=False, ret=None):
-    """inference.py:32-52.  `criterion` must be None (training losses are outside the hot paths)."""
+    """inference.py:32-52: moves the batch to `device`, optionally symmetrises it, runs the model and, when a criterion is
+    given (dust3r_b200.losses), evaluates criterion(view1, view2, pred1, pred2) -> (loss, details) on the predictions.
+    `use_amp` is accepted for the reference's signature; the forward's precision is fixed by the model."""
     view1, view2 = batch
     for view in batch:
         for name in view.keys():
@@ -47,10 +70,9 @@ def loss_of_one_batch(batch, model, criterion, device, symmetrize_batch=False, u
             view[name] = view[name].to(device, non_blocking=True)
     if symmetrize_batch:
         view1, view2 = make_batch_symmetric(batch)
-    if criterion is not None:
-        raise NotImplementedError('training criteria are not part of the inference hot path')
     pred1, pred2 = model(view1, view2)
-    result = dict(view1=view1, view2=view2, pred1=pred1, pred2=pred2, loss=None)
+    loss = criterion(view1, view2, pred1, pred2) if criterion is not None else None
+    result = dict(view1=view1, view2=view2, pred1=pred1, pred2=pred2, loss=loss)
     return result[ret] if ret else result
 
 

@@ -134,3 +134,67 @@ def find_reciprocal_matches(P1, P2):
     mutual_2 = to_p2[to_p1] == np.arange(len(to_p1))
     assert (to_p1[to_p2] == np.arange(len(to_p2))).sum() == mutual_2.sum()     # the relation is symmetric
     return mutual_2, to_p1, mutual_2.sum()
+
+
+NORM_MODES = ('avg_dis',)
+_REFERENCE_NORM_MODES = ('avg_log1p', 'avg_warp-log1p', 'median_dis', 'sqrt_dis')
+
+
+def check_norm_mode(norm_mode):
+    """A falsy mode (no normalisation) or one of NORM_MODES; the reference's other modes raise NotImplementedError."""
+    if not norm_mode or norm_mode in NORM_MODES:
+        return
+    known = norm_mode in _REFERENCE_NORM_MODES
+    raise (NotImplementedError if known else ValueError)(
+        f'norm_mode={norm_mode!r} is {"not supported" if known else "unknown"}: supported modes are {NORM_MODES} or a falsy value')
+
+
+def normalize_pointcloud(pts1, pts2, norm_mode='avg_dis', valid1=None, valid2=None, ret_factor=False):
+    """dust3r/utils/geometry.py:249-308 for norm_mode 'avg_dis': both pointmaps (B,H,W,3) divided by the mean distance to the
+    origin of the valid points of the two together (per batch item, clipped below at 1e-8).  Invalid points do not enter the
+    mean, whatever they hold."""
+    from .misc import invalid_to_zeros
+    check_norm_mode(norm_mode)
+    assert pts1.ndim >= 3 and pts1.shape[-1] == 3
+    assert pts2 is None or (pts2.ndim >= 3 and pts2.shape[-1] == 3)
+    z1, nnz1 = invalid_to_zeros(pts1, valid1, ndim=3)
+    z2, nnz2 = invalid_to_zeros(pts2, valid2, ndim=3) if pts2 is not None else (None, 0)
+    allp = torch.cat((z1, z2), dim=1) if pts2 is not None else z1
+    factor = allp.norm(dim=-1).sum(dim=1) / (nnz1 + nnz2 + 1e-8)
+    factor = factor.clip(min=1e-8)
+    while factor.ndim < pts1.ndim:
+        factor = factor.unsqueeze(-1)
+    res = pts1 / factor
+    if pts2 is not None:
+        res = (res, pts2 / factor)
+    if ret_factor:
+        res = res + (factor,)
+    return res
+
+
+@torch.no_grad()
+def get_joint_pointcloud_depth(z1, z2, valid_mask1, valid_mask2=None, quantile=0.5):
+    """dust3r/utils/geometry.py:311-324: per batch item, the median (torch.nanmedian: the lower one) of the valid depths of
+    both maps together; NaN for an item without any."""
+    from .misc import invalid_to_nans
+    zz = invalid_to_nans(z1, valid_mask1).reshape(len(z1), -1)
+    if z2 is not None:
+        zz = torch.cat((zz, invalid_to_nans(z2, valid_mask2).reshape(len(z2), -1)), dim=-1)
+    if quantile == 0.5:
+        return torch.nanmedian(zz, dim=-1).values
+    return torch.nanquantile(zz, quantile, dim=-1)
+
+
+@torch.no_grad()
+def get_joint_pointcloud_center_scale(pts1, pts2, valid_mask1=None, valid_mask2=None, z_only=False, center=True):
+    """dust3r/utils/geometry.py:327-342: per batch item, the per-coordinate median of the valid points of both maps (B,1,1,3)
+    and the median distance of those points to it (B,1,1,1)."""
+    from .misc import invalid_to_nans
+    pp = invalid_to_nans(pts1, valid_mask1).reshape(len(pts1), -1, 3)
+    if pts2 is not None:
+        pp = torch.cat((pp, invalid_to_nans(pts2, valid_mask2).reshape(len(pts2), -1, 3)), dim=1)
+    c = torch.nanmedian(pp, dim=1, keepdim=True).values
+    if z_only:
+        c[..., :2] = 0
+    scale = torch.nanmedian(((pp - c) if center else pp).norm(dim=-1), dim=1).values
+    return c[:, None, :, :], scale[:, None, None, None]

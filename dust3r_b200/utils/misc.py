@@ -53,3 +53,29 @@ def interleave(x, y):
     a[0::2], a[1::2] = x, y
     b[0::2], b[1::2] = y, x
     return a, b
+
+
+def invalid_to_nans(arr, valid_mask, ndim=999):
+    """dust3r/utils/misc.py:103-109: a copy of `arr` with NaN where `valid_mask` is false (`arr` itself when the mask is None),
+    its trailing spatial dimensions flattened so that it has at most `ndim` dimensions.  A uint8 mask counts as nonzero = valid."""
+    if valid_mask is not None:
+        arr = arr.clone()
+        arr[~valid_mask.bool()] = float('nan')
+    if arr.ndim > ndim:
+        arr = arr.flatten(-2 - (arr.ndim - ndim), -2)
+    return arr
+
+
+def invalid_to_zeros(arr, valid_mask, ndim=999):
+    """dust3r/utils/misc.py:112-121: (copy of `arr` with 0 where `valid_mask` is false, number of valid entries per batch item);
+    without a mask, `arr` itself and the number of entries per item.  Trailing spatial dimensions flattened as invalid_to_nans."""
+    if valid_mask is not None:
+        valid_mask = valid_mask.bool()
+        arr = arr.clone()
+        arr[~valid_mask] = 0
+        nnz = valid_mask.view(len(valid_mask), -1).sum(1)
+    else:
+        nnz = arr.numel() // len(arr) if len(arr) else 0
+    if arr.ndim > ndim:
+        arr = arr.flatten(-2 - (arr.ndim - ndim), -2)
+    return arr, nnz

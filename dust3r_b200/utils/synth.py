@@ -191,3 +191,61 @@ def synth_photo(H: int, W: int, seed: int = 0):
         img[y0:y1, x0:x1] = torch.randint(0, 2, (3,), generator=g).to(torch.float32) * 255
     img = img + torch.randn((H, W, 3), generator=g) * 12
     return img.clamp(0, 255).to(torch.uint8).numpy()
+
+
+def synth_criterion_batch(B: int, hw1, hw2, seed: int = 0, invalid: float = 0.2, garbage: bool = True, empty_view2: bool = False,
+                          noise: float = 0.02):
+    """Ground truth and predictions for the evaluation criteria (dust3r_b200.losses): B pairs of views of sizes hw1 and hw2.
+    Per pair, two cameras on a small arc look at smooth random depth maps; the views carry the world points 'pts3d', a
+    'valid_mask' (a random `invalid` share of the pixels and a rectangular hole are invalid; all of view 2 with empty_view2)
+    and the 'camera_pose' (camera to world).  The predictions are the exact points in camera 1's frame at a random scale per
+    pair plus noise, with confidences in [1, 5].  With garbage, invalid ground truth holds NaN, +-Inf and 1e30, which must not
+    reach any result.  Returns (gt1, gt2, pred1, pred2), CPU fp32."""
+    g = _gen(seed, f'criterion{B}:{tuple(hw1)}:{tuple(hw2)}')
+
+    def cam_points(H, W):
+        f = 1.2 * max(H, W)
+        vs, us = torch.meshgrid(torch.arange(H, dtype=torch.float32), torch.arange(W, dtype=torch.float32), indexing='ij')
+        depth = 2.0 + torch.nn.functional.interpolate(torch.rand((1, 1, 4, 4), generator=g), size=(H, W), mode='bicubic',
+                                                      align_corners=True)[0, 0]
+        return torch.stack(((us - W / 2) * depth / f, (vs - H / 2) * depth / f, depth), dim=-1)
+
+    def pose(ang, t):
+        c2w = torch.eye(4)
+        c2w[:3, :3] = torch.tensor([[math.cos(ang), 0, math.sin(ang)], [0, 1, 0], [-math.sin(ang), 0, math.cos(ang)]])
+        c2w[:3, 3] = torch.tensor(t)
+        return c2w
+
+    def mask(H, W):
+        m = torch.rand((H, W), generator=g) >= invalid
+        y0, x0 = int(torch.randint(0, H // 2, (1,), generator=g)), int(torch.randint(0, W // 2, (1,), generator=g))
+        m[y0:y0 + H // 4, x0:x0 + W // 4] = False
+        return m
+
+    views = ([], [], [], [], [], [], [], [])   # gt1, gt2, valid1, valid2, pose1, pose2, pred1, pred2
+    for b in range(B):
+        ang = 0.3 * float(torch.rand((), generator=g)) - 0.15
+        c1 = pose(ang, [0.1 * b, 0.0, 0.0])
+        c2 = pose(ang + 0.25, [0.1 * b + 0.6, 0.05, 0.1])
+        p1, p2 = cam_points(*hw1), cam_points(*hw2)
+        w1 = p1 @ c1[:3, :3].T + c1[:3, 3]
+        w2 = p2 @ c2[:3, :3].T + c2[:3, 3]
+        w2c1 = torch.linalg.inv(c1)
+        p2_in_1 = w2 @ w2c1[:3, :3].T + w2c1[:3, 3]
+        s = 0.5 + 1.5 * float(torch.rand((), generator=g))
+        for k, v in enumerate((w1, w2, mask(*hw1), mask(*hw2), c1, c2,
+                               s * p1 + noise * torch.randn(p1.shape, generator=g),
+                               s * p2_in_1 + noise * torch.randn(p2.shape, generator=g))):
+            views[k].append(v)
+    gt1, gt2, v1, v2, pose1, pose2, pr1, pr2 = (torch.stack(v) for v in views)
+    if empty_view2:
+        v2[:] = False
+    if garbage:
+        junk = torch.tensor([float('nan'), float('inf'), -float('inf'), 1e30])
+        for gt, v in ((gt1, v1), (gt2, v2)):
+            bad = (~v).nonzero()
+            gt[bad[:, 0], bad[:, 1], bad[:, 2]] = junk[torch.arange(len(bad)) % 4, None]
+    conf1 = 1 + 4 * torch.rand(v1.shape, generator=g)
+    conf2 = 1 + 4 * torch.rand(v2.shape, generator=g)
+    return (dict(pts3d=gt1, valid_mask=v1, camera_pose=pose1), dict(pts3d=gt2, valid_mask=v2, camera_pose=pose2),
+            dict(pts3d=pr1, conf=conf1), dict(pts3d_in_other_view=pr2, conf=conf2))

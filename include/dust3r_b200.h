@@ -379,6 +379,33 @@ int64_t d3r_segment_sky_workspace_bytes(int32_t n_imgs, int64_t total_px);
 int d3r_segment_sky(int32_t n_imgs, const int32_t* hw_dev, const int64_t* off_dev, int32_t max_area, int64_t total_px,
                     const uint8_t* rgb_dev, uint8_t* sky_out_dev, void* workspace_dev, int64_t workspace_bytes, void* stream);
 
+/* Segmented lower nanmedian (torch.nanmedian(vals, dim=-1).values): vals [n_seg][seg_len] fp32 -> out [n_seg], element
+ * (n - 1) / 2 of the sorted non-NaN values of each row, NaN for a row with none.  Radix select on order-preserving uint32 keys
+ * (8-bit digits, most significant first): one memset and 4 x (histogram, select) launches whatever the content; -0 sorts below
+ * +0.  n_seg <= 65535, seg_len < 2^32.  Workspace: d3r_nanmedian_workspace_bytes(n_seg) bytes, no initialisation. */
+int64_t d3r_nanmedian_workspace_bytes(int32_t n_seg);
+int d3r_segmented_nanmedian(int32_t n_seg, int64_t seg_len, const float* vals_dev, float* out_dev, void* workspace_dev,
+                            int64_t workspace_bytes, void* stream);
+/* The evaluation criteria of dust3r/losses.py (Regr3D, Regr3D_ShiftInv / _ScaleInv / _ScaleShiftInv with L21, ConfLoss) for B
+ * pairs of views of n1 and n2 pixels, inference-only (no gradient):
+ *   T [B][16] inv(camera_pose of view 1) row-major; gt1/gt2 [B][n][3] ground-truth points in world coordinates (anything at
+ *   invalid pixels); valid1/valid2 [B][n] uint8 (nonzero = valid); pr1 / pr2 [B][n][3] predicted pts3d of view 1 and
+ *   pts3d_in_other_view of view 2; conf1 / conf2 [B][n] (flag 16 only).
+ *   flags: 1 'avg_dis' normalisation, 2 gt_scale, 4 shift-invariant (joint median depth), 8 scale-invariant (median centre and
+ *   scale), 16 ConfLoss weighting with `alpha`, 32 dist_clip.  reduction: 0 mean, 1 sum, 2 none.
+ *   out [7] fp32: the two views' distance (mean, 0 for an empty view | sum | with reduction 2 the mean, NaN for an empty view),
+ *   the two views' confidence loss (mean, 0 for an empty view), the criterion's value (Regr3D: view 1 + view 2, ConfLoss: the two
+ *   confidence losses; NaN with reduction 2), then the two valid counts as int32 bits.  With reduction 2, pix1 / pix2 (B * n
+ *   floats each, or NULL) receive the distances of the valid pixels compacted in row-major (b, pixel) order and mask1 / mask2
+ *   (B * n bytes each, or NULL) the valid mask.  fp64 sums reduced in a fixed order: two calls give the same bits.
+ *   B * (n1 + n2) < 2^31, B <= 10922.  Workspace: d3r_criterion_workspace_bytes(B, n1, n2, flags) bytes, no initialisation. */
+int64_t d3r_criterion_workspace_bytes(int32_t B, int64_t n1, int64_t n2, int32_t flags);
+int d3r_criterion(int32_t B, int64_t n1, int64_t n2, int32_t flags, int32_t reduction, float dist_clip, float alpha,
+                  const float* T_dev, const float* gt1_dev, const float* gt2_dev, const uint8_t* valid1_dev, const uint8_t* valid2_dev,
+                  const float* pr1_dev, const float* pr2_dev, const float* conf1_dev, const float* conf2_dev, float* out_dev,
+                  float* pix1_dev, float* pix2_dev, uint8_t* mask1_dev, uint8_t* mask2_dev, void* workspace_dev,
+                  int64_t workspace_bytes, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Path 1 — pairwise forward: replaces AsymmetricCroCo3DStereo.forward (dust3r/model.py:199-211 =
  * _encode_symmetrized :153-170, _decoder :172-191, downstream heads :193-208) as an encode call and a
