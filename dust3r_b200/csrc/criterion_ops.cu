@@ -431,6 +431,7 @@ __global__ void __launch_bounds__(kThreads) final_kernel(Args a, const double* _
   }
 }
 
+// tests/test_criterion_float64_gpu.py reads P back: the first kFields * B floats of the workspace, in enum Field order
 struct Layout {
   long long P, part_prep, part_loss, off, cols, med, bytes;
   int ncols;
