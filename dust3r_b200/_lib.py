@@ -8,6 +8,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+from ._lib_fwd import Model
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, 'libdust3r_b200.so')
 
@@ -39,69 +41,76 @@ class AlignDesc(C.Structure):
     ]
 
 
-def _declare(lib):
-    vp, i32, i64, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_float
-    lib.d3r_last_error.restype = C.c_char_p
-    lib.d3r_last_error.argtypes = []
-    lib.d3r_abi_version.restype = C.c_int
-    lib.d3r_check_device.restype = C.c_int
-    lib.d3r_align_chunk_pixels.restype = C.c_int
-    lib.d3r_launch_count.restype = C.c_longlong
-    lib.d3r_launch_count_reset.restype = None
-    lib.d3r_prof_enable.restype = None
-    lib.d3r_prof_enable.argtypes = [C.c_int]
-    lib.d3r_prof_report.restype = C.c_int
-    lib.d3r_prof_report.argtypes = [C.c_char_p, C.c_int]
-    lib.d3r_prof_dump.restype = C.c_int
-    lib.d3r_prof_dump.argtypes = [C.c_char_p, C.c_int]
-    lib.d3r_sizeof_align_desc.restype = C.c_int
-    lib.d3r_align_workspace_floats.restype = i64
-    lib.d3r_align_workspace_floats.argtypes = [i32, i32]
-    for name in ('d3r_align_prepare',):
-        getattr(lib, name).restype = C.c_int
-        getattr(lib, name).argtypes = [C.POINTER(AlignDesc), vp]
-    lib.d3r_align_run.restype = C.c_int
-    lib.d3r_align_run.argtypes = [C.POINTER(AlignDesc), i32, i32, vp]
-    for name in ('d3r_align_pixel_pass', 'd3r_align_small_step'):
-        getattr(lib, name).restype = C.c_int
-        getattr(lib, name).argtypes = [C.POINTER(AlignDesc), i32, vp]
-    lib.d3r_align_reduce_block.restype = C.c_int
-    lib.d3r_align_reduce_block.argtypes = [i32, i32, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]
-    lib.d3r_align_loss_grad.restype = C.c_int
-    lib.d3r_align_loss_grad.argtypes = [C.POINTER(AlignDesc), vp, vp, vp, vp]
-    lib.d3r_align_overflow_flag.restype = C.c_int
-    lib.d3r_align_overflow_flag.argtypes = [C.POINTER(AlignDesc), C.POINTER(C.c_int32), vp]
-    lib.d3r_align_pts3d.restype = C.c_int
-    lib.d3r_align_pts3d.argtypes = [C.POINTER(AlignDesc), vp, vp]
-    lib.d3r_align_pack_entries.restype = C.c_int
-    lib.d3r_align_pack_entries.argtypes = [vp, i32, i32, i32, i32, vp, vp]
-    lib.d3r_clean_pointcloud.restype = C.c_int
-    lib.d3r_clean_pointcloud.argtypes = [i32, vp, vp, i32, vp, vp, vp, vp, vp, f32, f32, vp]
-    lib.d3r_procrustes_moments.restype = C.c_int
-    lib.d3r_procrustes_moments.argtypes = [i32, i32, vp, vp, vp, vp, vp]
-    lib.d3r_weiszfeld_focal.restype = C.c_int
-    lib.d3r_weiszfeld_focal.argtypes = [i32, i32, i32, vp, vp, i32, vp, vp]
-    lib.d3r_nearest_neighbours.restype = C.c_int
-    lib.d3r_nearest_neighbours.argtypes = [i32, i32, vp, vp, vp, vp]
-    lib.d3r_image_resize_crop_normalize.restype = C.c_int
-    lib.d3r_image_resize_crop_normalize.argtypes = [vp, i32, i32, i32, i32, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32,
-                                                    vp, vp, vp, vp]
-    lib.d3r_segment_sky_workspace_bytes.restype = i64
-    lib.d3r_segment_sky_workspace_bytes.argtypes = [i32, i64]
-    lib.d3r_segment_sky.restype = C.c_int
-    lib.d3r_segment_sky.argtypes = [i32, vp, vp, i32, i64, vp, vp, vp, i64, vp]
-    lib.d3r_nanmedian_workspace_bytes.restype = i64
-    lib.d3r_nanmedian_workspace_bytes.argtypes = [i32]
-    lib.d3r_segmented_nanmedian.restype = C.c_int
-    lib.d3r_segmented_nanmedian.argtypes = [i32, i64, vp, vp, vp, i64, vp]
-    lib.d3r_criterion_workspace_bytes.restype = i64
-    lib.d3r_criterion_workspace_bytes.argtypes = [i32, i64, i64, i32]
-    lib.d3r_criterion.restype = C.c_int
-    lib.d3r_criterion.argtypes = [i32, i64, i64, i32, i32, f32, f32] + [vp] * 15 + [i64, vp]
-    for name in ('d3r_sizeof_align_item', 'd3r_sizeof_pack_entry', 'd3r_align_stream_slots_per_item',
-                 'd3r_align_stream_warps_per_cta', 'd3r_align_stream_max_window'):
-        getattr(lib, name).restype = C.c_int
-        getattr(lib, name).argtypes = []
+vp, i32, i64, u32, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_float
+_DESC, _MODEL = C.POINTER(AlignDesc), C.POINTER(Model)
+
+# restype, argtypes of every function include/dust3r_b200.h declares, in its order (tests/test_c_abi.py checks the two agree).
+PROTOTYPES = {
+    'd3r_last_error': (C.c_char_p, []),
+    'd3r_abi_version': (i32, []),
+    'd3r_check_device': (i32, []),
+    'd3r_launch_count': (i64, []),
+    'd3r_launch_count_reset': (None, []),
+    'd3r_prof_enable': (None, [i32]),
+    'd3r_prof_report': (i32, [C.c_char_p, i32]),
+    'd3r_prof_dump': (i32, [C.c_char_p, i32]),
+    # global alignment
+    'd3r_sizeof_align_desc': (i32, []),
+    'd3r_sizeof_align_item': (i32, []),
+    'd3r_align_chunk_pixels': (i32, []),
+    'd3r_align_workspace_floats': (i64, [i32, i32]),
+    'd3r_align_prepare': (i32, [_DESC, vp]),
+    'd3r_align_run': (i32, [_DESC, i32, i32, vp]),
+    'd3r_align_pixel_pass': (i32, [_DESC, i32, vp]),
+    'd3r_align_small_step': (i32, [_DESC, i32, vp]),
+    'd3r_align_reduce_block': (i32, [i32, i32, C.POINTER(i64), C.POINTER(i64)]),
+    'd3r_align_loss_grad': (i32, [_DESC, vp, vp, vp, vp]),
+    'd3r_align_overflow_flag': (i32, [_DESC, C.POINTER(i32), vp]),
+    'd3r_align_pts3d': (i32, [_DESC, vp, vp]),
+    'd3r_align_set_debug': (i32, [vp]),
+    'd3r_sizeof_pack_entry': (i32, []),
+    'd3r_align_stream_slots_per_item': (i32, []),
+    'd3r_align_stream_warps_per_cta': (i32, []),
+    'd3r_align_stream_max_window': (i32, []),
+    'd3r_align_pack_entries': (i32, [vp, i32, i32, i32, i32, vp, vp]),
+    # forward building blocks
+    'd3r_gemm_bf16': (i32, [vp, vp, vp, vp, vp, vp, i32, i32, i32, i64, u32, vp, vp, i32, i32, i32, vp]),
+    'd3r_conv3x3_bf16': (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, u32, vp]),
+    'd3r_attention_hd64': (i32, [vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, i32, i32, f32, vp]),
+    'd3r_conv_transpose_bf16': (i32, [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]),
+    'd3r_conv3x3_head_tail': (i32, [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, f32, vp]),
+    'd3r_layernorm_bf16': (i32, [vp, vp, vp, vp, i32, i32, f32, vp]),
+    'd3r_upsample2x_bf16': (i32, [vp, vp, i32, i32, i32, i32, i32, i32, vp]),
+    'd3r_im2col_3x3_s2_bf16': (i32, [vp, vp, i32, i32, i32, i32, vp]),
+    'd3r_patch_im2col16': (i32, [vp, vp, i32, i32, i32, vp]),
+    'd3r_linear_head_postprocess': (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp]),
+    'd3r_set_gemm_impl': (None, [i32]),
+    'd3r_set_gemm_pair_min_kblocks': (None, [i32]),
+    'd3r_set_gemm_store': (None, [i32]),
+    'd3r_set_conv_store': (None, [i32]),
+    'd3r_set_attention_impl': (None, [i32]),
+    # scene-level operators
+    'd3r_clean_pointcloud': (i32, [i32, vp, vp, i32, vp, vp, vp, vp, vp, f32, f32, vp]),
+    'd3r_procrustes_moments': (i32, [i32, i32, vp, vp, vp, vp, vp]),
+    'd3r_weiszfeld_focal': (i32, [i32, i32, i32, vp, vp, i32, vp, vp]),
+    'd3r_nearest_neighbours': (i32, [i32, i32, vp, vp, vp, vp]),
+    'd3r_image_resize_crop_normalize': (i32, [vp, i32, i32, i32, i32, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32,
+                                              vp, vp, vp, vp]),
+    'd3r_segment_sky_workspace_bytes': (i64, [i32, i64]),
+    'd3r_segment_sky': (i32, [i32, vp, vp, i32, i64, vp, vp, vp, i64, vp]),
+    'd3r_nanmedian_workspace_bytes': (i64, [i32]),
+    'd3r_segmented_nanmedian': (i32, [i32, i64, vp, vp, vp, i64, vp]),
+    'd3r_criterion_workspace_bytes': (i64, [i32, i64, i64, i32]),
+    'd3r_criterion': (i32, [i32, i64, i64, i32, i32, f32, f32] + [vp] * 15 + [i64, vp]),
+    # pairwise forward
+    'd3r_sizeof_model': (i32, []),
+    'd3r_encode_workspace_bytes': (i64, [_MODEL, i32, i32, i32]),
+    'd3r_encode_images': (i32, [_MODEL, vp, i32, i32, i32, vp, vp, i64, vp]),
+    'd3r_decode_workspace_bytes': (i64, [_MODEL, i32, i32, i32, i32, i32]),
+    'd3r_decode_pairs': (i32, [_MODEL, vp, i32, i32, i32, vp, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), i32,
+                               vp, vp, vp, vp, vp, i64, vp]),
+    'd3r_forward_set_debug': (i32, [i32, vp, i64]),
+}
 
 
 def lib_available() -> bool:
@@ -116,9 +125,9 @@ def get_lib():
             raise D3RError(f'{LIB_PATH} not found: the CUDA extension is required (no CPU/torch fallback). '
                            f'Build it with `python -m dust3r_b200.build`.')
         lib = C.CDLL(LIB_PATH)
-        _declare(lib)
-        from . import _lib_fwd  # forward-path prototypes live next to their host code
-        _lib_fwd.declare(lib)
+        for name, (restype, argtypes) in PROTOTYPES.items():
+            fn = getattr(lib, name)
+            fn.restype, fn.argtypes = restype, argtypes
         _lib = lib
     return _lib
 
@@ -140,6 +149,15 @@ def require_cuda_device(device):
     with torch.cuda.device(dev):
         check(get_lib().d3r_check_device())
     return dev
+
+
+def launch(device, name, *args):
+    """Calls the entry point `name` with `args` and the current stream of `device`, with `device` current, and raises
+    D3RError when it fails.  The stream is `device`'s, never the current device's: a scene on cuda:1 runs while cuda:0 is
+    current."""
+    import torch
+    with torch.cuda.device(device):
+        check(getattr(get_lib(), name)(*args, C.c_void_p(torch.cuda.current_stream(device).cuda_stream)))
 
 
 def stream_ptr():

@@ -1,4 +1,5 @@
-"""ctypes mirror of the forward-path part of include/dust3r_b200.h ("Path 1")."""
+"""ctypes mirror of the forward-path structures and epilogue flags of include/dust3r_b200.h ("Path 1"); the prototypes are
+in _lib.PROTOTYPES."""
 import ctypes as C
 
 F_BIAS, F_GELU, F_RELU, F_OUT_F32, F_RESID_INPLACE = 1, 2, 4, 8, 16
@@ -45,46 +46,3 @@ class Model(C.Structure):
                 ('dec1', C.POINTER(DecBlock)), ('dec2', C.POINTER(DecBlock)), ('dec_norm', Norm),
                 ('dpt', C.POINTER(DptHead) * 2), ('lin_head', Linear * 2)]
 
-
-def declare(lib):
-    vp, i32, i64, u32, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_float
-    lib.d3r_gemm_bf16.restype = C.c_int
-    lib.d3r_gemm_bf16.argtypes = [vp, vp, vp, vp, vp, vp, i32, i32, i32, i64, u32, vp, vp, i32, i32, i32, vp]
-    lib.d3r_conv3x3_bf16.restype = C.c_int
-    lib.d3r_conv3x3_bf16.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, u32, vp]
-    lib.d3r_attention_hd64.restype = C.c_int
-    lib.d3r_attention_hd64.argtypes = [vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, i32, i32, f32, vp]
-    lib.d3r_conv_transpose_bf16.restype = C.c_int
-    lib.d3r_conv_transpose_bf16.argtypes = [vp, vp, vp, vp, i32, i32, i32, i32, i32, i32, vp]
-    lib.d3r_conv3x3_head_tail.restype = C.c_int
-    lib.d3r_conv3x3_head_tail.argtypes = [vp, vp, vp, vp, vp, vp, vp, i32, i32, i32, i32, i32, f32, f32, vp]
-    lib.d3r_layernorm_bf16.restype = C.c_int
-    lib.d3r_layernorm_bf16.argtypes = [vp, vp, vp, vp, i32, i32, f32, vp]
-    lib.d3r_upsample2x_bf16.restype = C.c_int
-    lib.d3r_upsample2x_bf16.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, vp]
-    lib.d3r_im2col_3x3_s2_bf16.restype = C.c_int
-    lib.d3r_im2col_3x3_s2_bf16.argtypes = [vp, vp, i32, i32, i32, i32, vp]
-    lib.d3r_patch_im2col16.restype = C.c_int
-    lib.d3r_patch_im2col16.argtypes = [vp, vp, i32, i32, i32, vp]
-    lib.d3r_linear_head_postprocess.restype = C.c_int
-    lib.d3r_linear_head_postprocess.argtypes = [vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp]
-    lib.d3r_set_gemm_impl.restype = None
-    lib.d3r_set_gemm_impl.argtypes = [i32]
-    lib.d3r_set_gemm_store.restype = None
-    lib.d3r_set_gemm_store.argtypes = [i32]
-    lib.d3r_set_conv_store.restype = None
-    lib.d3r_set_conv_store.argtypes = [i32]
-    lib.d3r_set_attention_impl.restype = None
-    lib.d3r_set_attention_impl.argtypes = [i32]
-    lib.d3r_encode_workspace_bytes.restype = i64
-    lib.d3r_encode_workspace_bytes.argtypes = [C.POINTER(Model), i32, i32, i32]
-    lib.d3r_encode_images.restype = C.c_int
-    lib.d3r_encode_images.argtypes = [C.POINTER(Model), vp, i32, i32, i32, vp, vp, i64, vp]
-    lib.d3r_decode_workspace_bytes.restype = i64
-    lib.d3r_decode_workspace_bytes.argtypes = [C.POINTER(Model), i32, i32, i32, i32, i32]
-    lib.d3r_decode_pairs.restype = C.c_int
-    lib.d3r_decode_pairs.argtypes = [C.POINTER(Model), vp, i32, i32, i32, vp, i32, i32, i32, C.POINTER(i32), C.POINTER(i32), i32,
-                                     vp, vp, vp, vp, vp, i64, vp]
-    lib.d3r_forward_set_debug.restype = C.c_int
-    lib.d3r_forward_set_debug.argtypes = [i32, vp, i64]
-    lib.d3r_sizeof_model.restype = C.c_int

@@ -222,9 +222,8 @@ class AlignEngine:
         k0, k1 = int(ent_ptr[lo]), int(ent_ptr[hi])      # entries of the packed images (all of them unless sharded)
         table_dev = torch.from_numpy(np.ascontiguousarray(table[k0:k1]).view(np.uint8)).to(dev)
         if k1 > k0:
-            with torch.cuda.device(dev):
-                _lib.check(self.lib.d3r_align_pack_entries(table_dev.data_ptr(), k1 - k0, int(max(areas[lo:hi])), _CONF_MODES[conf_mode],
-                                                           1 if stream else 0, self.obs.data_ptr(), self._stream()))
+            _lib.launch(dev, 'd3r_align_pack_entries', table_dev.data_ptr(), k1 - k0, int(max(areas[lo:hi])), _CONF_MODES[conf_mode],
+                        1 if stream else 0, self.obs.data_ptr())
         if keep:
             torch.cuda.current_stream(dev).synchronize()     # the staged copies may be freed after this point
         del keep, table_dev
@@ -252,14 +251,10 @@ class AlignEngine:
         self.norm_pw_scale = True
         self.tied_focal = True
 
-    def _stream(self):
-        """cudaStream_t of the engine's device (never the current device's: global_aligner(out, 'cuda:1') must work
-        while cuda:0 is current)."""
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
     def _call(self, fn, *args):
-        with torch.cuda.device(self.device):
-            _lib.check(fn(*args, self._stream()))
+        """_lib.launch on the engine's device for a caller that holds the library function `fn` itself (an attribute of
+        _lib.get_lib()), e.g. a test that runs a range of iterations with d3r_align_run."""
+        _lib.launch(self.device, fn.__name__, *args)
 
     def _no_items(self):
         self.stream_grid = self.stream_ppt = self.stream_window = self.n_items = 0
@@ -419,7 +414,7 @@ class AlignEngine:
 
     def prepare(self):
         d = self._desc()
-        self._call(self.lib.d3r_align_prepare, C.byref(d))
+        _lib.launch(self.device, 'd3r_align_prepare', C.byref(d))
         self._prepared = True
 
     @staticmethod
@@ -461,7 +456,7 @@ class AlignEngine:
         if not getattr(self, '_prepared', False):
             self.prepare()
         d = self._desc()
-        self._call(self.lib.d3r_align_run, C.byref(d), 0, niter)
+        _lib.launch(self.device, 'd3r_align_run', C.byref(d), 0, niter)
         return self.loss_out
 
     # ------------------------------------------------------------------ sharded iterations
@@ -482,9 +477,9 @@ class AlignEngine:
         """Pixel pass over this rank's items, the exact integer all-reduce of the accumulators, the small step: all three on
         the engine's stream, nothing waits on the host."""
         if self.n_items:
-            self._call(self.lib.d3r_align_pixel_pass, C.byref(d), it)
+            _lib.launch(self.device, 'd3r_align_pixel_pass', C.byref(d), it)
         tdist.all_reduce(self._reduce, op=tdist.ReduceOp.SUM, group=self.group)
-        self._call(self.lib.d3r_align_small_step, C.byref(d), it)
+        _lib.launch(self.device, 'd3r_align_small_step', C.byref(d), it)
 
     def _sync_end(self):
         """Every owner broadcasts its images' log-depths, so that every rank holds the whole scene."""
@@ -496,7 +491,7 @@ class AlignEngine:
         """Raises if a fixed-point accumulator left its range (host sync)."""
         flag = C.c_int32(0)
         d = self._desc()
-        self._call(self.lib.d3r_align_overflow_flag, C.byref(d), C.byref(flag))
+        _lib.launch(self.device, 'd3r_align_overflow_flag', C.byref(d), C.byref(flag))
         if flag.value:
             raise _lib.D3RError('alignment: a gradient sum left the fixed-point accumulator range (partial >= 2^18 or total >= 2^22, or NaN / Inf); '
                                 'rescale the scene (pointmaps are expected in metric-like units)')
@@ -513,7 +508,7 @@ class AlignEngine:
             return self.loss_out[0]
         self.prepare()
         d = self._desc(eval_only=True)
-        self._call(self.lib.d3r_align_run, C.byref(d), 0, 1)
+        _lib.launch(self.device, 'd3r_align_run', C.byref(d), 0, 1)
         return self.loss_out[0]
 
     def loss_and_grad(self, entry_loss=False):
@@ -533,8 +528,8 @@ class AlignEngine:
         self.prepare()
         d = self._desc()
         d.loss_out = loss.data_ptr()
-        self._call(self.lib.d3r_align_loss_grad, C.byref(d), logd_grad.data_ptr(), small_grad.data_ptr(),
-                   ent.data_ptr() if ent is not None else None)
+        _lib.launch(self.device, 'd3r_align_loss_grad', C.byref(d), logd_grad.data_ptr(), small_grad.data_ptr(),
+                    ent.data_ptr() if ent is not None else None)
         return loss, logd_grad, small_grad, ent
 
     def pts3d(self):
@@ -542,5 +537,5 @@ class AlignEngine:
         self.prepare()
         out = torch.zeros((int(self.pix_off[-1]), 3), dtype=torch.float32, device=self.device)
         d = self._desc()
-        self._call(self.lib.d3r_align_pts3d, C.byref(d), out.data_ptr())
+        _lib.launch(self.device, 'd3r_align_pts3d', C.byref(d), out.data_ptr())
         return out

@@ -11,8 +11,6 @@ The host ports dispatch here when their inputs live on the GPU; CPU tensors keep
 reference does: these run once per scene, not per iteration)."""
 from __future__ import annotations
 
-import ctypes as C
-
 import numpy as np
 import torch
 
@@ -23,16 +21,11 @@ def _f32(t):
     return t.to(torch.float32).contiguous()
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-
-
 @torch.no_grad()
 def clean_pointcloud(im_confs, K, cams, depthmaps, all_pts3d, tol=0.001, bad_conf=0):
     """Per-image lists (any mix of image sizes) -> list of new confidence maps, same shapes as im_confs."""
     dev = im_confs[0].device
     _lib.require_cuda_device(dev)
-    lib = _lib.get_lib()
     n = len(im_confs)
     assert n == len(cams) == len(K) == len(depthmaps) == len(all_pts3d)
     assert 0 <= tol < 1
@@ -47,9 +40,8 @@ def clean_pointcloud(im_confs, K, cams, depthmaps, all_pts3d, tol=0.001, bad_con
     Td = _f32(torch.stack([torch.as_tensor(c) for c in cams]).to(dev)).reshape(n, 16)
     hw = torch.tensor(shapes, dtype=torch.int32, device=dev)
     offd = torch.from_numpy(off).to(dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.d3r_clean_pointcloud(n, hw.data_ptr(), offd.data_ptr(), int(max(areas)), pts.data_ptr(), conf.data_ptr(),
-                                            depth.data_ptr(), Kd.data_ptr(), Td.data_ptr(), float(tol), float(bad_conf), _stream(dev)))
+    _lib.launch(dev, 'd3r_clean_pointcloud', n, hw.data_ptr(), offd.data_ptr(), int(max(areas)), pts.data_ptr(), conf.data_ptr(),
+                depth.data_ptr(), Kd.data_ptr(), Td.data_ptr(), float(tol), float(bad_conf))
     return [conf[off[i]:off[i + 1]].reshape(shapes[i]).to(im_confs[i].dtype) for i in range(n)]
 
 
@@ -63,12 +55,10 @@ def rigid_registration(x, y, weights, compute_scaling=True):
         x, y, weights = x[None], y[None], weights[None]
     dev = x.device
     _lib.require_cuda_device(dev)
-    lib = _lib.get_lib()
     B, P = int(x.shape[0]), int(x.shape[1])
     x, y, w = _f32(x), _f32(y), _f32(weights)
     m = torch.empty((B, 17), dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.d3r_procrustes_moments(B, P, x.data_ptr(), y.data_ptr(), w.data_ptr(), m.data_ptr(), _stream(dev)))
+    _lib.launch(dev, 'd3r_procrustes_moments', B, P, x.data_ptr(), y.data_ptr(), w.data_ptr(), m.data_ptr())
     sw = m[:, 0]
     xm, ym = m[:, 1:4] / sw[:, None], m[:, 4:7] / sw[:, None]
     M = m[:, 7:16].reshape(B, 3, 3) - sw[:, None, None] * ym[:, :, None] * xm[:, None, :]      # sum w (y - ym)(x - xm)^T
@@ -93,13 +83,11 @@ def weiszfeld_focal(pts3d, pp, steps=10):
     """pts3d (B,H,W,3) camera-frame pointmaps, pp (B,2) -> (B,) focals (before the caller's clipping)."""
     dev = pts3d.device
     _lib.require_cuda_device(dev)
-    lib = _lib.get_lib()
     B, H, W, _ = pts3d.shape
     p = _f32(pts3d)
     c = _f32(pp.to(dev)).reshape(B, 2)
     out = torch.empty((B,), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.d3r_weiszfeld_focal(int(B), int(H), int(W), p.data_ptr(), c.data_ptr(), int(steps), out.data_ptr(), _stream(dev)))
+    _lib.launch(dev, 'd3r_weiszfeld_focal', int(B), int(H), int(W), p.data_ptr(), c.data_ptr(), int(steps), out.data_ptr())
     return out
 
 
@@ -108,11 +96,9 @@ def nearest_neighbours(queries, points):
     """(N,3), (M,3) CUDA tensors -> (N,) int64 index of the nearest row of `points` for every query."""
     dev = queries.device
     _lib.require_cuda_device(dev)
-    lib = _lib.get_lib()
     q, p = _f32(queries).reshape(-1, 3), _f32(points.to(dev)).reshape(-1, 3)
     nn = torch.empty((q.shape[0],), dtype=torch.int32, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.d3r_nearest_neighbours(int(q.shape[0]), int(p.shape[0]), q.data_ptr(), p.data_ptr(), nn.data_ptr(), _stream(dev)))
+    _lib.launch(dev, 'd3r_nearest_neighbours', int(q.shape[0]), int(p.shape[0]), q.data_ptr(), p.data_ptr(), nn.data_ptr())
     return nn.long()
 
 
@@ -136,9 +122,8 @@ def _segment_sky_u8(rgb, shapes):
     offd = torch.from_numpy(off[:n]).to(dev)
     out = torch.empty((total,), dtype=torch.uint8, device=dev)
     ws = torch.empty((int(lib.d3r_segment_sky_workspace_bytes(n, total)),), dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.d3r_segment_sky(n, hw.data_ptr(), offd.data_ptr(), int(max(areas)), total, rgb.data_ptr(), out.data_ptr(),
-                                       ws.data_ptr(), ws.numel(), _stream(dev)))
+    _lib.launch(dev, 'd3r_segment_sky', n, hw.data_ptr(), offd.data_ptr(), int(max(areas)), total, rgb.data_ptr(), out.data_ptr(),
+                ws.data_ptr(), ws.numel())
     sky = out.view(torch.bool)
     return [sky[off[i]:off[i + 1]].view(shapes[i]) for i in range(n)]
 

@@ -27,7 +27,6 @@ Deviations from the reference, all deliberate:
 from __future__ import annotations
 
 import contextlib
-import ctypes as C
 from copy import copy, deepcopy
 
 import torch
@@ -261,15 +260,12 @@ def _run_cuda(crit, gt1, gt2, pred1, pred2, dist_clip=None, alpha=None):
     out = torch.empty(8, dtype=torch.float32, device=dev)
     pix = [torch.empty(B * n, dtype=torch.float32, device=dev) for n in (n1, n2)] if pixels else [None, None]
     msk = [torch.empty(s, dtype=torch.bool, device=dev) for s in ((B, H1, W1), (B, H2, W2))] if pixels else [None, None]
-    lib = _lib.get_lib()
-    nbytes = int(lib.d3r_criterion_workspace_bytes(B, n1, n2, flags))
+    nbytes = int(_lib.get_lib().d3r_criterion_workspace_bytes(B, n1, n2, flags))
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
     ptr = lambda t: None if t is None else t.data_ptr()
-    with torch.cuda.device(dev):
-        _lib.check(lib.d3r_criterion(B, n1, n2, flags, _REDUCTIONS[red], float(dist_clip or 0.0), float(alpha or 0.0),
-                                     ptr(T), ptr(g1), ptr(g2), ptr(m1), ptr(m2), ptr(p1), ptr(p2), ptr(c1), ptr(c2), ptr(out),
-                                     ptr(pix[0]), ptr(pix[1]), ptr(msk[0]), ptr(msk[1]), ptr(ws), nbytes,
-                                     C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    _lib.launch(dev, 'd3r_criterion', B, n1, n2, flags, _REDUCTIONS[red], float(dist_clip or 0.0), float(alpha or 0.0),
+                ptr(T), ptr(g1), ptr(g2), ptr(m1), ptr(m2), ptr(p1), ptr(p2), ptr(c1), ptr(c2), ptr(out),
+                ptr(pix[0]), ptr(pix[1]), ptr(msk[0]), ptr(msk[1]), ptr(ws), nbytes)
     return out, pix, msk
 
 
@@ -432,10 +428,7 @@ def cuda_nanmedian(x):
     dev = _lib.require_cuda_device(x.device)
     rows = x.reshape(-1, x.shape[-1]).to(torch.float32).contiguous()
     out = torch.empty(rows.shape[0], dtype=torch.float32, device=dev)
-    lib = _lib.get_lib()
-    nbytes = int(lib.d3r_nanmedian_workspace_bytes(rows.shape[0]))
+    nbytes = int(_lib.get_lib().d3r_nanmedian_workspace_bytes(rows.shape[0]))
     ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
-    with torch.cuda.device(dev):
-        _lib.check(lib.d3r_segmented_nanmedian(rows.shape[0], rows.shape[1], rows.data_ptr(), out.data_ptr(), ws.data_ptr(), nbytes,
-                                               C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    _lib.launch(dev, 'd3r_segmented_nanmedian', rows.shape[0], rows.shape[1], rows.data_ptr(), out.data_ptr(), ws.data_ptr(), nbytes)
     return out.reshape(x.shape[:-1])

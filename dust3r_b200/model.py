@@ -484,9 +484,8 @@ class _PackedModel:
         p = self.cfg.patch_size
         ws = self._workspace('encode', self.lib.d3r_encode_workspace_bytes(C.byref(self.cmodel), n, H, W))
         feat = torch.empty((n, H // p, W // p, self.cfg.enc_embed_dim), dtype=torch.bfloat16, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.d3r_encode_images(C.byref(self.cmodel), imgs.data_ptr(), n, H, W, feat.data_ptr(), ws.data_ptr(),
-                                                  ws.numel(), _lib.stream_ptr()))
+        _lib.launch(self.device, 'd3r_encode_images', C.byref(self.cmodel), imgs.data_ptr(), n, H, W, feat.data_ptr(), ws.data_ptr(),
+                    ws.numel())
         return feat
 
     def decode(self, feat1, idx1, feat2, idx2):
@@ -499,9 +498,8 @@ class _PackedModel:
         outs = [r[k].data_ptr() if k in r else None for r in res for k in ('pts3d', 'conf')]
         i1 = (C.c_int32 * B)(*[int(v) for v in idx1])
         i2 = (C.c_int32 * B)(*[int(v) for v in idx2])
-        with torch.cuda.device(self.device):
-            _lib.check(self.lib.d3r_decode_pairs(C.byref(self.cmodel), feat1.data_ptr(), n1, H1, W1, feat2.data_ptr(), n2, H2, W2,
-                                                 i1, i2, B, *outs, ws.data_ptr(), ws.numel(), _lib.stream_ptr()))
+        _lib.launch(self.device, 'd3r_decode_pairs', C.byref(self.cmodel), feat1.data_ptr(), n1, H1, W1, feat2.data_ptr(), n2, H2, W2,
+                    i1, i2, B, *outs, ws.data_ptr(), ws.numel())
         return res
 
     def forward(self, imgs, idx1, idx2, B, H, W, debug=None):

@@ -10,7 +10,6 @@ H100 (`d3r_image_resize_crop_normalize`, csrc/image_ops.cu) -- bit-identical to 
 in HBM and inference() uses it in place."""
 from __future__ import annotations
 
-import ctypes
 import functools
 import math
 import os
@@ -266,10 +265,7 @@ def preprocess_image_u8(pixels, size, square_ok=False, device='cuda', patch_size
     src = src.contiguous().to(dev)
     tmp = torch.empty((plan['rows'], plan['w2'], 3), dtype=torch.uint8, device=dev)
     out = torch.empty((1, 3, plan['h2'], plan['w2']), dtype=torch.float32, device=dev)
-    with torch.cuda.device(dev):
-        st = ctypes.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        _lib.check(_lib.get_lib().d3r_image_resize_crop_normalize(
-            src.data_ptr(), h0, w0, plan['h1'], plan['w1'], xb.data_ptr(), xk.data_ptr(), kx, yb.data_ptr(), yk.data_ptr(), ky,
-            plan['row0'], plan['rows'], plan['left'], plan['upper'], plan['h2'], plan['w2'], lut.data_ptr(), tmp.data_ptr(),
-            out.data_ptr(), st))
+    _lib.launch(dev, 'd3r_image_resize_crop_normalize', src.data_ptr(), h0, w0, plan['h1'], plan['w1'], xb.data_ptr(), xk.data_ptr(), kx,
+                yb.data_ptr(), yk.data_ptr(), ky, plan['row0'], plan['rows'], plan['left'], plan['upper'], plan['h2'], plan['w2'],
+                lut.data_ptr(), tmp.data_ptr(), out.data_ptr())
     return out

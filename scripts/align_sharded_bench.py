@@ -36,6 +36,7 @@ os.environ.setdefault('MASTER_ADDR', '127.0.0.1')
 os.environ.setdefault('MASTER_PORT', '29512')
 dist.init_process_group('nccl', device_id=dev, rank=rank, world_size=world)
 
+from dust3r_b200 import _lib
 from dust3r_b200.cloud_opt import GlobalAlignerMode, global_aligner
 from dust3r_b200.distributed import _AlignShard, shard_images
 from dust3r_b200.utils.synth import synth_pair_predictions
@@ -89,11 +90,11 @@ def split_breakdown(eng, niter):
     for it in range(niter):
         ev[it][0].record()
         if eng.n_items:
-            eng._call(eng.lib.d3r_align_pixel_pass, ctypes.byref(d), it)
+            _lib.launch(eng.device, 'd3r_align_pixel_pass', ctypes.byref(d), it)
         ev[it][1].record()
         dist.all_reduce(eng._reduce, op=dist.ReduceOp.SUM)
         ev[it][2].record()
-        eng._call(eng.lib.d3r_align_small_step, ctypes.byref(d), it)
+        _lib.launch(eng.device, 'd3r_align_small_step', ctypes.byref(d), it)
         ev[it][3].record()
     sync()
     parts = [sum(ev[it][k].elapsed_time(ev[it][k + 1]) for it in range(niter)) / niter for k in range(3)]

@@ -2,7 +2,7 @@
 state prints where the iteration's wall time goes -- PDL wait release, streaming, warp-imbalance tail, ticket,
 small-parameter step phases -- as the per-phase budget DESIGN.md quotes.
 Usage: python scripts/align_stream_timeline.py [n_views=8]"""
-import sys, os, ctypes as C, json
+import sys, os, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
 from dust3r_b200 import _lib
@@ -18,7 +18,6 @@ eng = net._get_engine(); net._engine_push(eng)
 assert eng.kernel == 'stream'
 eng.run(20); torch.cuda.synchronize()
 lib = _lib.get_lib()
-lib.d3r_align_set_debug.argtypes = [C.c_void_p]
 nw = eng.stream_grid * 8
 rows = []
 for rep in range(5):

@@ -9,9 +9,7 @@ lib = _lib.get_lib()
 CASES = [(49152, 4096, 1024, (1, 3, 5)), (49152, 3072, 1024, (1, 3)), (49152, 1024, 1024, (1, 9, 0x11)),
          (24576, 768, 768, (1, 9, 0x11)), (49152, 1024, 4096, (1, 0x11)), (24576, 3072, 768, (1, 3)),
          (24576, 768, 3072, (0x11,)), (24576, 2304, 768, (1,))]
-import ctypes
 MINKB = int(sys.argv[1]) if len(sys.argv) > 1 else 16
-lib.d3r_set_gemm_pair_min_kblocks.argtypes = [ctypes.c_int32]
 lib.d3r_set_gemm_pair_min_kblocks(MINKB)
 for (M, N, K, flagset) in CASES:
     A = torch.randn((M, K), device='cuda').bfloat16(); B = torch.randn((N, K), device='cuda').bfloat16()

@@ -6,7 +6,6 @@ from dust3r_b200 import _lib
 from scripts.forward_quick_bench import timeit
 from bench import build_model, H, W
 lib = _lib.get_lib()
-lib.d3r_set_gemm_pair_min_kblocks.argtypes = [__import__('ctypes').c_int32]
 net, cfg = build_model(torch.device('cuda:0'))
 packed = net.repack()
 B = 32
