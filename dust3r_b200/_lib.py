@@ -85,7 +85,6 @@ PROTOTYPES = {
     'd3r_patch_im2col16': (i32, [vp, vp, i32, i32, i32, vp]),
     'd3r_linear_head_postprocess': (i32, [vp, vp, vp, i32, i32, i32, i32, i32, i32, f32, f32, vp]),
     'd3r_set_gemm_impl': (None, [i32]),
-    'd3r_set_gemm_pair_min_kblocks': (None, [i32]),
     'd3r_set_gemm_store': (None, [i32]),
     'd3r_set_conv_store': (None, [i32]),
     'd3r_set_attention_impl': (None, [i32]),

@@ -59,7 +59,7 @@ int encode_tensor_map(CUtensorMap* m, const void* base, int rank, const cuuint64
 
 extern "C" const char* d3r_last_error(void) { return d3r::g_err; }
 
-extern "C" int d3r_abi_version(void) { return 5; }
+extern "C" int d3r_abi_version(void) { return 6; }
 
 extern "C" int d3r_check_device(void) {
   int dev = 0;

@@ -23,11 +23,11 @@ static int pick_block_n(int N, int mode, uint32_t flags, int conv_m_tiles = 0) {
 }
 
 // 0: 1-CTA kernels, 1: CTA-pair kernels (cluster of two, B tile multicast) whenever BLOCK_N >= 128, 2 (default): pair
-// kernels from g_pair_min_kb k-blocks of 64 on, 1-CTA kernels for the shortest reductions (K = 96 / 192 of the DPT
+// kernels from kPairMinKb k-blocks of 64 on, 1-CTA kernels for the shortest reductions (K = 96 / 192 of the DPT
 // re-assembly), whose time goes to the epilogue rather than to operand traffic.
 static int g_impl = 2;
-static int g_pair_min_kb = 4;
-static bool use_pair(int bn, int num_kb) { return bn >= 128 && (g_impl == 1 || (g_impl == 2 && num_kb >= g_pair_min_kb)); }
+constexpr int kPairMinKb = 4;
+static bool use_pair(int bn, int num_kb) { return bn >= 128 && (g_impl == 1 || (g_impl == 2 && num_kb >= kPairMinKb)); }
 
 // 0: register-store epilogues everywhere (the bit-identical A/B reference), 1 (default): the specialised epilogues on
 // 128x256 tiles stage their output in shared memory and write it by TMA store / TMA reduce-add, when TMA can address it
@@ -276,7 +276,6 @@ int conv3x3_head_tail(const void* x_nhwc, const void* w_packed, const float* bia
 using namespace d3r;
 
 extern "C" void d3r_set_gemm_impl(int32_t impl) { gemm::g_impl = impl; }
-extern "C" void d3r_set_gemm_pair_min_kblocks(int32_t kb) { gemm::g_pair_min_kb = kb; }
 extern "C" void d3r_set_gemm_store(int32_t store) { gemm::g_store = store; }
 extern "C" void d3r_set_conv_store(int32_t store) { gemm::g_conv_store = store; }
 

@@ -307,11 +307,9 @@ int d3r_linear_head_postprocess(const float* feat_dev, float* pts3d_dev, float* 
                                 int32_t nch, int32_t depth_mode, int32_t conf_mode, float conf_min, float conf_max, void* stream);
 
 /* Selects the GEMM / conv kernel family: 0 = 1-CTA kernels, 1 = CTA-pair kernels (a cluster of two CTAs on two
- * M tiles sharing one multicast B tile), 2 (default) = CTA-pair kernels from 4 k-blocks of 64 on (K >= 256), 1-CTA
- * for shorter reductions. */
+ * M tiles sharing one multicast B tile), 2 (default) = CTA-pair kernels from 4 k-blocks of 64 on (K >= 256, a fixed
+ * threshold), 1-CTA for shorter reductions. */
 void d3r_set_gemm_impl(int32_t impl);
-/* Tuning aid for impl 2: minimum number of 64-wide k-blocks for which the CTA-pair kernel is used (default 4). */
-void d3r_set_gemm_pair_min_kblocks(int32_t kblocks);
 /* Selects how the specialised epilogues on 128x256 tiles (bias / GELU / ReLU -> bf16, bias + RoPE -> bf16, fp32 residual
  * update) write their result: 1 (default) = staged in shared memory and written by TMA store, or TMA reduce-add for the
  * residual update, overlapping the next tile's main loop; 0 = every thread stores straight from its accumulator

@@ -6,16 +6,14 @@ ModularPointCloudOptimizer, at --c5-hw pixels) it prints one JSON line each with
   fused_iter_us       CUDA-event time per iteration of compute_global_alignment (tag `align_stream` / `align_iter`)
   forward_backward_ms wall time per `loss = net(); loss.backward()` (host synchronised)
   adam_iter_ms        wall time per iteration of the reference loop body driven by torch.optim.Adam(betas=(0.9, 0.9))
-together with the GPU name and its power limit.
+together with the card line (GPU name, power limit and SM clocks) in `gpu` and the power limit alone in `power_limit`.
 
 Usage:  python scripts/align_grad_bench.py [--iters 50] [--c5-hw 192 256]
 """
 import argparse
 import json
 import os
-import subprocess
 import sys
-import time
 
 import torch
 
@@ -24,27 +22,12 @@ from dust3r_b200 import _lib  # noqa: E402
 from dust3r_b200.cloud_opt import GlobalAlignerMode, global_aligner  # noqa: E402
 from dust3r_b200.cloud_opt.commons import cosine_schedule  # noqa: E402
 from dust3r_b200.utils.synth import synth_pair_predictions  # noqa: E402
-
-
-def gpu_info():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    name, power = (q.stdout.strip().splitlines() or ['?, ?'])[0].split(', ')
-    return name, power
+from common import card, wall_ms  # noqa: E402
 
 
 def per_launch_us(report, tag):
     r = report.get(tag)
     return None if not r else 1e3 * r['ms'] / r['count']
-
-
-def wall_ms(fn, iters):
-    fn()
-    torch.cuda.synchronize()
-    t0 = time.perf_counter()
-    for _ in range(iters):
-        fn()
-    torch.cuda.synchronize()
-    return 1e3 * (time.perf_counter() - t0) / iters
 
 
 def bench(name, n, hw, mode, iters, dev):
@@ -85,7 +68,7 @@ def bench(name, n, hw, mode, iters, dev):
         opt.step()
         it[0] += 1
     res = dict(config=name, n=n, E=len(edges), H=H, W=W, kernel=eng.kernel, grad_launch_us=per_launch_us(rep, 'align_grad'),
-               fused_iter_us=fused, forward_backward_ms=wall_ms(fwd_bwd, iters), adam_iter_ms=wall_ms(adam_iter, iters))
+               fused_iter_us=fused, forward_backward_ms=wall_ms(fwd_bwd, iters, 1), adam_iter_ms=wall_ms(adam_iter, iters, 1))
     del net, eng, opt
     torch.cuda.empty_cache()
     return res
@@ -97,12 +80,12 @@ def main():
     ap.add_argument('--c5-hw', type=int, nargs=2, default=(192, 256))
     a = ap.parse_args()
     dev = torch.device('cuda:0')
-    gpu, power = gpu_info()
+    gpu = card(dev)
     runs = [('config3', 8, (384, 512), GlobalAlignerMode.PointCloudOptimizer),
             ('config5_graph', 50, tuple(a.c5_hw), GlobalAlignerMode.ModularPointCloudOptimizer)]
     for name, n, hw, mode in runs:
         r = bench(name, n, hw, mode, a.iters, dev)
-        r.update(gpu=gpu, power_limit=power)
+        r.update(gpu=gpu, power_limit=gpu.split(', ')[1])
         print(json.dumps(r), flush=True)
 
 

@@ -13,7 +13,6 @@ figures are valid, its times are not.  Random-init weights: the numbers are timi
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -21,42 +20,14 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import torch.distributed as dist
 
-ap = argparse.ArgumentParser()
-ap.add_argument('--niter', type=int, default=300)
-ap.add_argument('--backend', default='nccl', choices=('nccl', 'gloo'))
-ap.add_argument('--batch-size', type=int, default=32)
-ap.add_argument('--out', default=None, help='also write the results to this JSON file')
-args = ap.parse_args()
-
-rank, world, local = int(os.environ.get('RANK', 0)), int(os.environ.get('WORLD_SIZE', 1)), int(os.environ.get('LOCAL_RANK', 0))
-dev = torch.device('cuda', local if args.backend == 'nccl' else 0)
-torch.cuda.set_device(dev)
-os.environ.setdefault('MASTER_ADDR', '127.0.0.1')
-os.environ.setdefault('MASTER_PORT', '29513')
-if args.backend == 'nccl':
-    dist.init_process_group('nccl', device_id=dev, rank=rank, world_size=world)
-else:
-    dist.init_process_group('gloo', rank=rank, world_size=world)
-
 from bench import build_model
+from common import barrier_sync, card
 from dust3r_b200.cloud_opt import GlobalAlignerMode
 from dust3r_b200.distributed import global_aligner_sharded, inference_sharded
 from dust3r_b200.image_pairs import make_pairs
 from dust3r_b200.utils.synth import synth_images
 
 H, W, N = 384, 512, 50
-MODE = GlobalAlignerMode.ModularPointCloudOptimizer
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '-i', str(dev.index), '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm',
-                        '--format=csv,noheader'], capture_output=True, text=True)
-    return q.stdout.strip() or torch.cuda.get_device_name(dev)
-
-
-def sync():
-    torch.cuda.synchronize(dev)
-    dist.barrier()
 
 
 def kept_bytes(out):
@@ -67,50 +38,72 @@ def kept_bytes(out):
     return n
 
 
-net, _ = build_model(dev)
-imgs = synth_images(N, H, W, seed=21)
-pairs = make_pairs(imgs, scene_graph='complete', prefilter=None, symmetrize=False)
-results = []
-for keep in ('all', 'owned'):
-    # warm-up with full batches: the forward's work buffers then count as resident in both legs
-    inference_sharded(pairs[:args.batch_size * world], net, dev, batch_size=args.batch_size, verbose=False, gather_device=dev,
-                      return_images=False, keep=keep)
-    sync()
-    torch.cuda.empty_cache()
-    torch.cuda.reset_peak_memory_stats(dev)
-    resident = torch.cuda.memory_allocated(dev)
-    t0 = time.perf_counter()
-    fwd = inference_sharded(pairs, net, dev, batch_size=args.batch_size, verbose=False, gather_device=dev,
-                            return_images=False, keep=keep)
-    sync()
-    t_fwd = time.perf_counter() - t0
-    torch.manual_seed(0)
-    scene = global_aligner_sharded(fwd, dev, mode=MODE, verbose=False)
-    scene.compute_global_alignment(init=None, niter=5)        # engine build, packing, module loads
-    sync()
-    t1 = time.perf_counter()
-    loss = scene.compute_global_alignment(init=None, niter=args.niter, schedule='cosine', lr=0.01)
-    sync()
-    t_align = time.perf_counter() - t1
-    peak = torch.cuda.max_memory_allocated(dev)
-    mine = dict(rank=rank, kept_bytes=kept_bytes(fwd), peak_bytes=peak, peak_above_resident_bytes=peak - resident,
-                routing_buffers=fwd['owned'].allocated if keep == 'owned' else None)
-    every = [None] * world
-    dist.all_gather_object(every, mine)
-    res = dict(keep=keep, world=world, backend=args.backend, n_views=N, n_pairs=len(pairs), size=f'{W}x{H}', niter=args.niter,
-               forward_and_route_s=round(t_fwd, 3) if args.backend == 'nccl' else 'not measured',
-               align_it_per_s=round(args.niter / t_align, 1) if args.backend == 'nccl' else 'not measured',
-               final_loss=loss, ranks=every, card=card(),
-               note='random-init weights; forward_and_route_s is the forward plus the all-gather (all) or all_to_all (owned)')
-    if rank == 0:
-        print(json.dumps(res), flush=True)
-        results.append(res)
-    del scene, fwd
-    torch.cuda.empty_cache()
-    sync()
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--niter', type=int, default=300)
+    ap.add_argument('--backend', default='nccl', choices=('nccl', 'gloo'))
+    ap.add_argument('--batch-size', type=int, default=32)
+    ap.add_argument('--out', default=None, help='also write the results to this JSON file')
+    args = ap.parse_args()
 
-if rank == 0 and args.out:
-    with open(args.out, 'w') as f:
-        json.dump(results, f, indent=1)
-dist.barrier()
-dist.destroy_process_group()
+    rank, world, local = int(os.environ.get('RANK', 0)), int(os.environ.get('WORLD_SIZE', 1)), int(os.environ.get('LOCAL_RANK', 0))
+    dev = torch.device('cuda', local if args.backend == 'nccl' else 0)
+    torch.cuda.set_device(dev)
+    os.environ.setdefault('MASTER_ADDR', '127.0.0.1')
+    os.environ.setdefault('MASTER_PORT', '29513')
+    if args.backend == 'nccl':
+        dist.init_process_group('nccl', device_id=dev, rank=rank, world_size=world)
+    else:
+        dist.init_process_group('gloo', rank=rank, world_size=world)
+
+    net, _ = build_model(dev)
+    imgs = synth_images(N, H, W, seed=21)
+    pairs = make_pairs(imgs, scene_graph='complete', prefilter=None, symmetrize=False)
+    results = []
+    for keep in ('all', 'owned'):
+        # warm-up with full batches: the forward's work buffers then count as resident in both legs
+        inference_sharded(pairs[:args.batch_size * world], net, dev, batch_size=args.batch_size, verbose=False, gather_device=dev,
+                          return_images=False, keep=keep)
+        barrier_sync()
+        torch.cuda.empty_cache()
+        torch.cuda.reset_peak_memory_stats(dev)
+        resident = torch.cuda.memory_allocated(dev)
+        t0 = time.perf_counter()
+        fwd = inference_sharded(pairs, net, dev, batch_size=args.batch_size, verbose=False, gather_device=dev,
+                                return_images=False, keep=keep)
+        barrier_sync()
+        t_fwd = time.perf_counter() - t0
+        torch.manual_seed(0)
+        scene = global_aligner_sharded(fwd, dev, mode=GlobalAlignerMode.ModularPointCloudOptimizer, verbose=False)
+        scene.compute_global_alignment(init=None, niter=5)        # engine build, packing, module loads
+        barrier_sync()
+        t1 = time.perf_counter()
+        loss = scene.compute_global_alignment(init=None, niter=args.niter, schedule='cosine', lr=0.01)
+        barrier_sync()
+        t_align = time.perf_counter() - t1
+        peak = torch.cuda.max_memory_allocated(dev)
+        mine = dict(rank=rank, kept_bytes=kept_bytes(fwd), peak_bytes=peak, peak_above_resident_bytes=peak - resident,
+                    routing_buffers=fwd['owned'].allocated if keep == 'owned' else None)
+        every = [None] * world
+        dist.all_gather_object(every, mine)
+        res = dict(keep=keep, world=world, backend=args.backend, n_views=N, n_pairs=len(pairs), size=f'{W}x{H}', niter=args.niter,
+                   forward_and_route_s=round(t_fwd, 3) if args.backend == 'nccl' else 'not measured',
+                   align_it_per_s=round(args.niter / t_align, 1) if args.backend == 'nccl' else 'not measured',
+                   final_loss=loss, ranks=every, card=card(dev),
+                   note='random-init weights; forward_and_route_s is the forward plus the all-gather (all) or all_to_all (owned)')
+        if rank == 0:
+            print(json.dumps(res), flush=True)
+            results.append(res)
+        del scene, fwd
+        torch.cuda.empty_cache()
+        barrier_sync()
+
+    if rank == 0 and args.out:
+        with open(args.out, 'w') as f:
+            json.dump(results, f, indent=1)
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+if __name__ == '__main__':
+    main()

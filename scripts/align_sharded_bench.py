@@ -14,7 +14,6 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -22,41 +21,19 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 import torch.distributed as dist
 
-ap = argparse.ArgumentParser()
-ap.add_argument('--niter', type=int, default=300)
-ap.add_argument('--no-e2e', action='store_true')
-ap.add_argument('--configs', default='5,3')
-ap.add_argument('--out', default=None, help='also write the results of every config to this JSON file')
-args = ap.parse_args()
-
-rank, world, local = int(os.environ.get('RANK', 0)), int(os.environ.get('WORLD_SIZE', 1)), int(os.environ.get('LOCAL_RANK', 0))
-torch.cuda.set_device(local)
-dev = torch.device('cuda', local)
-os.environ.setdefault('MASTER_ADDR', '127.0.0.1')
-os.environ.setdefault('MASTER_PORT', '29512')
-dist.init_process_group('nccl', device_id=dev, rank=rank, world_size=world)
-
+from bench import build_model
+from common import barrier_sync, card
 from dust3r_b200 import _lib
 from dust3r_b200.cloud_opt import GlobalAlignerMode, global_aligner
-from dust3r_b200.distributed import _AlignShard, shard_images
-from dust3r_b200.utils.synth import synth_pair_predictions
+from dust3r_b200.distributed import _AlignShard, global_aligner_sharded, inference_sharded, shard_images
+from dust3r_b200.image_pairs import make_pairs
+from dust3r_b200.utils.synth import synth_images, synth_pair_predictions
 
 H, W = 384, 512
 CONFIGS = {'5': (50, 'ModularPointCloudOptimizer'), '3': (8, 'PointCloudOptimizer')}
 
 
-def card():
-    q = subprocess.run(['nvidia-smi', '-i', str(torch.cuda.current_device()), '--query-gpu=name,power.limit,clocks.sm,clocks.max.sm',
-                        '--format=csv,noheader'], capture_output=True, text=True)
-    return q.stdout.strip() or torch.cuda.get_device_name()
-
-
-def sync():
-    torch.cuda.synchronize()
-    dist.barrier()
-
-
-def sharded_scene(out, mode):
+def sharded_scene(out, mode, dev, world):
     """The scene global_aligner_sharded returns, also at world 1 (where global_aligner_sharded hands back the fused scene)."""
     torch.manual_seed(0)
     scene = global_aligner(out, dev, mode=GlobalAlignerMode[mode], verbose=False)
@@ -70,23 +47,23 @@ def sharded_scene(out, mode):
 
 def timed_alignment(scene, niter):
     scene.compute_global_alignment(init=None, niter=5)          # warm-up: engine build, packing, module loads
-    sync()
+    barrier_sync()
     t0 = time.perf_counter()
     loss = scene.compute_global_alignment(init=None, niter=niter, schedule='cosine', lr=0.01)
-    sync()
+    barrier_sync()
     return time.perf_counter() - t0, loss
 
 
 def split_breakdown(eng, niter):
     """Mean ms of the pixel pass, the all-reduce and the small step per iteration (CUDA events around each)."""
     eng.reset_adam()
-    eng.sched = torch.from_numpy(eng.make_schedule(niter, 0.01, 'cosine', 1e-6)).to(dev)
-    eng.loss_out = torch.zeros((niter,), dtype=torch.float32, device=dev)
+    eng.sched = torch.from_numpy(eng.make_schedule(niter, 0.01, 'cosine', 1e-6)).to(eng.device)
+    eng.loss_out = torch.zeros((niter,), dtype=torch.float32, device=eng.device)
     eng._sync_start()
     eng.prepare()
     d = eng._desc()
     ev = [[torch.cuda.Event(enable_timing=True) for _ in range(4)] for _ in range(niter)]
-    sync()
+    barrier_sync()
     for it in range(niter):
         ev[it][0].record()
         if eng.n_items:
@@ -96,79 +73,94 @@ def split_breakdown(eng, niter):
         ev[it][2].record()
         _lib.launch(eng.device, 'd3r_align_small_step', ctypes.byref(d), it)
         ev[it][3].record()
-    sync()
+    barrier_sync()
     parts = [sum(ev[it][k].elapsed_time(ev[it][k + 1]) for it in range(niter)) / niter for k in range(3)]
     return dict(pixel_pass_ms=round(parts[0], 4), all_reduce_ms=round(parts[1], 4), small_step_ms=round(parts[2], 4))
 
 
-res_all = []
-for key in args.configs.split(','):
-    n, mode = CONFIGS[key]
-    edges = [(i, j) for i in range(n) for j in range(i)]
-    out = synth_pair_predictions(n, edges, H, W, seed=0)
-    res = dict(config=key, n_views=n, n_pairs=len(edges), mode=mode, niter=args.niter, world=world, card=card())
-    # fused single-GPU loop on rank 0's GPU alone
-    if rank == 0:
-        torch.manual_seed(0)
-        scene = global_aligner(out, dev, mode=GlobalAlignerMode[mode], verbose=False)
-        scene.compute_global_alignment(init=None, niter=5)
-        torch.cuda.synchronize()
-        t0 = time.perf_counter()
-        loss = scene.compute_global_alignment(init=None, niter=args.niter, schedule='cosine', lr=0.01)
-        torch.cuda.synchronize()
-        dt = time.perf_counter() - t0
-        res.update(fused_1gpu_s=round(dt, 4), fused_1gpu_it_per_s=round(args.niter / dt, 1), fused_final_loss=loss)
-        del scene
-        torch.cuda.empty_cache()
-    sync()
-    scene = sharded_scene(out, mode)
-    dt, loss = timed_alignment(scene, args.niter)
-    eng = scene._get_engine()
-    obs = [None] * world
-    dist.all_gather_object(obs, (eng.owned, eng.total_obs * 16))
-    res.update(sharded_s=round(dt, 4), sharded_it_per_s=round(args.niter / dt, 1), sharded_final_loss=loss,
-               shards=[o[0] for o in obs], obs_bytes_per_rank=[o[1] for o in obs],
-               obs_bytes_max_over_mean=round(max(o[1] for o in obs) / (sum(o[1] for o in obs) / world), 4))
-    res.update(split_breakdown(eng, args.niter))
-    del scene, eng
-    torch.cuda.empty_cache()
-    if key == '5' and not args.no_e2e:
-        # config 5 end to end: sharded forward + one all-gather, then the sharded alignment on every rank
-        from bench import build_model
-        from dust3r_b200.distributed import global_aligner_sharded, inference_sharded
-        from dust3r_b200.image_pairs import make_pairs
-        from dust3r_b200.utils.synth import synth_images
-        net, _ = build_model(dev)
-        imgs = synth_images(n, H, W, seed=21)
-        pairs = make_pairs(imgs, scene_graph='complete', prefilter=None, symmetrize=False)
-        inference_sharded(pairs[:2 * world], net, dev, batch_size=32, verbose=False, gather_device=dev)   # warm-up
-        sync()
-        t0 = time.perf_counter()
-        fwd = inference_sharded(pairs, net, dev, batch_size=32, verbose=False, gather_device=dev, return_images=False)
-        sync()
-        t_fwd = time.perf_counter() - t0
-        del net
-        torch.manual_seed(0)
-        scene = sharded_scene(fwd, mode) if world == 1 else global_aligner_sharded(
-            fwd, dev, mode=GlobalAlignerMode[mode], verbose=False)
-        sync()
-        t_build = time.perf_counter() - t0 - t_fwd
-        t1 = time.perf_counter()
-        scene.compute_global_alignment(init=None, niter=args.niter, schedule='cosine', lr=0.01)
-        sync()
-        t_align = time.perf_counter() - t1
-        res.update(e2e_forward_and_gather_s=round(t_fwd, 3), e2e_aligner_build_s=round(t_build, 3),
-                   e2e_align_s=round(t_align, 3), e2e_total_s=round(time.perf_counter() - t0, 3),
-                   e2e_note='random-init weights, init=None: timing only; the align time includes the engine build and packing')
-        del scene, fwd
-        torch.cuda.empty_cache()
-    if rank == 0:
-        print(json.dumps(res), flush=True)
-        res_all.append(res)
-    sync()
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument('--niter', type=int, default=300)
+    ap.add_argument('--no-e2e', action='store_true')
+    ap.add_argument('--configs', default='5,3')
+    ap.add_argument('--out', default=None, help='also write the results of every config to this JSON file')
+    args = ap.parse_args()
 
-if rank == 0 and args.out:
-    with open(args.out, 'w') as f:
-        json.dump(res_all, f, indent=1)
-dist.barrier()
-dist.destroy_process_group()
+    rank, world, local = int(os.environ.get('RANK', 0)), int(os.environ.get('WORLD_SIZE', 1)), int(os.environ.get('LOCAL_RANK', 0))
+    torch.cuda.set_device(local)
+    dev = torch.device('cuda', local)
+    os.environ.setdefault('MASTER_ADDR', '127.0.0.1')
+    os.environ.setdefault('MASTER_PORT', '29512')
+    dist.init_process_group('nccl', device_id=dev, rank=rank, world_size=world)
+
+    res_all = []
+    for key in args.configs.split(','):
+        n, mode = CONFIGS[key]
+        edges = [(i, j) for i in range(n) for j in range(i)]
+        out = synth_pair_predictions(n, edges, H, W, seed=0)
+        res = dict(config=key, n_views=n, n_pairs=len(edges), mode=mode, niter=args.niter, world=world, card=card(dev))
+        # fused single-GPU loop on rank 0's GPU alone
+        if rank == 0:
+            torch.manual_seed(0)
+            scene = global_aligner(out, dev, mode=GlobalAlignerMode[mode], verbose=False)
+            scene.compute_global_alignment(init=None, niter=5)
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            loss = scene.compute_global_alignment(init=None, niter=args.niter, schedule='cosine', lr=0.01)
+            torch.cuda.synchronize()
+            dt = time.perf_counter() - t0
+            res.update(fused_1gpu_s=round(dt, 4), fused_1gpu_it_per_s=round(args.niter / dt, 1), fused_final_loss=loss)
+            del scene
+            torch.cuda.empty_cache()
+        barrier_sync()
+        scene = sharded_scene(out, mode, dev, world)
+        dt, loss = timed_alignment(scene, args.niter)
+        eng = scene._get_engine()
+        obs = [None] * world
+        dist.all_gather_object(obs, (eng.owned, eng.total_obs * 16))
+        res.update(sharded_s=round(dt, 4), sharded_it_per_s=round(args.niter / dt, 1), sharded_final_loss=loss,
+                   shards=[o[0] for o in obs], obs_bytes_per_rank=[o[1] for o in obs],
+                   obs_bytes_max_over_mean=round(max(o[1] for o in obs) / (sum(o[1] for o in obs) / world), 4))
+        res.update(split_breakdown(eng, args.niter))
+        del scene, eng
+        torch.cuda.empty_cache()
+        if key == '5' and not args.no_e2e:
+            # config 5 end to end: sharded forward + one all-gather, then the sharded alignment on every rank
+            net, _ = build_model(dev)
+            imgs = synth_images(n, H, W, seed=21)
+            pairs = make_pairs(imgs, scene_graph='complete', prefilter=None, symmetrize=False)
+            inference_sharded(pairs[:2 * world], net, dev, batch_size=32, verbose=False, gather_device=dev)   # warm-up
+            barrier_sync()
+            t0 = time.perf_counter()
+            fwd = inference_sharded(pairs, net, dev, batch_size=32, verbose=False, gather_device=dev, return_images=False)
+            barrier_sync()
+            t_fwd = time.perf_counter() - t0
+            del net
+            torch.manual_seed(0)
+            scene = sharded_scene(fwd, mode, dev, world) if world == 1 else global_aligner_sharded(
+                fwd, dev, mode=GlobalAlignerMode[mode], verbose=False)
+            barrier_sync()
+            t_build = time.perf_counter() - t0 - t_fwd
+            t1 = time.perf_counter()
+            scene.compute_global_alignment(init=None, niter=args.niter, schedule='cosine', lr=0.01)
+            barrier_sync()
+            t_align = time.perf_counter() - t1
+            res.update(e2e_forward_and_gather_s=round(t_fwd, 3), e2e_aligner_build_s=round(t_build, 3),
+                       e2e_align_s=round(t_align, 3), e2e_total_s=round(time.perf_counter() - t0, 3),
+                       e2e_note='random-init weights, init=None: timing only; the align time includes the engine build and packing')
+            del scene, fwd
+            torch.cuda.empty_cache()
+        if rank == 0:
+            print(json.dumps(res), flush=True)
+            res_all.append(res)
+        barrier_sync()
+
+    if rank == 0 and args.out:
+        with open(args.out, 'w') as f:
+            json.dump(res_all, f, indent=1)
+    dist.barrier()
+    dist.destroy_process_group()
+
+
+if __name__ == '__main__':
+    main()

@@ -17,7 +17,7 @@ import torch.nn.functional as F
 
 from dust3r_b200 import _lib
 from dust3r_b200._lib_fwd import F_BIAS, F_RELU, F_ADD0, F_ADD1, F_OUT2_RELU
-from gemm_store_ab import gpu_info, events_ms
+from common import card, events_ms
 
 B = 32
 LEVELS = [(96, 128), (48, 64), (24, 32), (12, 16)]   # run_dpt Hs / Ws of the 24x32 grid
@@ -39,7 +39,7 @@ def main():
     _lib.require_cuda_device(dev)
     lib = _lib.get_lib()
     g = torch.Generator(device='cpu').manual_seed(0)
-    print(json.dumps(dict(kind='gpu', nvidia_smi=gpu_info())), flush=True)
+    print(json.dumps(dict(kind='gpu', nvidia_smi=card(dev))), flush=True)
     for name, H, W, Cin, Cout, flags in SHAPES:
         x = torch.randn((B, H, W, Cin), generator=g).bfloat16().to(dev)
         w = (torch.randn((Cout, Cin, 3, 3), generator=g) * (9 * Cin) ** -0.5).bfloat16().to(dev)
@@ -63,17 +63,16 @@ def main():
 
         for store in (0, 1):
             lib.d3r_set_conv_store(store)
-            events_ms(run, args.warmup)
-            torch.cuda.synchronize()
+            events_ms(run, args.warmup, 0)
             res[store] = [t.clone() for t in (out, out2) if t is not None]
-        events_ms(ref, args.warmup)
+        events_ms(ref, args.warmup, 0)
         same = all(torch.equal(a.view(torch.int16), b.view(torch.int16)) for a, b in zip(res[0], res[1]))
         times = {0: [], 1: [], 'cudnn': []}
         for _ in range(args.rounds):
             for store in (0, 1):
                 lib.d3r_set_conv_store(store)
-                times[store].append(events_ms(run, args.iters))
-            times['cudnn'].append(events_ms(ref, args.iters))
+                times[store].append(events_ms(run, args.iters, 0))
+            times['cudnn'].append(events_ms(ref, args.iters, 0))
         lib.d3r_set_conv_store(1)
         flop = 2.0 * B * H * W * Cout * 9 * Cin
         best = {k: min(v) for k, v in times.items()}
@@ -83,7 +82,7 @@ def main():
                               cudnn_tflops=round(flop / best['cudnn'] / 1e9, 1), speedup=round(best[0] / best[1], 3),
                               rounds={str(k): [round(t, 4) for t in v] for k, v in times.items()})), flush=True)
         del x, w, wp, add0, add1, out, out2, res
-    print(json.dumps(dict(kind='gpu', nvidia_smi=gpu_info())), flush=True)
+    print(json.dumps(dict(kind='gpu', nvidia_smi=card(dev))), flush=True)
 
 
 if __name__ == '__main__':

@@ -14,7 +14,6 @@ All times are CUDA-event times after warm-up.  Prints one JSON line, with the ca
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -26,18 +25,13 @@ import dust3r_b200.losses as L  # noqa: E402
 from dust3r_b200.inference import loss_of_one_batch  # noqa: E402
 from dust3r_b200.utils.geometry import geotrf  # noqa: E402
 from dust3r_b200.utils.synth import synth_consistent_scene  # noqa: E402
+from common import card, events_ms  # noqa: E402
 
 H, W = 384, 512
 PAIRS = 32
 TRAIN = "ConfLoss(Regr3D(L21, norm_mode='avg_dis'), alpha=0.2)"
 TEST = "Regr3D_ScaleShiftInv(L21, gt_scale=True)"
 BYTES_PER_PIXEL_VIEW = 29
-
-
-def card():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader', '-i',
-                        str(torch.cuda.current_device())], capture_output=True, text=True)
-    return q.stdout.strip() or torch.cuda.get_device_name()
 
 
 def batch(n_pairs, device, seed=0):
@@ -61,19 +55,6 @@ def batch(n_pairs, device, seed=0):
     return tuple({k: v.to(device) for k, v in d.items()} for d in (gt1, gt2, pred1, pred2))
 
 
-def timed(fn, iters, warmup):
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--iters', type=int, default=20)
@@ -86,12 +67,12 @@ def main():
     dev = torch.device('cuda', torch.cuda.current_device())
     inputs = batch(PAIRS, dev)
     floor_bytes = BYTES_PER_PIXEL_VIEW * 2 * PAIRS * H * W
-    res = dict(card=card(), pairs=PAIRS, H=H, W=W, floor_bytes=floor_bytes, criteria={})
+    res = dict(card=card(dev), pairs=PAIRS, H=H, W=W, floor_bytes=floor_bytes, criteria={})
     for expr in (TRAIN, TEST):
         crit = eval(expr, vars(L))
-        ours = timed(lambda: crit(*inputs), args.iters, args.warmup)
+        ours = events_ms(lambda: crit(*inputs), args.iters, args.warmup)
         with L.host_port():
-            ref = timed(lambda: crit(*inputs), max(3, args.iters // 4), 1)
+            ref = events_ms(lambda: crit(*inputs), max(3, args.iters // 4), 1)
             ref_loss = float(crit(*inputs)[0])
         loss = float(crit(*inputs)[0])
         res['criteria'][expr] = dict(cuda_ms=round(ours, 4), host_port_on_gpu_ms=round(ref, 3), speedup=round(ref / ours, 2),
@@ -113,8 +94,8 @@ def main():
             def step(c=crit):
                 with torch.no_grad():
                     return loss_of_one_batch(tuple(dict(v) for v in views), net, c, dev, symmetrize_batch=True, ret='loss')
-            with_ms = timed(step, max(3, args.iters // 4), 2)
-            without_ms = timed(lambda: step(None), max(3, args.iters // 4), 1)
+            with_ms = events_ms(step, max(3, args.iters // 4), 2)
+            without_ms = events_ms(lambda: step(None), max(3, args.iters // 4), 1)
             r = res['criteria'][expr]
             r['step_ms'] = round(with_ms, 2)
             r['step_without_criterion_ms'] = round(without_ms, 2)

@@ -9,7 +9,6 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -18,31 +17,13 @@ import torch
 from dust3r_b200 import _lib
 from dust3r_b200._lib_fwd import F_BIAS, F_GELU, F_RESID_INPLACE, F_ROPE
 from oracle.forward_oracle import rope_tables
+from common import card, events_ms
 
 ENC, DEC = 64 * 768, 32 * 768
 SHAPES = [('enc qkv', ENC, 3072, 1024, 'rope'), ('enc proj', ENC, 1024, 1024, 'resid'), ('enc fc1', ENC, 4096, 1024, 'gelu'),
           ('enc fc2', ENC, 1024, 4096, 'resid'), ('dec qkv', DEC, 2304, 768, 'rope'), ('dec proj', DEC, 768, 768, 'resid'),
           ('dec fc1', DEC, 3072, 768, 'gelu'), ('dec fc2', DEC, 768, 3072, 'resid')]
 GH, GW = 24, 32
-
-
-def gpu_info():
-    q = 'name,power.limit,clocks.sm,clocks.max.sm'
-    try:
-        return subprocess.run(['nvidia-smi', f'--query-gpu={q}', '--format=csv,noheader'], capture_output=True, text=True,
-                              timeout=30).stdout.strip().splitlines()[0]
-    except (OSError, subprocess.SubprocessError, IndexError):
-        return 'unknown'
-
-
-def events_ms(fn, iters):
-    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    start.record()
-    for _ in range(iters):
-        fn()
-    end.record()
-    torch.cuda.synchronize()
-    return start.elapsed_time(end) / iters
 
 
 def main():
@@ -56,7 +37,7 @@ def main():
     lib = _lib.get_lib()
     g = torch.Generator(device='cpu').manual_seed(0)
     cos, sin = (t.to(dev).contiguous() for t in rope_tables(64, max(GH, GW), 100.0))
-    print(json.dumps(dict(kind='gpu', nvidia_smi=gpu_info())), flush=True)
+    print(json.dumps(dict(kind='gpu', nvidia_smi=card(dev))), flush=True)
     for name, M, N, K, epi in SHAPES:
         A = torch.randn((M, K), generator=g).bfloat16().to(dev)
         B = (torch.randn((N, K), generator=g) * K ** -0.5).bfloat16().to(dev)
@@ -79,13 +60,13 @@ def main():
         times = {0: [], 1: [], 'torch': []}
         for store in (0, 1):
             lib.d3r_set_gemm_store(store)
-            events_ms(run, args.warmup)
-        events_ms(ref, args.warmup)
+            events_ms(run, args.warmup, 0)
+        events_ms(ref, args.warmup, 0)
         for _ in range(args.rounds):
             for store in (0, 1):
                 lib.d3r_set_gemm_store(store)
-                times[store].append(events_ms(run, args.iters))
-            times['torch'].append(events_ms(ref, args.iters))
+                times[store].append(events_ms(run, args.iters, 0))
+            times['torch'].append(events_ms(ref, args.iters, 0))
         lib.d3r_set_gemm_store(1)
         flop = 2.0 * M * N * K
         best = {k: min(v) for k, v in times.items()}
@@ -95,7 +76,7 @@ def main():
                               torch_tflops=round(flop / best['torch'] / 1e9, 1), speedup=round(best[0] / best[1], 3),
                               rounds={str(k): [round(t, 4) for t in v] for k, v in times.items()})), flush=True)
         del A, B, out
-    print(json.dumps(dict(kind='gpu', nvidia_smi=gpu_info())), flush=True)
+    print(json.dumps(dict(kind='gpu', nvidia_smi=card(dev))), flush=True)
 
 
 if __name__ == '__main__':

@@ -24,6 +24,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
 
+from common import card
+
 ENC_GFLOP, PAIR_GFLOP = 1046.1 / 2, 437.3 + 373.4
 CASES = dict(sym50_bs1=(50, 0, 1), sym50_bs32=(50, 0, 32), mixed12_bs16=(6, 6, 16))   # landscape views, portrait views, batch
 
@@ -92,7 +94,7 @@ def main():
         tflop = (passes * ENC_GFLOP + len(pairs) * PAIR_GFLOP) / 1e3
         print(json.dumps(dict(case=name, views=n_land + n_port, pairs=len(pairs), batch_size=bs, seconds=[round(x, 3) for x in times],
                               pairs_per_s=round(len(pairs) / t, 1), encoder_passes=passes, algorithmic_tflop=round(tflop, 1),
-                              algorithmic_tflop_per_s=round(tflop / t, 1))), flush=True)
+                              algorithmic_tflop_per_s=round(tflop / t, 1), card=card(dev))), flush=True)
         if args.dump_outputs:
             os.makedirs(args.dump_outputs, exist_ok=True)
             np.savez(os.path.join(args.dump_outputs, f'{name}.npz'), **sample(out))

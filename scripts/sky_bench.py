@@ -9,7 +9,8 @@ one JSON line with
                      scene's deepcopy, the pinned upload of scene.imgs, quantisation, the kernels and the im_conf writes
   segment_ms         wall time of the batched segmentation alone, from the float host images (pinned upload included)
   host_ms            wall time of the host path (OpenCV + scipy, dust3r_b200.viz.segment_sky on numpy) on the same images
-together with the GPU name and its power limit, read in the same run.
+together with the card line (GPU name, power limit and SM clocks) in `gpu` and the power limit alone in `power_limit`, read
+in the same run.
 
 Usage:  python scripts/sky_bench.py [--n 50] [--hw 384 512] [--iters 20] [--out FILE]
 """
@@ -17,7 +18,6 @@ import argparse
 import copy
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -30,24 +30,9 @@ from dust3r_b200.cloud_opt import global_aligner  # noqa: E402
 from dust3r_b200.cloud_opt.scene_ops import _quantise, segment_sky_host_images  # noqa: E402
 from dust3r_b200.utils.synth import synth_pair_predictions, synth_sky_image  # noqa: E402
 from dust3r_b200.viz import segment_sky  # noqa: E402
+from common import card, events_ms, wall_ms  # noqa: E402
 
 BYTES_PER_PIXEL = 44
-
-
-def gpu_info():
-    q = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit', '--format=csv,noheader'], capture_output=True, text=True)
-    name, power = (q.stdout.strip().splitlines() or ['?, ?'])[0].split(', ')
-    return name, power
-
-
-def wall_ms(fn, iters):
-    fn()
-    torch.cuda.synchronize()
-    t = time.perf_counter()
-    for _ in range(iters):
-        fn()
-    torch.cuda.synchronize()
-    return 1e3 * (time.perf_counter() - t) / iters
 
 
 def main():
@@ -75,24 +60,16 @@ def main():
     def kernels():
         _lib.check(lib.d3r_segment_sky(n, hw.data_ptr(), off.data_ptr(), H * W, total, rgb.data_ptr(), out.data_ptr(), ws.data_ptr(),
                                        ws.numel(), stream))
-    for _ in range(3):
-        kernels()
-    start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    start.record()
-    for _ in range(a.iters):
-        kernels()
-    end.record()
-    torch.cuda.synchronize()
-    kernel_ms = start.elapsed_time(end) / a.iters
+    kernel_ms = events_ms(kernels, a.iters, 3)
 
-    segment_ms = wall_ms(lambda: segment_sky_host_images(images, dev), a.iters)
+    segment_ms = wall_ms(lambda: segment_sky_host_images(images, dev), a.iters, 1)
 
     edges = [(i, i + 1) for i in range(n - 1)]
     out_pairs = synth_pair_predictions(n, edges + [(j, i) for i, j in edges], H, W, seed=1)
     for view in ('view1', 'view2'):
         out_pairs[view]['img'] = torch.stack([torch.from_numpy(2 * images[i] - 1).permute(2, 0, 1) for i in out_pairs[view]['idx']])
     scene = global_aligner(out_pairs, dev, verbose=False)
-    mask_sky_ms = wall_ms(scene.mask_sky, max(a.iters // 4, 3))
+    mask_sky_ms = wall_ms(scene.mask_sky, max(a.iters // 4, 3), 1)
 
     host_iters = max(a.iters // 10, 1)
     t = time.perf_counter()
@@ -101,12 +78,12 @@ def main():
     host_ms = 1e3 * (time.perf_counter() - t) / host_iters
     same = all(torch.equal(h, d.cpu()) for h, d in zip(host, segment_sky_host_images(images, dev)))
 
-    gpu, power = gpu_info()
+    gpu = card(dev)
     algo = BYTES_PER_PIXEL * total
     r = dict(bench='segment_sky', n=n, H=H, W=W, kernel_ms=round(kernel_ms, 4), kernel_GBps=round(algo / kernel_ms / 1e6, 1),
              algo_bytes=algo, segment_ms=round(segment_ms, 3), mask_sky_ms=round(mask_sky_ms, 3), host_ms=round(host_ms, 2),
              host_threads=int(__import__('cv2').getNumThreads()), sky_fraction=round(float(out.float().mean()), 4),
-             host_equals_device=same, gpu=gpu, power_limit=power)
+             host_equals_device=same, gpu=gpu, power_limit=gpu.split(', ')[1])
     line = json.dumps(r)
     print(line)
     if a.out:

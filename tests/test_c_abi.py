@@ -54,10 +54,10 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, n), f'{n} declared in include/dust3r_b200.h but not exported'
 
 
-def test_abi_version_5_and_struct_size():
+def test_abi_version_6_and_struct_size():
     from dust3r_b200 import _lib
     lib = _lib.get_lib()
-    assert lib.d3r_abi_version() == 5
+    assert lib.d3r_abi_version() == 6
     assert lib.d3r_align_chunk_pixels() == 2048   # maximum; the host picks chunk_px <= this per problem
     # python mirror of d3r_align_desc must match the C layout: probe through workspace sizing
     assert lib.d3r_align_workspace_floats(8, 28) > 0
