@@ -41,8 +41,23 @@ class AlignDesc(C.Structure):
     ]
 
 
+class JpegHuff(C.Structure):
+    """Mirror of `d3r_jpeg_huff` (include/dust3r_b200.h)."""
+    _fields_ = [('maxcode', C.c_int32 * 18), ('valoff', C.c_int32 * 18), ('look', C.c_uint16 * 512), ('val', C.c_uint8 * 256)]
+
+
+class JpegDesc(C.Structure):
+    """Mirror of `d3r_jpeg_desc` (include/dust3r_b200.h)."""
+    _fields_ = [
+        ('width', C.c_int32), ('height', C.c_int32), ('n_comp', C.c_int32), ('restart_interval', C.c_int32),
+        ('orientation', C.c_int32), ('reserved', C.c_int32), ('scan_begin', C.c_int64),
+        ('h_samp', C.c_int32 * 3), ('v_samp', C.c_int32 * 3), ('dc_table', C.c_int32 * 3), ('ac_table', C.c_int32 * 3),
+        ('quant', (C.c_uint16 * 64) * 3), ('huff', JpegHuff * 8),
+    ]
+
+
 vp, i32, i64, u32, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_float
-_DESC, _MODEL = C.POINTER(AlignDesc), C.POINTER(Model)
+_DESC, _MODEL, _JPEG = C.POINTER(AlignDesc), C.POINTER(Model), C.POINTER(JpegDesc)
 
 # restype, argtypes of every function include/dust3r_b200.h declares, in its order (tests/test_c_abi.py checks the two agree).
 PROTOTYPES = {
@@ -95,6 +110,9 @@ PROTOTYPES = {
     'd3r_nearest_neighbours': (i32, [i32, i32, vp, vp, vp, vp]),
     'd3r_image_resize_crop_normalize': (i32, [vp, i32, i32, i32, i32, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32,
                                               vp, vp, vp, vp]),
+    'd3r_sizeof_jpeg_desc': (i32, []),
+    'd3r_jpeg_decode_workspace_bytes': (i64, [_JPEG, i64]),
+    'd3r_jpeg_decode': (i32, [_JPEG, vp, i64, vp, vp, vp, i64, vp]),
     'd3r_segment_sky_workspace_bytes': (i64, [i32, i64]),
     'd3r_segment_sky': (i32, [i32, vp, vp, i32, i64, vp, vp, vp, i64, vp]),
     'd3r_nanmedian_workspace_bytes': (i64, [i32]),

@@ -4,8 +4,9 @@ turns normalised tensors back into displayable arrays for the optimizer's `imgs`
 are those of dust3r/utils/image.py:74-128.
 
 `load_images(..., device=None)` is the reference's host path (PIL resize + crop on a CPU core, float image to be uploaded by
-inference()).  `load_images(..., device='cuda')` (SURVEY §8f rank 4) only DECODES on the host: the 8-bit RGB pixels go up once
-and the resize (Pillow's two-pass fixed-point resampling, restated as two integer kernels), the crop and ImgNorm run on the
+inference()).  `load_images(..., device='cuda')` (SURVEY §8f rank 4) reads each file and parses its header on the host; baseline JPEGs go
+up compressed and are decoded on the H100 (`decode_jpeg`, csrc/jpeg_ops.cu, bit-identical to Pillow), other files are decoded
+by Pillow and their 8-bit RGB pixels go up; then the resize (Pillow's two-pass fixed-point resampling, restated as two integer kernels), the crop and ImgNorm run on the
 H100 (`d3r_image_resize_crop_normalize`, csrc/image_ops.cu) -- bit-identical to the host path, the normalised image is born
 in HBM and inference() uses it in place."""
 from __future__ import annotations
@@ -77,6 +78,67 @@ def _open_rgb(path):
     return exif_transpose(PIL.Image.open(path)).convert('RGB')
 
 
+def _pillow_rgb(data):
+    import io
+    import PIL.Image
+    from PIL.ImageOps import exif_transpose
+    return np.array(exif_transpose(PIL.Image.open(io.BytesIO(data))).convert('RGB'), dtype=np.uint8)
+
+
+def _jpeg_stage(data):
+    """Host half of decode_jpeg, safe to run on a worker thread: (descriptor, oriented (width, height), pinned bytes), or None
+    when the file is outside the device decoder's set (csrc/jpeg_ops.cu)."""
+    from . import jpeg
+    try:
+        head = jpeg.parse(data)
+    except jpeg.Unsupported:
+        return None
+    orient = jpeg.orientation(data)
+    pinned = torch.frombuffer(bytearray(data), dtype=torch.uint8)
+    if torch.cuda.is_available():
+        pinned = pinned.pin_memory()
+    return jpeg.descriptor(head, orient), jpeg.oriented_size(head, orient), pinned
+
+
+def _jpeg_launch(staged, dev):
+    """Uploads the bytes and enqueues the decode on `dev`'s current stream -> (uint8 (H, W, 3) image, int32 status) on `dev`."""
+    import ctypes
+    from .. import _lib
+    desc, (w, h), pinned = staged
+    lib = _lib.get_lib()
+    n = int(pinned.numel())
+    ws_bytes = int(lib.d3r_jpeg_decode_workspace_bytes(ctypes.byref(desc), n))
+    if ws_bytes <= 0:
+        raise _lib.D3RError('d3r_jpeg_decode_workspace_bytes rejected the descriptor')
+    src = pinned.to(dev, non_blocking=True)
+    out = torch.empty((h, w, 3), dtype=torch.uint8, device=dev)
+    status = torch.empty((1,), dtype=torch.int32, device=dev)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+    _lib.launch(dev, 'd3r_jpeg_decode', ctypes.byref(desc), src.data_ptr(), n, out.data_ptr(), status.data_ptr(), ws.data_ptr(),
+                ws_bytes)
+    return out, status
+
+
+@torch.no_grad()
+def decode_jpeg(data, device='cuda'):
+    """JPEG file contents (bytes) -> uint8 (H, W, 3) RGB tensor on `device`, equal to
+    np.asarray(exif_transpose(PIL.Image.open(f)).convert('RGB')).  Baseline files (8-bit sequential Huffman, grey or YCbCr at
+    4:4:4, 4:2:2 or 4:2:0) are decoded by the GPU kernels of csrc/jpeg_ops.cu; any other file, and any stream those kernels
+    report they cannot reproduce exactly, is decoded by Pillow and uploaded -- the choice is made from the file, so the result
+    is Pillow's either way (including the exception Pillow raises for a broken file)."""
+    from .. import _lib
+    dev = _lib.require_cuda_device(device)
+    if dev.index is None:
+        dev = torch.device('cuda', torch.cuda.current_device())
+    data = bytes(data)
+    staged = _jpeg_stage(data)
+    if staged is not None:
+        img, status = _jpeg_launch(staged, dev)
+        if int(status.item()) == 0:
+            return img
+    return torch.from_numpy(_pillow_rgb(data)).to(dev)
+
+
 def _host_view(pil, size, square_ok, patch_size):
     """The reference's per-image pipeline on a decoded PIL image: resize, centre crop, ImgNorm -> (1, 3, H, W) CPU tensor."""
     w_in, h_in = pil.size
@@ -91,8 +153,9 @@ def _host_view(pil, size, square_ok, patch_size):
 def load_images(folder_or_list, size, square_ok=False, verbose=True, patch_size=16, device=None, workers=None):
     """Folder name or list of file names -> list of dict(img (1,3,H,W) in [-1,1], true_shape int32 [[H,W]], idx,
     instance) ready for make_pairs / inference.  Files that are not .jpg/.jpeg/.png are skipped.
-    device=None: the reference's host pipeline, `img` is a CPU tensor.  device=<an H100>: decode on the host, resize / crop /
-    normalise on that GPU (same bits), `img` is resident there.
+    device=None: the reference's host pipeline, `img` is a CPU tensor.  device=<an H100>: baseline JPEGs decoded on that GPU
+    (other files, and streams the GPU decoder reports it cannot reproduce, by Pillow), resize / crop / normalise on that GPU
+    (same bits), `img` is resident there.
     Files are decoded (device=None: decoded, resized and normalised) by `workers` threads -- PIL releases the GIL in its codecs
     and resampling loops -- while the results are consumed in file order, so idx / instance / verbose output are those of the
     reference's sequential loop; default min(8, cores), workers=1 is strictly sequential."""
@@ -105,7 +168,14 @@ def load_images(folder_or_list, size, square_ok=False, verbose=True, patch_size=
     names = [name for name in names if name.lower().endswith(_EXTENSIONS)]
 
     def host_stage(name):
-        pil = _open_rgb(os.path.join(root, name))
+        path = os.path.join(root, name)
+        if device is not None:
+            with open(path, 'rb') as f:
+                data = f.read()
+            staged = _jpeg_stage(data)
+            if staged is not None:              # decoded on the GPU; data kept for the Pillow path if the stream is refused
+                return staged[1], (data, staged)
+        pil = _open_rgb(path)
         if device is None:
             return pil.size, _host_view(pil, size, square_ok, patch_size)
         return pil.size, np.array(pil, dtype=np.uint8)
@@ -114,21 +184,54 @@ def load_images(folder_or_list, size, square_ok=False, verbose=True, patch_size=
         workers = min(8, os.cpu_count() or 1)
     workers = max(1, min(int(workers), len(names)))
     views = []
+    # device path: decodes and resizes are enqueued without waiting; each file's status word comes back through pinned memory
+    # behind an event, and files are finalised (status checked, Pillow used where the kernels refused the stream, verbose
+    # line, view appended) strictly in file order, so that output and exceptions are those of the sequential loop
+    from collections import deque
+    pending = deque()
 
-    def consume(name, staged):
-        (w_in, h_in), item = staged
-        img = item if device is None else preprocess_image_u8(item, size, square_ok, device, patch_size)
+    def finalize(entry):
+        name, (w_in, h_in), img, check = entry
+        if check is not None:
+            event, status, data = check
+            event.synchronize()
+            if int(status[0]) != 0:
+                img = preprocess_image_u8(_pillow_rgb(data), size, square_ok, device, patch_size)
         h_out, w_out = int(img.shape[-2]), int(img.shape[-1])
         if verbose:
             print(f' - adding {name} with resolution {w_in}x{h_in} --> {w_out}x{h_out}')
         views.append(dict(img=img, true_shape=np.int32([[h_out, w_out]]), idx=len(views), instance=str(len(views))))
+
+    def consume(name, staged):
+        size_in, item = staged
+        check = None
+        if device is None:
+            img = item
+        elif isinstance(item, np.ndarray):
+            img = preprocess_image_u8(item, size, square_ok, device, patch_size)
+        else:
+            from .. import _lib
+            dev = _lib.require_cuda_device(device)
+            if dev.index is None:
+                dev = torch.device('cuda', torch.cuda.current_device())
+            data, jpeg_staged = item
+            pixels, status_dev = _jpeg_launch(jpeg_staged, dev)
+            img = preprocess_image_u8(pixels, size, square_ok, dev, patch_size)
+            with torch.cuda.device(dev):
+                status = torch.empty((1,), dtype=torch.int32, pin_memory=True)
+                status.copy_(status_dev, non_blocking=True)
+                event = torch.cuda.Event()
+                event.record(torch.cuda.current_stream(dev))
+            check = (event, status, data)
+        pending.append((name, size_in, img, check))
+        while pending and (pending[0][3] is None or pending[0][3][0].query() or len(pending) > 2 * workers):
+            finalize(pending.popleft())
 
     if workers == 1:
         for name in names:
             consume(name, host_stage(name))
     else:
         # at most 2 x workers files in flight (a decoded 12 Mpx photograph is 36 MB), consumed strictly in file order
-        from collections import deque
         from concurrent.futures import ThreadPoolExecutor
         with ThreadPoolExecutor(max_workers=workers) as pool:
             window, todo = deque(), iter(names)
@@ -140,6 +243,8 @@ def load_images(folder_or_list, size, square_ok=False, verbose=True, patch_size=
             while window:
                 first, fut = window.popleft()
                 consume(first, fut.result())
+    while pending:
+        finalize(pending.popleft())
     assert views, 'no images found at ' + root
     if verbose:
         print(f' (Found {len(views)} images)')

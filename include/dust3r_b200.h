@@ -364,6 +364,44 @@ int d3r_image_resize_crop_normalize(const uint8_t* src_dev, int32_t H0, int32_t 
                                     const int32_t* ybounds_dev, const int32_t* ycoefs_dev, int32_t ky, int32_t row0, int32_t rows,
                                     int32_t crop_x0, int32_t crop_y0, int32_t H2, int32_t W2, const float* lut_dev, uint8_t* tmp_dev,
                                     float* out_dev, void* stream);
+/* Baseline JPEG decode (Pillow's np.asarray(exif_transpose(Image.open(f)).convert('RGB')), bit-exact): sequential Huffman,
+ * 8-bit, 1 component or 3 YCbCr components at 4:4:4, 4:2:2 or 4:2:0, any restart interval.  The host parses the header into a
+ * d3r_jpeg_desc; the compressed bytes [0, n_bytes) sit in device memory, the entropy-coded scan starts at scan_begin and ends at
+ * the first marker other than RSTn.  out = uint8 [H][W][3] RGB after the EXIF orientation (W and H swapped for 5-8).
+ * A stream that cannot be decoded exactly as libjpeg-turbo would sets bits of *status_dev (0 = decoded); the call itself only
+ * fails on bad arguments.  Workspace: d3r_jpeg_decode_workspace_bytes(desc, n_bytes) bytes, no initialisation. */
+typedef struct d3r_jpeg_huff {
+  int32_t maxcode[18];     /* largest code of each length 1..16 (-1: none); [0] and [17] unused */
+  int32_t valoff[18];      /* index into val of a code of each length, minus that code */
+  uint16_t look[512];      /* next 9 bits -> (length << 8) | symbol, length 0 when the code is longer than 9 bits */
+  uint8_t val[256];        /* symbols in code order, unused entries 0 */
+} d3r_jpeg_huff;
+
+typedef struct d3r_jpeg_desc {
+  int32_t width, height;           /* frame size before the orientation */
+  int32_t n_comp;                  /* 1 (grey) or 3 (YCbCr) */
+  int32_t restart_interval;        /* MCUs per restart interval, 0 = none */
+  int32_t orientation;             /* EXIF orientation 1..8 */
+  int32_t reserved;
+  int64_t scan_begin;              /* first byte of entropy-coded data, after the SOS header */
+  int32_t h_samp[3], v_samp[3];    /* sampling factors, scan order */
+  int32_t dc_table[3], ac_table[3];/* Huffman table slots 0..3 per component */
+  uint16_t quant[3][64];           /* quantisation table per component, natural (row-major) order */
+  d3r_jpeg_huff huff[8];           /* DC slots 0..3, then AC slots 0..3 */
+} d3r_jpeg_desc;
+
+#define D3R_JPEG_BAD_CODE 1        /* no Huffman code matches, or a run past coefficient 63 */
+#define D3R_JPEG_SHORT 2           /* a restart interval or the scan ends before (or after) its last block, or not at EOI */
+#define D3R_JPEG_BAD_RESTART 4     /* a restart marker out of sequence, or one without a restart interval */
+#define D3R_JPEG_MARKER_COUNT 8    /* the scan ends before its last restart interval */
+#define D3R_JPEG_RANGE 16          /* a DC value or an IDCT value outside the 16 / 32-bit lanes of Pillow's SIMD IDCT, or an IDCT
+                                      output outside [-512, 511] (where Pillow saturates and libjpeg's C code wraps) */
+
+int32_t d3r_sizeof_jpeg_desc(void);
+int64_t d3r_jpeg_decode_workspace_bytes(const d3r_jpeg_desc* desc, int64_t n_bytes);
+int d3r_jpeg_decode(const d3r_jpeg_desc* desc, const uint8_t* data_dev, int64_t n_bytes, uint8_t* out_dev, int32_t* status_dev,
+                    void* workspace_dev, int64_t workspace_bytes, void* stream);
+
 /* segment_sky (dust3r/viz.py:345-381, behind BasePCOptimizer.mask_sky, dust3r/cloud_opt/base_opt.py:289-295), bit-exact, for
  * n images of any mix of sizes in one call (seven launches whatever the content):
  *   rgb [total_px][3] uint8, image i = pixels [off[i], off[i] + hw[2i] * hw[2i+1]) row-major: the bytes uint8(255 * clip(img, 0, 1))
