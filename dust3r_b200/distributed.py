@@ -13,6 +13,10 @@ the world size; one row gather otherwise).  `PairOutputGather` is the object bot
 `bench.py --gpus N` use; with `async_op=True` it double-buffers so that the gather of step k overlaps the
 forward of step k+1.  Works with backend 'nccl' (GPU) and 'gloo' (CPU tests).
 
+A pair list of several image sizes (portrait and landscape photos) has no fixed row width: `MixedPairOutputGather` packs
+every rank's rows, each of its own pair's size, back to back into one send buffer padded to the largest rank's, and the
+same single all-gather rebuilds inference()'s per-pair lists as views of the gathered buffer.
+
 Global alignment shards the other way round: `global_aligner_sharded` gives every rank a contiguous range of images
 (`shard_images`); each rank streams only those images' observations and the ranks exchange the fixed-point accumulator
 block with one all-reduce per iteration (cloud_opt/engine.py).
@@ -354,14 +358,112 @@ class PairOutputGather:
         return out['pred1'], out['pred2']
 
 
+def row_shapes(pairs):
+    """((H, W) of view 1, (H, W) of view 2) of every row inference() returns for `pairs` -- one row per image of a pair's
+    views, in order -- and the number of rows of every pair."""
+    shapes, pair_rows = [], []
+    for a, b in pairs:
+        k = int(a['img'].shape[0])
+        hw = tuple(tuple(int(s) for s in v['img'].shape[-2:]) for v in (a, b))
+        shapes += [hw] * k
+        pair_rows.append(k)
+    return shapes, pair_rows
+
+
+class MixedPairOutputGather:
+    """The one all-gather of a pair list of several image sizes, whose rows have no common width.
+
+    shapes / pair_rows: what row_shapes returns for the global list; has_conf: as for PairOutputGather.  Rank r computes the
+    pairs shard_bounds(len(pair_rows), world, r).  A row is [pts3d | conf | pts3d_in_other_view | conf], each at its own
+    view's size.  Every rank packs its rows back to back into one fp32 send buffer padded to the largest rank's float count,
+    so rank r's rows start at r * width in the gathered buffer.  Row sizes follow from the pair list alone: every rank
+    computes every rank's count, and no sizes are exchanged."""
+
+    def __init__(self, shapes, pair_rows, has_conf, device, group=None):
+        self.group = group
+        self.world, self.rank = dist.get_world_size(group), dist.get_rank(group)
+        self.shapes = [(tuple(a), tuple(b)) for a, b in shapes]
+        c = 1 if has_conf else 0
+        # (prediction dict, key, channels, side): side 0 = view 1, side 1 = view 2; no conf column without confidences
+        self.cols = [col for col in (('pred1', 'pts3d', 3, 0), ('pred1', 'conf', c, 0),
+                                     ('pred2', 'pts3d_in_other_view', 3, 1), ('pred2', 'conf', c, 1)) if col[2]]
+        first = np.concatenate([[0], np.cumsum(pair_rows, dtype=np.int64)])
+        self.rows = [(int(first[lo]), int(first[hi])) for lo, hi in
+                     (shard_bounds(len(pair_rows), self.world, r) for r in range(self.world))]
+        self.start, self.counts = [], []        # every row's first float within its rank's block; every rank's floats
+        for lo, hi in self.rows:
+            ends = np.cumsum([0] + [self._floats(e) for e in range(lo, hi)], dtype=np.int64)
+            self.start += ends[:-1].tolist()
+            self.counts.append(int(ends[-1]))
+        self.width = max(self.counts)
+        self.device = torch.device(device)
+        self.send = None
+
+    def _layout(self, e):
+        """(prediction dict, key, first float within the row, shape) of every tensor of row e."""
+        out, o = [], 0
+        for which, key, ch, side in self.cols:
+            hw = self.shapes[e][side]
+            out.append((which, key, o, hw + ((3,) if ch == 3 else ())))
+            o += ch * hw[0] * hw[1]
+        return out
+
+    def _floats(self, e):
+        return sum(ch * self.shapes[e][side][0] * self.shapes[e][side][1] for _, _, ch, side in self.cols)
+
+    def pack(self, pred1, pred2):
+        """Copies this rank's rows into the send buffer, one copy per tensor.  pred1 / pred2: the prediction dicts of
+        inference() over this rank's pairs (stacked tensors when they share one size, per-row lists otherwise), None for a
+        rank without pairs."""
+        lo, hi = self.rows[self.rank]
+        self.send = torch.empty((self.width,), dtype=torch.float32, device=self.device)
+        self.send[self.counts[self.rank]:].zero_()
+        if hi == lo:
+            return
+        preds = dict(pred1=pred1, pred2=pred2)
+        layout = [self._layout(e) for e in range(lo, hi)]
+        for k, (which, key, _, _) in enumerate(self.cols):
+            # the packed model's forward names view 2's pointmap 'pts3d' until model.forward() renames it (model.py:199-211)
+            t = preds[which][key] if key in preds[which] else preds[which]['pts3d']
+            if torch.is_tensor(t):      # the rank's rows share one size: one strided copy into every row
+                n, o, shape = hi - lo, layout[0][k][2], layout[0][k][3]
+                size = int(np.prod(shape))
+                rows = self.send[:self.counts[self.rank]].view(n, -1)
+                rows[:, o:o + size].copy_(t.reshape(n, size), non_blocking=True)
+            else:
+                for e in range(lo, hi):
+                    o = self.start[e] + layout[e - lo][k][2]
+                    src = t[e - lo].reshape(-1)
+                    self.send[o:o + src.numel()].copy_(src, non_blocking=True)
+
+    def gather(self, out_device=None):
+        """The one collective; returns (pred1, pred2) with one list entry per row of the global list, each a view of the
+        gathered buffer (moved once to `out_device` when that is another device than the collective's)."""
+        recv = torch.empty((self.world * self.width,), dtype=torch.float32, device=self.device)
+        dist.all_gather_into_tensor(recv, self.send, group=self.group)
+        self.send = None
+        if out_device is not None and torch.device(out_device) != self.device:
+            recv = recv.to(out_device)
+        out = dict(pred1={}, pred2={})
+        for which, key, _, _ in self.cols:
+            out[which][key] = []
+        for r, (lo, hi) in enumerate(self.rows):
+            for e in range(lo, hi):
+                base = r * self.width + self.start[e]
+                for which, key, o, shape in self._layout(e):
+                    out[which][key].append(recv[base + o:base + o + int(np.prod(shape))].view(shape))
+        return out['pred1'], out['pred2']
+
+
 @torch.no_grad()
 def inference_sharded(pairs, model, device, batch_size=8, verbose=False, group=None, gather_device=None, return_images=True,
                       keep='all'):
     """inference() over this rank's slice of `pairs` + ONE collective.
 
-    keep='all': one all-gather -> the full result dict on every rank.  Same return structure as inference(); tensors live
-    on `gather_device` (default: CPU like the reference; pass the CUDA device to keep them resident for global_aligner --
-    they are then views of the gathered buffer).
+    keep='all': one all-gather -> the full result dict on every rank.  Same return structure as inference() (lists with one
+    entry per pair when the list holds several image sizes, MixedPairOutputGather); tensors live on `gather_device`
+    (default: CPU like the reference; pass the CUDA device to keep them resident for global_aligner -- they are then views
+    of the gathered buffer).
 
     keep='owned': the image ranges of global_aligner_sharded (shard_images over the pair graph) are decided before the
     forward, and one all_to_all_single (PairOutputRoute) leaves each rank holding only the rows its images need.  pred1 /
@@ -369,17 +471,16 @@ def inference_sharded(pairs, model, device, batch_size=8, verbose=False, group=N
     (OwnedRows) carries the image ranges and the group size for global_aligner_sharded.  Per rank, device memory peaks at
     its slice's output, one reordered copy of it (NCCL; gloo sends from host memory) and the rows it keeps.
 
-    All pairs must share one image size per view (what make_pairs over load_images(size=...) yields; mixed sizes make
-    inference() return lists, which have no packed row layout).  return_images=False leaves the collated 'img' tensors out
-    of view1 / view2 (2.4 MB per view and pair at 512x384 of pure host copying; the aligner only uses them for colours)."""
+    return_images=False leaves the collated 'img' tensors out of view1 / view2 (2.4 MB per view and pair at 512x384 of pure
+    host copying; the aligner only uses them for colours)."""
     if keep not in ('all', 'owned'):
         raise ValueError(f"keep must be 'all' or 'owned', not {keep!r}")
     if not (dist.is_available() and dist.is_initialized()):
         return inference(pairs, model, device, batch_size=batch_size, verbose=verbose)
     if len(pairs) == 0:
         raise ValueError('inference_sharded: empty pair list')
-    if not check_if_same_size(pairs):
-        raise ValueError('inference_sharded needs all pairs to share one image size per view (run mixed-size pair lists through inference())')
+    # decided from the whole list, as inference() decides it: a rank whose own slice is uniform still returns lists
+    mixed = not check_if_same_size(pairs)
     world, rank = dist.get_world_size(group), dist.get_rank(group)
     if keep == 'owned':
         edges, imshapes = pair_graph(pairs)
@@ -397,10 +498,19 @@ def inference_sharded(pairs, model, device, batch_size=8, verbose=False, group=N
         del local       # the slice output is not needed once it sits in the send buffer
         out_dev = torch.device('cpu') if gather_device is None else torch.device(gather_device)
         p1, p2 = route.exchange(out_dev)
-        view1 = collate_with_cat([drop(a) for a, b in pairs])
-        view2 = collate_with_cat([drop(b) for a, b in pairs])
+        view1 = collate_with_cat([drop(a) for a, b in pairs], lists=mixed)
+        view2 = collate_with_cat([drop(b) for a, b in pairs], lists=mixed)
         return dict(view1=view1, view2=view2, pred1=p1, pred2=p2, loss=None,
                     owned=OwnedRows(shards, world, imshapes, route.allocated))
+    if mixed:
+        shapes, pair_rows = row_shapes(pairs)
+        g = MixedPairOutputGather(shapes, pair_rows, _has_conf(model, local), comm_dev, group=group)
+        g.pack(local['pred1'] if local else None, local['pred2'] if local else None)
+        del local       # the slice output is not needed once it sits in the send buffer
+        p1, p2 = g.gather(torch.device('cpu') if gather_device is None else torch.device(gather_device))
+        view1 = collate_with_cat([drop(a) for a, b in pairs], lists=True)
+        view2 = collate_with_cat([drop(b) for a, b in pairs], lists=True)
+        return dict(view1=view1, view2=view2, pred1=p1, pred2=p2, loss=None)
     # shapes come from each view's own images, so a rank without pairs builds the same row layout as the others
     hw1 = tuple(int(s) for s in pairs[0][0]['img'].shape[-2:])
     hw2 = tuple(int(s) for s in pairs[0][1]['img'].shape[-2:])
