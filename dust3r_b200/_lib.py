@@ -56,8 +56,21 @@ class JpegDesc(C.Structure):
     ]
 
 
+class ViewDesc(C.Structure):
+    """Mirror of `d3r_view_desc` (include/dust3r_b200.h)."""
+    _fields_ = [
+        ('src', C.c_void_p), ('depth', C.c_void_p), ('src_pitch', C.c_int32), ('depth_pitch', C.c_int32),
+        ('H0', C.c_int32), ('W0', C.c_int32), ('H1', C.c_int32), ('W1', C.c_int32), ('crop_x0', C.c_int32), ('crop_y0', C.c_int32),
+        ('H2', C.c_int32), ('W2', C.c_int32), ('row0', C.c_int32), ('rows', C.c_int32), ('transpose', C.c_int32),
+        ('reserved', C.c_int32), ('xbounds', C.c_void_p), ('xcoefs', C.c_void_p), ('ybounds', C.c_void_p), ('ycoefs', C.c_void_p),
+        ('fu', C.c_float), ('fv', C.c_float), ('cu', C.c_float), ('cv', C.c_float), ('pose', C.c_float * 12),
+        ('tmp', C.c_void_p), ('img', C.c_void_p), ('depthmap', C.c_void_p), ('pts3d', C.c_void_p), ('valid', C.c_void_p),
+        ('blocks', C.c_int64 * 3),
+    ]
+
+
 vp, i32, i64, u32, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_float
-_DESC, _MODEL, _JPEG = C.POINTER(AlignDesc), C.POINTER(Model), C.POINTER(JpegDesc)
+_DESC, _MODEL, _JPEG, _VIEW = C.POINTER(AlignDesc), C.POINTER(Model), C.POINTER(JpegDesc), C.POINTER(ViewDesc)
 
 # restype, argtypes of every function include/dust3r_b200.h declares, in its order (tests/test_c_abi.py checks the two agree).
 PROTOTYPES = {
@@ -110,6 +123,8 @@ PROTOTYPES = {
     'd3r_nearest_neighbours': (i32, [i32, i32, vp, vp, vp, vp]),
     'd3r_image_resize_crop_normalize': (i32, [vp, i32, i32, i32, i32, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32,
                                               vp, vp, vp, vp]),
+    'd3r_sizeof_view_desc': (i32, []),
+    'd3r_prepare_views': (i32, [i32, _VIEW, vp, vp, vp]),
     'd3r_sizeof_jpeg_desc': (i32, []),
     'd3r_jpeg_decode_workspace_bytes': (i64, [_JPEG, i64]),
     'd3r_jpeg_decode': (i32, [_JPEG, vp, i64, vp, vp, vp, i64, vp]),

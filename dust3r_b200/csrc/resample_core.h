@@ -77,14 +77,9 @@ struct VerticalArgs {
   float* out;              // [3][H2][W2]
 };
 
-// thread t -> pixel (row y2, column x2) of out, all three channel planes; x2 fastest: a warp reads 96 contiguous bytes of an
-// intermediate row per tap (the coefficient is the same for the whole row: a broadcast load) and writes three coalesced
-// 128-byte lines
-D3R_IMG_HD void vertical_body(long long t, const VerticalArgs& a) {
-  const long long plane = (long long)a.H2 * a.W2;
-  if (t >= plane) return;
-  const int x2 = (int)(t % a.W2);
-  const int y2 = (int)(t / a.W2);
+// The resampled bytes of output pixel (y2, x2), before ImgNorm: the vertical pass of every caller (vertical_body below and the
+// view stage of view_core.h, which stores them elsewhere).  `out` is not read.
+D3R_IMG_HD void vertical_pixel(const VerticalArgs& a, int y2, int x2, uint8_t rgb[3]) {
   const int y1 = a.crop_y0 + y2;
   const int lo = a.bounds[2 * y1] - a.row0, cnt = a.bounds[2 * y1 + 1];
   const int32_t* k = a.coefs + y1;
@@ -98,9 +93,22 @@ D3R_IMG_HD void vertical_body(long long t, const VerticalArgs& a) {
     g += (uint32_t)((int32_t)q[1] * w);
     b += (uint32_t)((int32_t)q[2] * w);
   }
-  a.out[t] = a.lut[clip8(r)];
-  a.out[plane + t] = a.lut[clip8(g)];
-  a.out[2 * plane + t] = a.lut[clip8(b)];
+  rgb[0] = clip8(r);
+  rgb[1] = clip8(g);
+  rgb[2] = clip8(b);
+}
+
+// thread t -> pixel (row y2, column x2) of out, all three channel planes; x2 fastest: a warp reads 96 contiguous bytes of an
+// intermediate row per tap (the coefficient is the same for the whole row: a broadcast load) and writes three coalesced
+// 128-byte lines
+D3R_IMG_HD void vertical_body(long long t, const VerticalArgs& a) {
+  const long long plane = (long long)a.H2 * a.W2;
+  if (t >= plane) return;
+  uint8_t rgb[3];
+  vertical_pixel(a, (int)(t / a.W2), (int)(t % a.W2), rgb);
+  a.out[t] = a.lut[rgb[0]];
+  a.out[plane + t] = a.lut[rgb[1]];
+  a.out[2 * plane + t] = a.lut[rgb[2]];
 }
 
 }  // namespace image

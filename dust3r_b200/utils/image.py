@@ -348,6 +348,13 @@ def norm_lut():
     return torch.arange(256, dtype=torch.uint8).to(torch.float32).div(255).sub_(0.5).div_(0.5)
 
 
+def device_lut(dev):
+    """norm_lut() on `dev`, uploaded once."""
+    if (dev, 'lut') not in _DEVICE_TABLES:
+        _DEVICE_TABLES[(dev, 'lut')] = norm_lut().to(dev)
+    return _DEVICE_TABLES[(dev, 'lut')]
+
+
 @torch.no_grad()
 def preprocess_image_u8(pixels, size, square_ok=False, device='cuda', patch_size=16):
     """Decoded RGB image, uint8 (H, W, 3) numpy array or tensor (host or already on `device`) -> float32 (1, 3, H2, W2) on
@@ -364,9 +371,7 @@ def preprocess_image_u8(pixels, size, square_ok=False, device='cuda', patch_size
     plan = preprocess_plan(h0, w0, size, square_ok, patch_size)
     xb, xk, kx = _device_table(dev, w0, plan['w1'], plan['method'])
     yb, yk, ky = _device_table(dev, h0, plan['h1'], plan['method'])
-    if (dev, 'lut') not in _DEVICE_TABLES:
-        _DEVICE_TABLES[(dev, 'lut')] = norm_lut().to(dev)
-    lut = _DEVICE_TABLES[(dev, 'lut')]
+    lut = device_lut(dev)
     src = src.contiguous().to(dev)
     tmp = torch.empty((plan['rows'], plan['w2'], 3), dtype=torch.uint8, device=dev)
     out = torch.empty((1, 3, plan['h2'], plan['w2']), dtype=torch.float32, device=dev)

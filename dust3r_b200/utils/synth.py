@@ -249,3 +249,45 @@ def synth_criterion_batch(B: int, hw1, hw2, seed: int = 0, invalid: float = 0.2,
     conf2 = 1 + 4 * torch.rand(v2.shape, generator=g)
     return (dict(pts3d=gt1, valid_mask=v1, camera_pose=pose1), dict(pts3d=gt2, valid_mask=v2, camera_pose=pose2),
             dict(pts3d=pr1, conf=conf1), dict(pts3d_in_other_view=pr2, conf=conf2))
+
+
+def synth_rgbd_frame(H: int, W: int, seed: int = 0, pp=None, pose: bool = True):
+    """An RGB-D frame as a dataset hands it to the view stage (dust3r_b200.views): dict(img uint8 (H, W, 3) RGB, depthmap fp32
+    (H, W), camera_intrinsics fp32 3x3 without skew, camera_pose fp32 4x4 camera-to-world, left out with pose=False).  `pp` =
+    the principal point (default within 5 % of the centre).  The depth is a smooth positive field with a patch of zeros and one
+    of negative values (both invalid).  Built from uniform draws with + - * / and sqrt only, so the bytes are the same on every
+    machine and numpy build."""
+    import numpy as np
+    rng = np.random.default_rng([seed, H, W])
+    y, x = np.arange(H, dtype=np.float64)[:, None], np.arange(W, dtype=np.float64)[None, :]
+    u, v = x / max(W - 1, 1), y / max(H - 1, 1)
+    col = rng.random((4, 3)) * 255
+    img = (col[0] * (1 - u[..., None]) * (1 - v[..., None]) + col[1] * u[..., None] * (1 - v[..., None])
+           + col[2] * (1 - u[..., None]) * v[..., None] + col[3] * u[..., None] * v[..., None])
+    for _ in range(4):       # hard edges: saturated rectangles
+        r = rng.random(4)
+        y0, x0 = int(r[0] * H * 0.8), int(r[1] * W * 0.8)
+        img[y0:y0 + 1 + int(r[2] * H * 0.3), x0:x0 + 1 + int(r[3] * W * 0.3)] = (rng.random(3) < 0.5) * 255.0
+    img = img + (rng.random((H, W, 3)) - 0.5) * 24
+    img = np.clip(np.floor(img), 0, 255).astype(np.uint8)
+    a = rng.random(4)
+    depth = 1.0 + 4 * a[0] + 2 * a[1] * u + 3 * a[2] * v * v + a[3] * u * v + 0.01 * rng.random((H, W))
+    r = rng.random(4)
+    depth[int(r[0] * H * 0.7):int(r[0] * H * 0.7) + 1 + H // 8, int(r[1] * W * 0.7):int(r[1] * W * 0.7) + 1 + W // 8] = 0.0
+    depth[int(r[2] * H * 0.7):int(r[2] * H * 0.7) + 1 + H // 10, int(r[3] * W * 0.7):int(r[3] * W * 0.7) + 1 + W // 10] *= -1.0
+    k = rng.random(4)
+    f = (0.7 + 0.8 * k[0]) * max(H, W)
+    cx, cy = pp if pp is not None else (W / 2 + (k[1] - 0.5) * 0.1 * W, H / 2 + (k[2] - 0.5) * 0.1 * H)
+    K = np.array([[f, 0, cx], [0, f * (0.98 + 0.04 * k[3]), cy], [0, 0, 1]], dtype=np.float32)
+    frame = dict(img=img, depthmap=depth.astype(np.float32), camera_intrinsics=K)
+    if pose:
+        q = rng.random(4) * 2 - 1
+        q = q / np.sqrt((q * q).sum())
+        a, b, c, d = q
+        R = [[1 - 2 * (c * c + d * d), 2 * (b * c - a * d), 2 * (b * d + a * c)],
+             [2 * (b * c + a * d), 1 - 2 * (b * b + d * d), 2 * (c * d - a * b)],
+             [2 * (b * d - a * c), 2 * (c * d + a * b), 1 - 2 * (b * b + c * c)]]
+        T = np.eye(4)
+        T[:3, :3], T[:3, 3] = R, rng.random(3) * 4 - 2
+        frame['camera_pose'] = T.astype(np.float32)
+    return frame

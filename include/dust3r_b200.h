@@ -364,6 +364,44 @@ int d3r_image_resize_crop_normalize(const uint8_t* src_dev, int32_t H0, int32_t 
                                     const int32_t* ybounds_dev, const int32_t* ycoefs_dev, int32_t ky, int32_t row0, int32_t rows,
                                     int32_t crop_x0, int32_t crop_y0, int32_t H2, int32_t W2, const float* lut_dev, uint8_t* tmp_dev,
                                     float* out_dev, void* stream);
+/* The view stage of evaluation datasets (dust3r/datasets/base/base_stereo_view_dataset.py `_crop_resize_if_necessary` and
+ * `__getitem__`) for n_views RGB-D frames of any mix of sizes in one call (three launches whatever the batch holds), bit-exact:
+ *   image: the principal-point crop read in place, Pillow's 8-bit resize of it (as d3r_image_resize_crop_normalize), the final
+ *   crop, ImgNorm -> img [3][H2][W2] fp32;
+ *   depth: OpenCV's INTER_NEAREST resize of the same crop (source index min(floor(i * (1.0 / ((double)W1 / W0))), W0 - 1) per
+ *   axis), the final crop -> depthmap [H2][W2] fp32; pts3d [H2][W2][3] fp32 = camera_pose applied (fp32, no fused multiply-add)
+ *   to ((u - cu) * z / fu, (v - cv) * z / fv, z), the first two evaluated in fp64 and rounded once; valid [H2][W2] uint8 =
+ *   z > 0 and the three coordinates finite.
+ * With transpose != 0 (a portrait view) all four outputs are stored transposed: img [3][W2][H2], depthmap [W2][H2], pts3d
+ * [W2][H2][3], valid [W2][H2].  The host plan (dust3r_b200/views.py) computes every field; the call validates the sizes and
+ * windows of `desc` (host memory), uploads it to `desc_dev` (room for n_views descriptors, device memory, alive until the
+ * kernels finish) with the `blocks` fields filled in, and launches.  lut [256] = the fp32 value of every byte after ImgNorm. */
+typedef struct d3r_view_desc {
+  const uint8_t* src;          /* RGB uint8, pixel (0, 0) of the principal-point crop; rows src_pitch pixels apart */
+  const float* depth;          /* depth fp32, pixel (0, 0) of the principal-point crop; rows depth_pitch floats apart */
+  int32_t src_pitch, depth_pitch;
+  int32_t H0, W0;              /* principal-point crop = resize input */
+  int32_t H1, W1;              /* resized size */
+  int32_t crop_x0, crop_y0;    /* final crop window in the resized image */
+  int32_t H2, W2;              /* output size before the landscape transpose */
+  int32_t row0, rows;          /* crop rows the vertical pass reads: the union of the output rows' ybounds */
+  int32_t transpose, reserved;
+  const int32_t* xbounds;      /* [W1][2], xcoefs [kx][W1] tap-major: the Resample.c tables for W0 -> W1 */
+  const int32_t* xcoefs;
+  const int32_t* ybounds;      /* [H1][2], ycoefs [ky][H1] for H0 -> H1 */
+  const int32_t* ycoefs;
+  float fu, fv, cu, cv;        /* final camera intrinsics (before the transpose) */
+  float pose[12];              /* camera-to-world rows [R | t], row-major; NaN when the frame has no pose */
+  uint8_t* tmp;                /* workspace of rows * W2 * 3 bytes */
+  float* img;
+  float* depthmap;
+  float* pts3d;
+  uint8_t* valid;
+  int64_t blocks[3];           /* first 256-thread block of this view in each launch; written by d3r_prepare_views */
+} d3r_view_desc;
+
+int32_t d3r_sizeof_view_desc(void);
+int d3r_prepare_views(int32_t n_views, const d3r_view_desc* desc, d3r_view_desc* desc_dev, const float* lut_dev, void* stream);
 /* Baseline JPEG decode (Pillow's np.asarray(exif_transpose(Image.open(f)).convert('RGB')), bit-exact): sequential Huffman,
  * 8-bit, 1 component or 3 YCbCr components at 4:4:4, 4:2:2 or 4:2:0, any restart interval.  The host parses the header into a
  * d3r_jpeg_desc; the compressed bytes [0, n_bytes) sit in device memory, the entropy-coded scan starts at scan_begin and ends at
