@@ -56,6 +56,14 @@ class JpegDesc(C.Structure):
     ]
 
 
+class PngDesc(C.Structure):
+    """Mirror of `d3r_png_desc` (include/dust3r_b200.h)."""
+    _fields_ = [
+        ('width', C.c_int32), ('height', C.c_int32), ('color_type', C.c_int32), ('orientation', C.c_int32),
+        ('palette_len', C.c_int32), ('reserved', C.c_int32), ('idat_bytes', C.c_int64), ('palette', (C.c_uint8 * 3) * 256),
+    ]
+
+
 class ViewDesc(C.Structure):
     """Mirror of `d3r_view_desc` (include/dust3r_b200.h)."""
     _fields_ = [
@@ -70,7 +78,8 @@ class ViewDesc(C.Structure):
 
 
 vp, i32, i64, u32, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_float
-_DESC, _MODEL, _JPEG, _VIEW = C.POINTER(AlignDesc), C.POINTER(Model), C.POINTER(JpegDesc), C.POINTER(ViewDesc)
+_DESC, _MODEL, _JPEG, _PNG, _VIEW = (C.POINTER(AlignDesc), C.POINTER(Model), C.POINTER(JpegDesc), C.POINTER(PngDesc),
+                                     C.POINTER(ViewDesc))
 
 # restype, argtypes of every function include/dust3r_b200.h declares, in its order (tests/test_c_abi.py checks the two agree).
 PROTOTYPES = {
@@ -128,6 +137,9 @@ PROTOTYPES = {
     'd3r_sizeof_jpeg_desc': (i32, []),
     'd3r_jpeg_decode_workspace_bytes': (i64, [_JPEG, i64]),
     'd3r_jpeg_decode': (i32, [_JPEG, vp, i64, vp, vp, vp, i64, vp]),
+    'd3r_sizeof_png_desc': (i32, []),
+    'd3r_png_decode_workspace_bytes': (i64, [_PNG, i64]),
+    'd3r_png_decode': (i32, [_PNG, vp, i64, vp, vp, vp, i64, vp]),
     'd3r_segment_sky_workspace_bytes': (i64, [i32, i64]),
     'd3r_segment_sky': (i32, [i32, vp, vp, i32, i64, vp, vp, vp, i64, vp]),
     'd3r_nanmedian_workspace_bytes': (i64, [i32]),

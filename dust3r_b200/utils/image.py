@@ -4,8 +4,9 @@ turns normalised tensors back into displayable arrays for the optimizer's `imgs`
 are those of dust3r/utils/image.py:74-128.
 
 `load_images(..., device=None)` is the reference's host path (PIL resize + crop on a CPU core, float image to be uploaded by
-inference()).  `load_images(..., device='cuda')` (SURVEY §8f rank 4) reads each file and parses its header on the host; baseline JPEGs go
-up compressed and are decoded on the H100 (`decode_jpeg`, csrc/jpeg_ops.cu, bit-identical to Pillow), other files are decoded
+inference()).  `load_images(..., device='cuda')` (SURVEY §8f rank 4) reads each file and parses its header on the host; baseline JPEGs and
+8-bit non-interlaced PNGs of at least PNG_DEVICE_MIN_PIXELS go up compressed and are decoded on the H100 (`decode_jpeg`, csrc/jpeg_ops.cu; `decode_png`,
+csrc/png_ops.cu; bit-identical to Pillow), other files are decoded
 by Pillow and their 8-bit RGB pixels go up; then the resize (Pillow's two-pass fixed-point resampling, restated as two integer kernels), the crop and ImgNorm run on the
 H100 (`d3r_image_resize_crop_normalize`, csrc/image_ops.cu) -- bit-identical to the host path, the normalised image is born
 in HBM and inference() uses it in place."""
@@ -100,6 +101,21 @@ def _jpeg_stage(data):
     return jpeg.descriptor(head, orient), jpeg.oriented_size(head, orient), pinned
 
 
+def _png_stage(data):
+    """Host half of decode_png, safe to run on a worker thread: (descriptor, oriented (width, height), pinned zlib stream), or
+    None when the file is outside the device decoder's set (csrc/png_ops.cu)."""
+    from . import png
+    try:
+        head = png.parse(data)
+        orient = png.orientation(head)
+    except png.Unsupported:
+        return None
+    pinned = torch.frombuffer(bytearray(head['idat']), dtype=torch.uint8)
+    if torch.cuda.is_available():
+        pinned = pinned.pin_memory()
+    return png.descriptor(head, orient), png.oriented_size(head, orient), pinned
+
+
 def _jpeg_launch(staged, dev):
     """Uploads the bytes and enqueues the decode on `dev`'s current stream -> (uint8 (H, W, 3) image, int32 status) on `dev`."""
     import ctypes
@@ -117,6 +133,47 @@ def _jpeg_launch(staged, dev):
     _lib.launch(dev, 'd3r_jpeg_decode', ctypes.byref(desc), src.data_ptr(), n, out.data_ptr(), status.data_ptr(), ws.data_ptr(),
                 ws_bytes)
     return out, status
+
+
+def _png_launch(staged, dev):
+    """Uploads the zlib stream and enqueues the decode on `dev`'s current stream -> (uint8 (H, W, 3) image, int32 status) on
+    `dev`."""
+    import ctypes
+    from .. import _lib
+    desc, (w, h), pinned = staged
+    lib = _lib.get_lib()
+    n = int(pinned.numel())
+    ws_bytes = int(lib.d3r_png_decode_workspace_bytes(ctypes.byref(desc), n))
+    if ws_bytes <= 0:
+        raise _lib.D3RError('d3r_png_decode_workspace_bytes rejected the descriptor')
+    src = pinned.to(dev, non_blocking=True)
+    out = torch.empty((h, w, 3), dtype=torch.uint8, device=dev)
+    status = torch.empty((1,), dtype=torch.int32, device=dev)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+    _lib.launch(dev, 'd3r_png_decode', ctypes.byref(desc), src.data_ptr(), n, out.data_ptr(), status.data_ptr(), ws.data_ptr(),
+                ws_bytes)
+    return out, status
+
+
+_PNG_SIGNATURE = b'\x89PNG\r\n\x1a\n'
+# load_images decodes a PNG on the GPU from this many pixels on.  Each GPU decode costs a fixed ~35 ms (one thread per DEFLATE
+# block decodes it, twice) plus ~3.4 ns per pixel end to end; Pillow on 8 worker threads costs ~8.5 ns per pixel end to end
+# (H100 80GB HBM3, 700 W; scripts/png_bench.py, DESIGN.md PNG section): the GPU is faster at 12 Mpx, slower at 1.2 Mpx.
+PNG_DEVICE_MIN_PIXELS = 8_000_000
+
+
+def _device_stage(data):
+    """(launch, staged) of a file the GPU decoders take -- PNGs of at least PNG_DEVICE_MIN_PIXELS by their signature,
+    everything else as a JPEG -- or None."""
+    if data[:8] == _PNG_SIGNATURE:
+        import struct
+        width, height = struct.unpack('>II', data[16:24]) if len(data) >= 24 else (0, 0)
+        if width * height < PNG_DEVICE_MIN_PIXELS:
+            return None
+        staged = _png_stage(data)
+        return None if staged is None else (_png_launch, staged)
+    staged = _jpeg_stage(data)
+    return None if staged is None else (_jpeg_launch, staged)
 
 
 @torch.no_grad()
@@ -139,6 +196,26 @@ def decode_jpeg(data, device='cuda'):
     return torch.from_numpy(_pillow_rgb(data)).to(dev)
 
 
+@torch.no_grad()
+def decode_png(data, device='cuda'):
+    """PNG file contents (bytes) -> uint8 (H, W, 3) RGB tensor on `device`, equal to
+    np.asarray(exif_transpose(PIL.Image.open(f)).convert('RGB')).  Non-interlaced 8-bit files (grey, RGB, palette, grey +
+    alpha, RGBA) are inflated, unfiltered and converted by the GPU kernels of csrc/png_ops.cu; any other file, and any stream
+    those kernels report they cannot reproduce exactly, is decoded by Pillow and uploaded -- the choice is made from the file,
+    so the result is Pillow's either way (including the exception Pillow raises for a broken file)."""
+    from .. import _lib
+    dev = _lib.require_cuda_device(device)
+    if dev.index is None:
+        dev = torch.device('cuda', torch.cuda.current_device())
+    data = bytes(data)
+    staged = _png_stage(data)
+    if staged is not None:
+        img, status = _png_launch(staged, dev)
+        if int(status.item()) == 0:
+            return img
+    return torch.from_numpy(_pillow_rgb(data)).to(dev)
+
+
 def _host_view(pil, size, square_ok, patch_size):
     """The reference's per-image pipeline on a decoded PIL image: resize, centre crop, ImgNorm -> (1, 3, H, W) CPU tensor."""
     w_in, h_in = pil.size
@@ -153,7 +230,8 @@ def _host_view(pil, size, square_ok, patch_size):
 def load_images(folder_or_list, size, square_ok=False, verbose=True, patch_size=16, device=None, workers=None):
     """Folder name or list of file names -> list of dict(img (1,3,H,W) in [-1,1], true_shape int32 [[H,W]], idx,
     instance) ready for make_pairs / inference.  Files that are not .jpg/.jpeg/.png are skipped.
-    device=None: the reference's host pipeline, `img` is a CPU tensor.  device=<an H100>: baseline JPEGs decoded on that GPU
+    device=None: the reference's host pipeline, `img` is a CPU tensor.  device=<an H100>: baseline JPEGs, and 8-bit
+    non-interlaced PNGs of at least PNG_DEVICE_MIN_PIXELS, decoded on that GPU
     (other files, and streams the GPU decoder reports it cannot reproduce, by Pillow), resize / crop / normalise on that GPU
     (same bits), `img` is resident there.
     Files are decoded (device=None: decoded, resized and normalised) by `workers` threads -- PIL releases the GIL in its codecs
@@ -172,9 +250,9 @@ def load_images(folder_or_list, size, square_ok=False, verbose=True, patch_size=
         if device is not None:
             with open(path, 'rb') as f:
                 data = f.read()
-            staged = _jpeg_stage(data)
+            staged = _device_stage(data)
             if staged is not None:              # decoded on the GPU; data kept for the Pillow path if the stream is refused
-                return staged[1], (data, staged)
+                return staged[1][1], (data, staged)
         pil = _open_rgb(path)
         if device is None:
             return pil.size, _host_view(pil, size, square_ok, patch_size)
@@ -214,8 +292,8 @@ def load_images(folder_or_list, size, square_ok=False, verbose=True, patch_size=
             dev = _lib.require_cuda_device(device)
             if dev.index is None:
                 dev = torch.device('cuda', torch.cuda.current_device())
-            data, jpeg_staged = item
-            pixels, status_dev = _jpeg_launch(jpeg_staged, dev)
+            data, (launch, dev_staged) = item
+            pixels, status_dev = launch(dev_staged, dev)
             img = preprocess_image_u8(pixels, size, square_ok, dev, patch_size)
             with torch.cuda.device(dev):
                 status = torch.empty((1,), dtype=torch.int32, pin_memory=True)

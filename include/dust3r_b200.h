@@ -440,6 +440,36 @@ int64_t d3r_jpeg_decode_workspace_bytes(const d3r_jpeg_desc* desc, int64_t n_byt
 int d3r_jpeg_decode(const d3r_jpeg_desc* desc, const uint8_t* data_dev, int64_t n_bytes, uint8_t* out_dev, int32_t* status_dev,
                     void* workspace_dev, int64_t workspace_bytes, void* stream);
 
+/* PNG decode (Pillow's np.asarray(exif_transpose(Image.open(f)).convert('RGB')), bit-exact): non-interlaced, 8-bit samples,
+ * colour type 0 (grey), 2 (RGB), 3 (palette), 4 (grey + alpha) or 6 (RGBA).  The host walks the chunks into a d3r_png_desc and
+ * concatenates every IDAT payload into one zlib stream of n_bytes (== desc->idat_bytes) bytes in device memory.  The stream is
+ * inflated, its Adler-32 checked, the rows unfiltered and converted as convert('RGB') does (grey replicated, alpha dropped,
+ * palette looked up, tRNS ignored).  out = uint8 [H][W][3] RGB after the EXIF orientation (W and H swapped for 5-8).
+ * A stream the kernels cannot reproduce exactly as zlib + Pillow would sets bits of *status_dev (0 = decoded); the call itself
+ * only fails on bad arguments.  Workspace: d3r_png_decode_workspace_bytes(desc, n_bytes) bytes, no initialisation. */
+typedef struct d3r_png_desc {
+  int32_t width, height;           /* image size before the orientation */
+  int32_t color_type;              /* 0, 2, 3, 4 or 6 */
+  int32_t orientation;             /* EXIF orientation 1..8 */
+  int32_t palette_len;             /* PLTE entries (colour type 3: 1..256), 0 otherwise */
+  int32_t reserved;
+  int64_t idat_bytes;              /* bytes of the concatenated IDAT payloads (the zlib stream) */
+  uint8_t palette[256][3];         /* PLTE, RGB; entries past palette_len unused */
+} d3r_png_desc;
+
+#define D3R_PNG_BAD_CODE 1         /* an invalid block header, code-length sequence, Huffman code or stored-block length */
+#define D3R_PNG_FAR 2              /* a distance beyond the output produced so far */
+#define D3R_PNG_SHORT 4            /* the stream ends early, data is left after the last block, the stream inflates to more or
+                                      fewer bytes than the image rows, or it holds more blocks than the workspace records */
+#define D3R_PNG_ADLER 8            /* Adler-32 mismatch */
+#define D3R_PNG_FILTER 16          /* a row filter type above 4 */
+#define D3R_PNG_PALETTE 32         /* a palette index at or past palette_len */
+
+int32_t d3r_sizeof_png_desc(void);
+int64_t d3r_png_decode_workspace_bytes(const d3r_png_desc* desc, int64_t n_bytes);
+int d3r_png_decode(const d3r_png_desc* desc, const uint8_t* zdata_dev, int64_t n_bytes, uint8_t* out_dev, int32_t* status_dev,
+                   void* workspace_dev, int64_t workspace_bytes, void* stream);
+
 /* segment_sky (dust3r/viz.py:345-381, behind BasePCOptimizer.mask_sky, dust3r/cloud_opt/base_opt.py:289-295), bit-exact, for
  * n images of any mix of sizes in one call (seven launches whatever the content):
  *   rgb [total_px][3] uint8, image i = pixels [off[i], off[i] + hw[2i] * hw[2i+1]) row-major: the bytes uint8(255 * clip(img, 0, 1))
