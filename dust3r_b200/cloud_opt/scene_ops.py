@@ -93,7 +93,9 @@ def weiszfeld_focal(pts3d, pp, steps=10):
 
 @torch.no_grad()
 def nearest_neighbours(queries, points):
-    """(N,3), (M,3) CUDA tensors -> (N,) int64 index of the nearest row of `points` for every query."""
+    """(N,3), (M,3) CUDA tensors -> (N,) int64 index of the nearest row of `points` for every query (squared Euclidean distance
+    in fp32, the lowest index on exact ties).  Non-finite input: a point with a NaN coordinate is never chosen, and a query
+    without any finite distance (a NaN query, or every point NaN) gets index 0."""
     dev = queries.device
     _lib.require_cuda_device(dev)
     q, p = _f32(queries).reshape(-1, 3), _f32(points.to(dev)).reshape(-1, 3)

@@ -1,6 +1,7 @@
-"""SURVEY §8f rows as CUDA kernels (csrc/scene_ops.cu) against their host ports (which are pinned against the live reference on
-CPU in tests/test_init_poses.py / test_host_logic.py): clean_pointcloud, weighted Procrustes, Weiszfeld focal, reciprocal
-nearest neighbours."""
+"""SURVEY §8f rows as CUDA kernels (csrc/scene_ops.cu) against their fp32 host ports: clean_pointcloud, weighted Procrustes,
+Weiszfeld focal, reciprocal nearest neighbours.  The host ports of clean_pointcloud and the Weiszfeld focal are pinned against
+the reference (tests/golden/scene_ops.npz) only through the float64 oracle in tests/test_scene_float64_host.py; the element-by-
+element kernel checks against that oracle are in tests/test_scene_float64_gpu.py."""
 import math
 
 import numpy as np
