@@ -77,7 +77,7 @@ class ViewDesc(C.Structure):
     ]
 
 
-vp, i32, i64, u32, f32 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_float
+vp, i32, i64, u32, f32, f64 = C.c_void_p, C.c_int32, C.c_int64, C.c_uint32, C.c_float, C.c_double
 _DESC, _MODEL, _JPEG, _PNG, _VIEW = (C.POINTER(AlignDesc), C.POINTER(Model), C.POINTER(JpegDesc), C.POINTER(PngDesc),
                                      C.POINTER(ViewDesc))
 
@@ -146,6 +146,9 @@ PROTOTYPES = {
     'd3r_segmented_nanmedian': (i32, [i32, i64, vp, vp, vp, i64, vp]),
     'd3r_criterion_workspace_bytes': (i64, [i32, i64, i64, i32]),
     'd3r_criterion': (i32, [i32, i64, i64, i32, i32, f32, f32] + [vp] * 15 + [i64, vp]),
+    'd3r_pnp_ransac_workspace_bytes': (i64, [i32]),
+    'd3r_pnp_ransac': (i32, [i32, vp, vp, f64, f64, f64, f64, f64, f64, i32, i64, vp, i64, vp, vp, vp, vp]),
+    'd3r_pnp_hypotheses': (i32, [i32, vp, vp, f64, f64, f64, f64, f64, i64, i32, i32, vp, vp, vp, vp]),
     # pairwise forward
     'd3r_sizeof_model': (i32, []),
     'd3r_encode_workspace_bytes': (i64, [_MODEL, i32, i32, i32]),

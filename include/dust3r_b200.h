@@ -510,6 +510,25 @@ int d3r_criterion(int32_t B, int64_t n1, int64_t n2, int32_t flags, int32_t redu
                   float* pix1_dev, float* pix2_dev, uint8_t* mask1_dev, uint8_t* mask2_dev, void* workspace_dev,
                   int64_t workspace_bytes, void* stream);
 
+
+/* PnP-RANSAC (dust3r_visloc/localization.py run_pnp: cv2.solvePnPRansac with SOLVEPNP_SQPNP flags up to its final refinement)
+ * on n >= 5 correspondences pts2d_dev fp32 [n][2] (pixels) / pts3d_dev fp32 [n][3] (world), pinhole fx, fy, cx, cy.
+ * OpenCV's loop with 5-point EPnP hypotheses in fp64, its fp32 inlier test (squared reprojection error <= fp32(threshold^2))
+ * and its stopping rule (confidence, at most max_iters hypotheses); the samples come from the counter-based generator of
+ * csrc/pnp_core.h keyed by `seed`.  Device outputs: result_dev int32[4] = {best hypothesis (-1: none), its inlier count,
+ * hypotheses evaluated, 1}; pose_dev fp64[12] = the best hypothesis' R (row-major, world -> camera) and t; mask_dev uint8[n]
+ * its inliers.  workspace_dev: d3r_pnp_ransac_workspace_bytes(max_iters) bytes, 16-byte aligned. */
+int64_t d3r_pnp_ransac_workspace_bytes(int32_t max_iters);
+int d3r_pnp_ransac(int32_t n, const float* pts2d_dev, const float* pts3d_dev, double fx, double fy, double cx, double cy,
+                   double threshold, double confidence, int32_t max_iters, int64_t seed, void* workspace_dev, int64_t workspace_bytes,
+                   int32_t* result_dev, double* pose_dev, uint8_t* mask_dev, void* stream);
+/* Hypotheses h0 .. h0 + n_hyp - 1 of d3r_pnp_ransac's sequence, without the loop: idx_dev int32[n_hyp][5] the samples (-1 when
+ * none could be drawn), pose_dev fp64[n_hyp][12] the EPnP poses (0 when invalid), counts_dev int32[n_hyp] the inlier counts
+ * (-1 when invalid). */
+int d3r_pnp_hypotheses(int32_t n, const float* pts2d_dev, const float* pts3d_dev, double fx, double fy, double cx, double cy,
+                       double threshold, int64_t seed, int32_t h0, int32_t n_hyp, int32_t* idx_dev, double* pose_dev,
+                       int32_t* counts_dev, void* stream);
+
 /* ------------------------------------------------------------------------------------------
  * Path 1 — pairwise forward: replaces AsymmetricCroCo3DStereo.forward (dust3r/model.py:199-211 =
  * _encode_symmetrized :153-170, _decoder :172-191, downstream heads :193-208) as an encode call and a
