@@ -198,6 +198,13 @@ def require_cuda_device(device):
     return dev
 
 
+def cuda_device(device):
+    """require_cuda_device, with a bare 'cuda' resolved to the current device: the device tensors and caches are keyed on."""
+    import torch
+    dev = require_cuda_device(device)
+    return torch.device('cuda', torch.cuda.current_device()) if dev.index is None else dev
+
+
 def launch(device, name, *args):
     """Calls the entry point `name` with `args` and the current stream of `device`, with `device` current, and raises
     D3RError when it fails.  The stream is `device`'s, never the current device's: a scene on cuda:1 runs while cuda:0 is

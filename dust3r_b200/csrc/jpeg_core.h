@@ -31,11 +31,7 @@
 
 #include "../../include/dust3r_b200.h"
 
-#if defined(__CUDACC__)
-#define D3R_JPG_HD __host__ __device__ __forceinline__
-#else
-#define D3R_JPG_HD inline
-#endif
+#include "hd.h"
 
 namespace d3r {
 namespace jpeg {
@@ -65,7 +61,7 @@ __constant__ unsigned char kNaturalDev[64] = D3R_JPEG_NATURAL;
 #endif
 static const unsigned char kNaturalHost[64] = D3R_JPEG_NATURAL;
 
-D3R_JPG_HD int natural(int k) {
+D3R_HD int natural(int k) {
 #if defined(__CUDA_ARCH__)
   return kNaturalDev[k];
 #else
@@ -114,7 +110,7 @@ struct Work {                // workspace pointers
   int* status;
 };
 
-D3R_JPG_HD void flag(int* status, int bit) {
+D3R_HD void flag(int* status, int bit) {
 #if defined(__CUDA_ARCH__)
   atomicOr(status, bit);
 #else
@@ -122,12 +118,12 @@ D3R_JPG_HD void flag(int* status, int bit) {
 #endif
 }
 
-D3R_JPG_HD bool same(const Cursor& a, const Cursor& b) { return a.pos == b.pos && a.unit == b.unit && a.zz == b.zz; }
+D3R_HD bool same(const Cursor& a, const Cursor& b) { return a.pos == b.pos && a.unit == b.unit && a.zz == b.zz; }
 
 // ------------------------------------------------------------------------------------------------ bit reader
 // Up to 8 data bytes from raw byte p, MSB first; returns the number of data bits and leaves in *stop the raw position where it
 // stopped (a marker, or the end of the buffer) when fewer than 64 bits were found.  FF 00 is a data byte FF.
-D3R_JPG_HD int gather(const uint8_t* d, long long n, long long p, uint64_t& w, long long& stop) {
+D3R_HD int gather(const uint8_t* d, long long n, long long p, uint64_t& w, long long& stop) {
   w = 0;
   int nb = 0;
   while (nb < 64) {
@@ -147,7 +143,7 @@ D3R_JPG_HD int gather(const uint8_t* d, long long n, long long p, uint64_t& w, l
 }
 
 // raw position after `k` data bytes starting at the data byte p (all of them inside what gather just read)
-D3R_JPG_HD long long skip_data(const uint8_t* d, long long p, int k) {
+D3R_HD long long skip_data(const uint8_t* d, long long p, int k) {
   for (int i = 0; i < k; ++i) p += d[p] == 0xFF ? 2 : 1;
   return p;
 }
@@ -160,11 +156,11 @@ struct Sink {
 };
 
 // blocks of restart interval s
-D3R_JPG_HD long long seg_len(const Plan& P, long long s) {
+D3R_HD long long seg_len(const Plan& P, long long s) {
   return s < P.nseg - 1 ? P.seg_blocks : P.blocks - (P.nseg - 1) * P.seg_blocks;
 }
 
-D3R_JPG_HD long long sink_block(const Sink& k, const Cursor& c, long long& seg) {
+D3R_HD long long sink_block(const Sink& k, const Cursor& c, long long& seg) {
   seg = k.seg + c.markers;
   const long long inseg = (c.markers == 0 ? k.inseg : 0) + c.blocks;
   if (seg >= k.P->nseg || inseg >= seg_len(*k.P, seg)) return -1;
@@ -172,7 +168,7 @@ D3R_JPG_HD long long sink_block(const Sink& k, const Cursor& c, long long& seg) 
 }
 
 // Decodes from c until its position reaches end_bit (or the scan ends).  Sync passes: sink == nullptr.
-D3R_JPG_HD void run(const Plan& P, const d3r_jpeg_desc& D, const uint8_t* d, Cursor& c, long long end_bit, Sink* sink) {
+D3R_HD void run(const Plan& P, const d3r_jpeg_desc& D, const uint8_t* d, Cursor& c, long long end_bit, Sink* sink) {
   const long long n = P.n_bytes;
   while (c.pos < end_bit) {
     const long long p = c.pos >> 3;
@@ -288,15 +284,15 @@ D3R_JPG_HD void run(const Plan& P, const d3r_jpeg_desc& D, const uint8_t* d, Cur
 }
 
 // raw position of the first marker other than RSTn after the scan start (n_bytes when there is none)
-D3R_JPG_HD long long scan_end(const Plan& P, const Work& w) { return P.n_bytes - (long long)w.ctl[0]; }
+D3R_HD long long scan_end(const Plan& P, const Work& w) { return P.n_bytes - (long long)w.ctl[0]; }
 
 // the last subsequence before the scan end runs until the scan ends, so that the end marker is always checked
-D3R_JPG_HD long long sub_end_bit(const Plan& P, long long se, long long s) {
+D3R_HD long long sub_end_bit(const Plan& P, long long se, long long s) {
   const long long e = P.scan_begin + (s + 1) * kSubBytes;
   return e < se ? e * 8 : kDone;
 }
 
-D3R_JPG_HD void atomic_max(unsigned long long* p, unsigned long long v) {
+D3R_HD void atomic_max(unsigned long long* p, unsigned long long v) {
 #if defined(__CUDA_ARCH__)
   atomicMax(p, v);
 #else
@@ -310,7 +306,7 @@ enum Step { kScanEnd, kPhase1, kUpdate, kRedecode, kFinish, kGroupSum, kGroupSca
 // thread t = bytes [scan_begin + 32 t, + 32): the first FF there that is not stuffing (FF 00) and not RSTn ends the scan.  The
 // second byte of FF 00 or FF Dn is never FF, so every FF the bit reader would stop at is a candidate here, and the earliest one
 // is where it stops.
-D3R_JPG_HD void scan_end_body(long long t, const Plan& P, Work& w) {
+D3R_HD void scan_end_body(long long t, const Plan& P, Work& w) {
   const long long n = P.n_bytes;
   const long long b = P.scan_begin + t * kMarkerScanBytes;
   if (b >= n) return;
@@ -328,7 +324,7 @@ D3R_JPG_HD void scan_end_body(long long t, const Plan& P, Work& w) {
 
 // phase 1: subsequence t from a guessed state (its first data byte, block 0, coefficient 0); subsequence 0 starts exactly there.
 // Subsequences past the end of the scan are finished before they start.
-D3R_JPG_HD void phase1_body(long long t, const Plan& P, Work& w) {
+D3R_HD void phase1_body(long long t, const Plan& P, Work& w) {
   if (t >= P.nsub) return;
   const long long se = scan_end(P, w);
   long long b = P.scan_begin + t * kSubBytes;
@@ -345,7 +341,7 @@ D3R_JPG_HD void phase1_body(long long t, const Plan& P, Work& w) {
 
 // sync round k: subsequence t takes its predecessor's end state; round kSyncRounds only records the first subsequence whose
 // start still disagrees, for the sequential finish
-D3R_JPG_HD void update_body(long long t, int k, const Plan& P, Work& w) {
+D3R_HD void update_body(long long t, int k, const Plan& P, Work& w) {
   if (t >= P.nsub || t == 0) return;
   if (k > 0 && w.changed[k - 1] == 0) return;
   Cursor want = w.end[t - 1];
@@ -365,7 +361,7 @@ D3R_JPG_HD void update_body(long long t, int k, const Plan& P, Work& w) {
 #endif
 }
 
-D3R_JPG_HD void redecode_body(long long t, const Plan& P, Work& w) {
+D3R_HD void redecode_body(long long t, const Plan& P, Work& w) {
   if (t >= P.nsub || !w.dirty[t]) return;
   w.dirty[t] = 0;
   Cursor c = w.start[t];
@@ -375,7 +371,7 @@ D3R_JPG_HD void redecode_body(long long t, const Plan& P, Work& w) {
 
 // one thread (t == 0): from the first inconsistent subsequence on, a sequential decoder that re-decodes a subsequence only where
 // its state differs from the stored start, and otherwise takes the stored end state (decoded from that very start)
-D3R_JPG_HD void finish_body(long long t, const Plan& P, Work& w) {
+D3R_HD void finish_body(long long t, const Plan& P, Work& w) {
   if (t != 0 || w.ctl[1] == 0) return;
   const long long se = scan_end(P, w);
   long long j = P.nsub - (long long)w.ctl[1];
@@ -394,14 +390,14 @@ D3R_JPG_HD void finish_body(long long t, const Plan& P, Work& w) {
 }
 
 // (markers, blocks) of a then b
-D3R_JPG_HD int2 combine(int2 a, int2 b) {
+D3R_HD int2 combine(int2 a, int2 b) {
   int2 r;
   r.x = a.x + b.x;
   r.y = b.x > 0 ? b.y : a.y + b.y;
   return r;
 }
 
-D3R_JPG_HD void group_sum_body(long long t, const Plan& P, Work& w) {
+D3R_HD void group_sum_body(long long t, const Plan& P, Work& w) {
   if (t >= P.ngrp) return;
   int2 acc{0, 0};
   const long long e = (t + 1) * P.grp < P.nsub ? (t + 1) * P.grp : P.nsub;
@@ -410,7 +406,7 @@ D3R_JPG_HD void group_sum_body(long long t, const Plan& P, Work& w) {
 }
 
 // the prefix of the groups before t is folded by every thread (a few hundred broadcast loads), then t's own subsequences
-D3R_JPG_HD void group_scan_body(long long t, const Plan& P, Work& w) {
+D3R_HD void group_scan_body(long long t, const Plan& P, Work& w) {
   if (t >= P.ngrp) return;
   int2 acc{0, 0};
   for (long long g = 0; g < t; ++g) acc = combine(acc, w.grp[g]);
@@ -421,7 +417,7 @@ D3R_JPG_HD void group_scan_body(long long t, const Plan& P, Work& w) {
   }
 }
 
-D3R_JPG_HD void write_body(long long t, const Plan& P, Work& w) {
+D3R_HD void write_body(long long t, const Plan& P, Work& w) {
   if (t >= P.nsub) return;
   Cursor c = w.start[t];
   if (c.pos == kDone) return;
@@ -432,7 +428,7 @@ D3R_JPG_HD void write_body(long long t, const Plan& P, Work& w) {
 }
 
 // DC: per-slice sums after the last restart in the slice, per component
-D3R_JPG_HD void dc_sum_body(long long t, const Plan& P, Work& w) {
+D3R_HD void dc_sum_body(long long t, const Plan& P, Work& w) {
   if (t >= P.ndc) return;
   int4 acc{0, 0, 0, 0};
   const long long m1 = (t + 1) * kDcSliceMcus < P.mcus ? (t + 1) * kDcSliceMcus : P.mcus;
@@ -449,7 +445,7 @@ D3R_JPG_HD void dc_sum_body(long long t, const Plan& P, Work& w) {
   w.dcsum[t] = acc;
 }
 
-D3R_JPG_HD void dc_scan_body(long long t, const Plan& P, Work& w) {
+D3R_HD void dc_scan_body(long long t, const Plan& P, Work& w) {
   if (t >= P.ndc) return;
   long long pred[3] = {0, 0, 0};       // 64-bit: a crafted stream may push a running DC sum far outside 32 bits
   for (long long g = 0; g < t; ++g) {
@@ -476,16 +472,16 @@ D3R_JPG_HD void dc_scan_body(long long t, const Plan& P, Work& w) {
 constexpr long long F0_298 = 2446, F0_390 = 3196, F0_541 = 4433, F0_765 = 6270, F0_899 = 7373, F1_175 = 9633, F1_501 = 12299,
                     F1_847 = 15137, F1_961 = 16069, F2_053 = 16819, F2_562 = 20995, F3_072 = 25172;
 
-D3R_JPG_HD long long descale(long long x, int n) { return (x + (1ll << (n - 1))) >> n; }
+D3R_HD long long descale(long long x, int n) { return (x + (1ll << (n - 1))) >> n; }
 
-D3R_JPG_HD bool fits16(long long v) { return v >= -32768 && v <= 32767; }
-D3R_JPG_HD bool fits32(long long v) { return v >= -2147483648ll && v <= 2147483647ll; }
+D3R_HD bool fits16(long long v) { return v >= -32768 && v <= 32767; }
+D3R_HD bool fits32(long long v) { return v >= -2147483648ll && v <= 2147483647ll; }
 
 // One 8-point pass of jpeg_idct_islow: in[0..7], results descaled by `sh`.  Returns false where the SIMD IDCT Pillow runs
 // (libjpeg-turbo's jidctint-avx2 / -sse2) could differ from this C arithmetic: it forms the pairwise input sums in 16 bits
 // (paddw / psubw, wrapping) and the products and output sums in 32 bits (pmaddwd / paddd, wrapping), so any such value outside
 // those widths is reported instead of restated.
-D3R_JPG_HD bool idct8(const long long* in, long long* out, int sh) {
+D3R_HD bool idct8(const long long* in, long long* out, int sh) {
   bool ok = fits16(in[0] + in[4]) && fits16(in[0] - in[4]) && fits16(in[2] + in[6]) && fits16(in[7] + in[1]) &&
             fits16(in[5] + in[3]) && fits16(in[7] + in[3]) && fits16(in[5] + in[1]) &&
             fits16(in[7] + in[3] + in[5] + in[1]);
@@ -536,7 +532,7 @@ D3R_JPG_HD bool idct8(const long long* in, long long* out, int sh) {
 }
 
 // IDCT_range_limit: the low 10 bits as a signed value, plus 128, clamped
-D3R_JPG_HD uint8_t range_limit(long long x) {
+D3R_HD uint8_t range_limit(long long x) {
   int v = (int)(x & 1023);
   if (v >= 512) v -= 1024;
   v += 128;
@@ -544,7 +540,7 @@ D3R_JPG_HD uint8_t range_limit(long long x) {
 }
 
 // thread t = block t of the scan (MCU-major): dequantise, IDCT, store the 8x8 samples into its component plane
-D3R_JPG_HD void idct_body(long long t, const Plan& P, Work& w) {
+D3R_HD void idct_body(long long t, const Plan& P, Work& w) {
   if (t >= P.blocks) return;
   const long long mcu = t / P.bpm;
   const int u = (int)(t - mcu * P.bpm);
@@ -578,7 +574,7 @@ D3R_JPG_HD void idct_body(long long t, const Plan& P, Work& w) {
 }
 
 // chroma sample at full resolution (x, y) of component c: libjpeg-turbo's fancy upsampling, box upsampling for narrow planes
-D3R_JPG_HD int upsample(const Plan& P, const uint8_t* pl, int c, int x, int y) {
+D3R_HD int upsample(const Plan& P, const uint8_t* pl, int c, int x, int y) {
   const int pw = P.plane_w[c], dw = P.dw[c], dh = P.dh[c];
   const bool h2 = P.h[c] * 2 == P.hmax, v2 = P.v[c] * 2 == P.vmax;
   if (!h2) return pl[(long long)y * pw + x];                 // 4:4:4
@@ -603,10 +599,10 @@ D3R_JPG_HD int upsample(const Plan& P, const uint8_t* pl, int c, int x, int y) {
   return (cs * 3 + r0[i + 1] * 3 + r1[i + 1] + 7) >> 4;
 }
 
-D3R_JPG_HD uint8_t clamp255(int v) { return (uint8_t)(v < 0 ? 0 : (v > 255 ? 255 : v)); }
+D3R_HD uint8_t clamp255(int v) { return (uint8_t)(v < 0 ? 0 : (v > 255 ? 255 : v)); }
 
 // thread t = source pixel (x, y): upsample, ycc_rgb_convert, store at its place after exif_transpose
-D3R_JPG_HD void colour_body(long long t, const Plan& P, Work& w) {
+D3R_HD void colour_body(long long t, const Plan& P, Work& w) {
   if (t >= (long long)P.W * P.H) return;
   const int y = (int)(t / P.W), x = (int)(t - (long long)y * P.W);
   const int Y = w.planes[P.plane_off[0] + (long long)y * P.plane_w[0] + x];
@@ -637,7 +633,7 @@ D3R_JPG_HD void colour_body(long long t, const Plan& P, Work& w) {
 }
 
 template <int S>
-D3R_JPG_HD void step(long long t, int k, const Plan& P, Work& w) {
+D3R_HD void step(long long t, int k, const Plan& P, Work& w) {
   if (S == kScanEnd) scan_end_body(t, P, w);
   else if (S == kPhase1) phase1_body(t, P, w);
   else if (S == kUpdate) update_body(t, k, P, w);
@@ -788,6 +784,29 @@ void decode(L& l, const Plan& P, const Layout& lay, Work& w, const d3r_jpeg_desc
   l.template launch<kIdct>(P.blocks, 0, P, w);
   l.template launch<kColour>((long long)P.W * P.H, 0, P, w);
 }
+
+// What the step-decoder launchers (csrc/step_decode.cuh, tests/native/step_host.h) need of this codec
+struct Codec {
+  using Desc = d3r_jpeg_desc;
+  using Plan = jpeg::Plan;
+  using Work = jpeg::Work;
+  using Layout = jpeg::Layout;
+  static constexpr const char* kEntry = "d3r_jpeg_decode";
+  static constexpr const char* kTag = "jpeg_decode";
+  static constexpr const uint8_t* Work::*kInput = &Work::data;
+  static const char* make_plan(const Desc& D, long long n_bytes, Plan& P) { return jpeg::make_plan(D, n_bytes, P); }
+  template <class L>
+  static void decode(L& l, const Plan& P, const Layout& lay, Work& w, const Desc& desc, char* ws) {
+    jpeg::decode(l, P, lay, w, desc, ws);
+  }
+  template <int S>
+  D3R_HD static void step(long long t, int k, const Plan& P, Work& w) { jpeg::step<S>(t, k, P, w); }
+  // compulsory traffic: the compressed bytes (read about three times), coefficients out and in, planes out and in, RGB out
+  static double traffic(const Plan& P, long long n_bytes) {
+    return 3.0 * double(n_bytes) + 2.0 * 132.0 * double(P.blocks) + 3.0 * double(P.W) * P.H * (P.ncomp == 3 ? 2 : 1);
+  }
+  static int launches(const Plan&) { return 2 * kSyncRounds + 12; }
+};
 
 }  // namespace jpeg
 }  // namespace d3r

@@ -34,13 +34,7 @@
 
 #include "../../include/dust3r_b200.h"
 
-#if defined(__CUDACC__)
-#define D3R_PNG_HD __host__ __device__ __forceinline__
-#define D3R_PNG_UNROLL _Pragma("unroll")
-#else
-#define D3R_PNG_HD inline
-#define D3R_PNG_UNROLL
-#endif
+#include "hd.h"
 
 namespace d3r {
 namespace png {
@@ -64,7 +58,7 @@ __constant__ unsigned char kClenOrderDev[19] = D3R_PNG_CLEN_ORDER;
 #endif
 static const unsigned char kClenOrderHost[19] = D3R_PNG_CLEN_ORDER;
 
-D3R_PNG_HD int clen_order(int i) {
+D3R_HD int clen_order(int i) {
 #if defined(__CUDA_ARCH__)
   return kClenOrderDev[i];
 #else
@@ -110,7 +104,7 @@ struct Work {                        // workspace pointers
   int* status;
 };
 
-D3R_PNG_HD void flag(int* status, int bit) {
+D3R_HD void flag(int* status, int bit) {
 #if defined(__CUDA_ARCH__)
   atomicOr(status, bit);
 #else
@@ -118,7 +112,7 @@ D3R_PNG_HD void flag(int* status, int bit) {
 #endif
 }
 
-D3R_PNG_HD int status_of(const Work& w) {
+D3R_HD int status_of(const Work& w) {
 #if defined(__CUDA_ARCH__)
   return *(volatile int*)w.status;
 #else
@@ -133,7 +127,7 @@ struct Bits {
   long long n, next;                // stream bytes, next byte to load
   uint64_t buf;
   int cnt;
-  D3R_PNG_HD void init(const uint8_t* data, long long n_bytes, long long bit) {
+  D3R_HD void init(const uint8_t* data, long long n_bytes, long long bit) {
     d = data;
     n = n_bytes;
     next = bit >> 3;
@@ -142,7 +136,7 @@ struct Bits {
     refill();
     drop((int)(bit & 7));
   }
-  D3R_PNG_HD void refill() {
+  D3R_HD void refill() {
     if (cnt > 56) return;
     if (next >= 0 && next + 8 <= n) {                         // whole bytes that fit, from eight independent loads
       uint64_t v = 0;
@@ -160,25 +154,25 @@ struct Bits {
       cnt += 8;
     }
   }
-  D3R_PNG_HD unsigned peek(int k) const { return (unsigned)(buf & ((1ull << k) - 1)); }
-  D3R_PNG_HD void drop(int k) {
+  D3R_HD unsigned peek(int k) const { return (unsigned)(buf & ((1ull << k) - 1)); }
+  D3R_HD void drop(int k) {
     buf >>= k;
     cnt -= k;
   }
-  D3R_PNG_HD unsigned get(int k) {      // k <= 32
+  D3R_HD unsigned get(int k) {      // k <= 32
     refill();
     const unsigned v = peek(k);
     drop(k);
     return v;
   }
-  D3R_PNG_HD long long pos() const { return next * 8 - cnt; }
-  D3R_PNG_HD bool over() const { return pos() > n * 8; }
+  D3R_HD long long pos() const { return next * 8 - cnt; }
+  D3R_HD bool over() const { return pos() > n * 8; }
 };
 
 // ------------------------------------------------------------------------------------------------ Huffman codes
 // Kraft sum of n code lengths (0 = unused): 0 complete, 1 a single code of length 1 (the only incomplete code zlib accepts for
 // literal/length and distance codes), 2 no code at all, -1 over-subscribed, -2 incomplete otherwise.
-D3R_PNG_HD int kraft(const uint8_t* len, int n, uint16_t* count) {
+D3R_HD int kraft(const uint8_t* len, int n, uint16_t* count) {
   for (int l = 0; l < 16; ++l) count[l] = 0;
   for (int i = 0; i < n; ++i) count[len[i]]++;
   if (count[0] == n) return 2;
@@ -202,14 +196,14 @@ struct Huff {
   uint16_t sym[N];
 };
 
-D3R_PNG_HD unsigned reverse_bits(unsigned c, int l) {
+D3R_HD unsigned reverse_bits(unsigned c, int l) {
   unsigned r = 0;
   for (int i = 0; i < l; ++i) r |= ((c >> i) & 1u) << (l - 1 - i);
   return r;
 }
 
 template <int B, int N>
-D3R_PNG_HD int build(Huff<B, N>& h, const uint8_t* len, int n) {
+D3R_HD int build(Huff<B, N>& h, const uint8_t* len, int n) {
   const int k = kraft(len, n, h.count);
   if (k < 0) return k;
   uint16_t offs[16];
@@ -232,7 +226,7 @@ D3R_PNG_HD int build(Huff<B, N>& h, const uint8_t* len, int n) {
 
 // next symbol, or -1 where no code matches
 template <int B, int N>
-D3R_PNG_HD int decode_sym(Bits& b, const Huff<B, N>& h) {
+D3R_HD int decode_sym(Bits& b, const Huff<B, N>& h) {
   b.refill();
   const unsigned e = h.fast[b.peek(B)];
   if (e) {
@@ -260,7 +254,7 @@ typedef Huff<kDistBits, 32> DistHuff;
 typedef Huff<7, 19> ClenHuff;
 
 // Reads a dynamic block header from HLIT on into lens[0, nlit + ndist); 0, or kBadCode where zlib's inflate would stop.
-D3R_PNG_HD int read_dynamic(Bits& b, uint8_t* lens, int& nlit, int& ndist) {
+D3R_HD int read_dynamic(Bits& b, uint8_t* lens, int& nlit, int& ndist) {
   nlit = (int)b.get(5) + 257;
   ndist = (int)b.get(5) + 1;
   const int ncode = (int)b.get(4) + 4;
@@ -305,7 +299,7 @@ struct Sink {
   int* status;
 };
 
-D3R_PNG_HD long long length_base(int i, int& extra) {   // literal/length symbol 257 + i
+D3R_HD long long length_base(int i, int& extra) {   // literal/length symbol 257 + i
   if (i < 8) {
     extra = 0;
     return 3 + i;
@@ -318,7 +312,7 @@ D3R_PNG_HD long long length_base(int i, int& extra) {   // literal/length symbol
   return ((long long)(4 + (i & 3)) << extra) + 3;
 }
 
-D3R_PNG_HD long long dist_base(int d, int& extra) {
+D3R_HD long long dist_base(int d, int& extra) {
   if (d < 4) {
     extra = 0;
     return d + 1;
@@ -329,7 +323,7 @@ D3R_PNG_HD long long dist_base(int d, int& extra) {
 
 // Decodes the block whose 3-bit header starts at bit p.  Without a sink it only measures (end, length, last-block flag, errors);
 // `limit` bounds the length (a block inflating to more than the image cannot be part of a valid stream).
-D3R_PNG_HD Block inflate_block(const uint8_t* z, long long n, long long p, long long limit, const Sink* sink) {
+D3R_HD Block inflate_block(const uint8_t* z, long long n, long long p, long long limit, const Sink* sink) {
   Block r{p, p, 0, 0, 0};
   Bits b;
   b.init(z, n, p);
@@ -447,13 +441,13 @@ D3R_PNG_HD Block inflate_block(const uint8_t* z, long long n, long long p, long 
 }
 
 // Header bits BFINAL, BTYPE = 2, HLIT <= 29, HDIST <= 29: the cheap first test of a candidate
-D3R_PNG_HD bool dynamic_head(unsigned head) {
+D3R_HD bool dynamic_head(unsigned head) {
   return ((head >> 1) & 3) == 2 && ((head >> 3) & 31) <= 29 && ((head >> 8) & 31) <= 29;
 }
 
 // Full candidate test for a dynamic block header at bit p whose first 13 bits passed dynamic_head (stricter than zlib: both
 // codes complete, or one distance code)
-D3R_PNG_HD bool dynamic_candidate(const uint8_t* z, long long n, long long p) {
+D3R_HD bool dynamic_candidate(const uint8_t* z, long long n, long long p) {
   Bits b;
   b.init(z, n, p);
   b.drop(13);
@@ -474,7 +468,7 @@ D3R_PNG_HD bool dynamic_candidate(const uint8_t* z, long long n, long long p) {
   return kd == 0 || kd == 1;
 }
 
-D3R_PNG_HD void mark(uint32_t* cand, long long bit) {
+D3R_HD void mark(uint32_t* cand, long long bit) {
 #if defined(__CUDA_ARCH__)
   atomicOr(cand + (bit >> 5), 1u << (bit & 31));
 #else
@@ -482,7 +476,7 @@ D3R_PNG_HD void mark(uint32_t* cand, long long bit) {
 #endif
 }
 
-D3R_PNG_HD void atomic_inc(unsigned long long* p, unsigned long long& old) {
+D3R_HD void atomic_inc(unsigned long long* p, unsigned long long& old) {
 #if defined(__CUDA_ARCH__)
   old = atomicAdd(p, 1ull);
 #else
@@ -494,7 +488,7 @@ D3R_PNG_HD void atomic_inc(unsigned long long* p, unsigned long long& old) {
 enum Step { kCand, kSpec, kChain, kWrite, kJump, kGather, kAdlerPart, kAdlerSum, kRows };
 
 // thread t = stream byte t: its 8 bit offsets as dynamic headers, and t as the LEN of a stored block
-D3R_PNG_HD void cand_body(long long t, const Plan& P, Work& w) {
+D3R_HD void cand_body(long long t, const Plan& P, Work& w) {
   if (t >= P.n_bytes) return;
   unsigned win = 0;
   for (int i = 0; i < 3; ++i) win |= (unsigned)(t + i < P.n_bytes ? w.z[t + i] : 0) << (8 * i);
@@ -513,7 +507,7 @@ D3R_PNG_HD void cand_body(long long t, const Plan& P, Work& w) {
 }
 
 // thread t = subsequence t: the block of every candidate in it, in stream order, up to kSlots
-D3R_PNG_HD void spec_body(long long t, const Plan& P, Work& w) {
+D3R_HD void spec_body(long long t, const Plan& P, Work& w) {
   if (t >= P.nsub) return;
   const long long w0 = t * (kSubBytes / 4), w1 = w0 + kSubBytes / 4 < P.n_bytes / 4 + 1 ? w0 + kSubBytes / 4 : P.n_bytes / 4 + 1;
   int k = 0;
@@ -530,7 +524,7 @@ D3R_PNG_HD void spec_body(long long t, const Plan& P, Work& w) {
 }
 
 // one thread: the true block chain from bit 16, each block's output offset, the zlib trailer
-D3R_PNG_HD void chain_body(long long t, const Plan& P, Work& w) {
+D3R_HD void chain_body(long long t, const Plan& P, Work& w) {
   if (t != 0) return;
   long long p = 16, off = 0, nb = 0;
   int err = 0;
@@ -577,7 +571,7 @@ D3R_PNG_HD void chain_body(long long t, const Plan& P, Work& w) {
 }
 
 // thread t = block t of the chain, decoded into place
-D3R_PNG_HD void write_body(long long t, const Plan& P, Work& w) {
+D3R_HD void write_body(long long t, const Plan& P, Work& w) {
   if (t >= (long long)w.ctl[0] || status_of(w)) return;
   const Link l = w.chain[t];
   Sink k{w.raw, w.src, l.out_off, P.total, w.status};
@@ -585,7 +579,7 @@ D3R_PNG_HD void write_body(long long t, const Plan& P, Work& w) {
 }
 
 // round k of pointer jumping, in place (a concurrent update only ever shortens the path a thread reads)
-D3R_PNG_HD void jump_body(long long t, int k, const Plan& P, Work& w) {
+D3R_HD void jump_body(long long t, int k, const Plan& P, Work& w) {
   if (t >= P.total || status_of(w)) return;
   if (k > 0 && w.changed[k - 1] == 0) return;
   const int s = w.src[t];
@@ -596,7 +590,7 @@ D3R_PNG_HD void jump_body(long long t, int k, const Plan& P, Work& w) {
   w.changed[k] = 1;
 }
 
-D3R_PNG_HD void gather_body(long long t, const Plan& P, Work& w) {
+D3R_HD void gather_body(long long t, const Plan& P, Work& w) {
   if (t >= P.total || status_of(w)) return;
   const int s = w.src[t];
   if (s != (int)t) w.raw[t] = w.raw[s];
@@ -605,7 +599,7 @@ D3R_PNG_HD void gather_body(long long t, const Plan& P, Work& w) {
 constexpr unsigned kAdlerMod = 65521;
 
 // thread t = segment t: (sum of bytes, sum of (bytes left in the segment) * byte), both mod 65521
-D3R_PNG_HD void adler_part_body(long long t, const Plan& P, Work& w) {
+D3R_HD void adler_part_body(long long t, const Plan& P, Work& w) {
   if (t >= P.nseg || status_of(w)) return;
   const long long b = t * kAdlerSeg, e = b + kAdlerSeg < P.total ? b + kAdlerSeg : P.total;
   unsigned long long s1 = 0, s2 = 0;
@@ -616,7 +610,7 @@ D3R_PNG_HD void adler_part_body(long long t, const Plan& P, Work& w) {
   w.adler[t] = (s1 % kAdlerMod) | (s2 % kAdlerMod) << 32;
 }
 
-D3R_PNG_HD void adler_sum_body(long long t, const Plan& P, Work& w) {
+D3R_HD void adler_sum_body(long long t, const Plan& P, Work& w) {
   if (t != 0 || status_of(w)) return;
   unsigned long long a = 1, b = 0;
   for (long long s = 0; s < P.nseg; ++s) {
@@ -628,7 +622,7 @@ D3R_PNG_HD void adler_sum_body(long long t, const Plan& P, Work& w) {
   if (((b << 16) | a) != w.ctl[2]) flag(w.status, kAdler);
 }
 
-D3R_PNG_HD int wait_progress(const int* p, int need) {
+D3R_HD int wait_progress(const int* p, int need) {
 #if defined(__CUDA_ARCH__)
   int v;
   while ((v = *(const volatile int*)p) < need) __nanosleep(64);
@@ -640,7 +634,7 @@ D3R_PNG_HD int wait_progress(const int* p, int need) {
 #endif
 }
 
-D3R_PNG_HD void publish(int* p, int v) {
+D3R_HD void publish(int* p, int v) {
 #if defined(__CUDA_ARCH__)
   __threadfence();
   *(volatile int*)p = v;
@@ -649,7 +643,7 @@ D3R_PNG_HD void publish(int* p, int v) {
 #endif
 }
 
-D3R_PNG_HD uint8_t load_above(const uint8_t* p) {      // a byte another thread unfiltered: read past L1
+D3R_HD uint8_t load_above(const uint8_t* p) {      // a byte another thread unfiltered: read past L1
 #if defined(__CUDA_ARCH__)
   return __ldcg(p);
 #else
@@ -657,14 +651,14 @@ D3R_PNG_HD uint8_t load_above(const uint8_t* p) {      // a byte another thread 
 #endif
 }
 
-D3R_PNG_HD int paeth(int a, int b, int c) {
+D3R_HD int paeth(int a, int b, int c) {
   const int p = a + b - c;
   const int pa = p > a ? p - a : a - p, pb = p > b ? p - b : b - p, pc = p > c ? p - c : c - p;
   if (pa <= pb && pa <= pc) return a;
   return pb <= pc ? b : c;
 }
 
-D3R_PNG_HD int orient_index(const Plan& P, int x, int y, int& oy) {
+D3R_HD int orient_index(const Plan& P, int x, int y, int& oy) {
   const int W = P.W, H = P.H;
   int ox = x;
   oy = y;
@@ -685,7 +679,7 @@ D3R_PNG_HD int orient_index(const Plan& P, int x, int y, int& oy) {
 // loaded together, unfiltered from registers, converted to RGB and stored at their oriented places, then the row's progress is
 // published.  Only Up, Average and Paeth rows read the row above, so only they wait for it.
 template <int BPP>
-D3R_PNG_HD void unfilter_row(long long y, const Plan& P, Work& w) {
+D3R_HD void unfilter_row(long long y, const Plan& P, Work& w) {
   uint8_t* cur = w.raw + y * P.row_bytes + 1;
   const int f = cur[-1];
   const uint8_t* up = y > 0 ? cur - P.row_bytes : nullptr;
@@ -704,14 +698,14 @@ D3R_PNG_HD void unfilter_row(long long y, const Plan& P, Work& w) {
     if (reads_up && x0 + nx > ready) ready = wait_progress(w.progress + y - 1, x0 + nx);
     const long long base = (long long)x0 * BPP;
     int a[kRowStep * BPP], b[kRowStep * BPP];
-D3R_PNG_UNROLL
+D3R_UNROLL
     for (int i = 0; i < kRowStep * BPP; ++i) {
       a[i] = i < nx * BPP ? cur[base + i] : 0;
       b[i] = reads_up && i < nx * BPP ? load_above(up + base + i) : 0;
     }
-D3R_PNG_UNROLL
+D3R_UNROLL
     for (int px = 0; px < kRowStep; ++px) {
-D3R_PNG_UNROLL
+D3R_UNROLL
       for (int c = 0; c < BPP; ++c) {
         const int i = px * BPP + c;
         int v = a[i];
@@ -725,11 +719,11 @@ D3R_PNG_UNROLL
         upleft[c] = b[i];
       }
     }
-D3R_PNG_UNROLL
+D3R_UNROLL
     for (int px = 0; px < kRowStep; ++px) {
       if (px >= nx) break;
       const int x = x0 + px;
-D3R_PNG_UNROLL
+D3R_UNROLL
       for (int c = 0; c < BPP; ++c) cur[base + px * BPP + c] = (uint8_t)a[px * BPP + c];
       int R, G, B;
       if (P.color == 3) {
@@ -762,7 +756,7 @@ D3R_PNG_UNROLL
 
 // wavefront: lane 0 of every warp claims rows in order (the row above was claimed by a warp that is already running, so every
 // wait ends) and works through them; the other lanes leave at once, so no lane spins against another of its own warp
-D3R_PNG_HD void rows_body(long long t, const Plan& P, Work& w) {
+D3R_HD void rows_body(long long t, const Plan& P, Work& w) {
   if ((t & 31) || (t >> 5) >= kRowWarps || status_of(w)) return;
   for (;;) {
     unsigned long long y;
@@ -776,7 +770,7 @@ D3R_PNG_HD void rows_body(long long t, const Plan& P, Work& w) {
 }
 
 template <int S>
-D3R_PNG_HD void step(long long t, int k, const Plan& P, Work& w) {
+D3R_HD void step(long long t, int k, const Plan& P, Work& w) {
   if (S == kCand) cand_body(t, P, w);
   else if (S == kSpec) spec_body(t, P, w);
   else if (S == kChain) chain_body(t, P, w);
@@ -882,6 +876,30 @@ void decode(L& l, const Plan& P, const Layout& lay, Work& w, const d3r_png_desc&
   l.template launch<kAdlerSum>(1, 0, P, w);
   l.template launch<kRows>(32ll * (P.H < kRowWarps ? P.H : kRowWarps), 0, P, w);
 }
+
+// What the step-decoder launchers (csrc/step_decode.cuh, tests/native/step_host.h) need of this codec
+struct Codec {
+  using Desc = d3r_png_desc;
+  using Plan = png::Plan;
+  using Work = png::Work;
+  using Layout = png::Layout;
+  static constexpr const char* kEntry = "d3r_png_decode";
+  static constexpr const char* kTag = "png_decode";
+  static constexpr const uint8_t* Work::*kInput = &Work::z;
+  static const char* make_plan(const Desc& D, long long n_bytes, Plan& P) { return png::make_plan(D, n_bytes, P); }
+  template <class L>
+  static void decode(L& l, const Plan& P, const Layout& lay, Work& w, const Desc& desc, char* ws) {
+    png::decode(l, P, lay, w, desc, ws);
+  }
+  template <int S>
+  D3R_HD static void step(long long t, int k, const Plan& P, Work& w) { png::step<S>(t, k, P, w); }
+  // compulsory traffic: the stream (read about three times), the inflated rows and their roots written, read and written
+  // again, the RGB out
+  static double traffic(const Plan& P, long long n_bytes) {
+    return 3.0 * double(n_bytes) + 4.0 * double(P.total) + 8.0 * double(P.total) + 3.0 * double(P.W) * P.H;
+  }
+  static int launches(const Plan& P) { return P.rounds + 8; }
+};
 
 }  // namespace png
 }  // namespace d3r

@@ -34,13 +34,7 @@
 #include <math.h>
 #include <stdint.h>
 
-#if defined(__CUDACC__)
-#define D3R_PNP_HD __host__ __device__ __forceinline__
-#define D3R_PNP_SUB __host__ __device__ __noinline__   // the EPnP stages: separate register allocations, no spills
-#else
-#define D3R_PNP_HD inline
-#define D3R_PNP_SUB inline
-#endif
+#include "hd.h"
 
 namespace d3r {
 namespace pnp {
@@ -52,37 +46,22 @@ constexpr int kGaussNewton = 5;      // Gauss-Newton steps per beta estimate (ep
 constexpr double kFlat = 1e-30;      // PCA eigenvalue ratio below which a direction is flat (OpenCV inverts all but exact 0)
 constexpr uint64_t kDefaultSeed = 0x5DEECE66Dull;
 
-// ---- explicitly rounded arithmetic (no FMA contraction on either side) ----
-#if defined(__CUDA_ARCH__)
-D3R_PNP_HD double dmul(double a, double b) { return __dmul_rn(a, b); }
-D3R_PNP_HD double dadd(double a, double b) { return __dadd_rn(a, b); }
-D3R_PNP_HD float fmul(float a, float b) { return __fmul_rn(a, b); }
-D3R_PNP_HD float fadd(float a, float b) { return __fadd_rn(a, b); }
-D3R_PNP_HD float fsub(float a, float b) { return __fsub_rn(a, b); }
-#else
-D3R_PNP_HD double dmul(double a, double b) { return a * b; }
-D3R_PNP_HD double dadd(double a, double b) { return a + b; }
-D3R_PNP_HD float fmul(float a, float b) { return a * b; }
-D3R_PNP_HD float fadd(float a, float b) { return a + b; }
-D3R_PNP_HD float fsub(float a, float b) { return a - b; }
-#endif
-
 // ---- sample draws ----
-D3R_PNP_HD uint64_t mix64(uint64_t z) {
+D3R_HD uint64_t mix64(uint64_t z) {
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
   z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
   return z ^ (z >> 31);
 }
 
-D3R_PNP_HD uint32_t draw(uint64_t seed, uint32_t h, uint32_t k, uint32_t n) {
+D3R_HD uint32_t draw(uint64_t seed, uint32_t h, uint32_t k, uint32_t n) {
   const uint64_t z = mix64(seed + 0x9E3779B97F4A7C15ull * ((((uint64_t)h) << 32 | k) + 1ull));
   return (uint32_t)(((z >> 32) * (uint64_t)n) >> 32);
 }
 
 // the 5 indices of hypothesis h (draw order); false when kMaxDraws draws did not give 5 distinct ones
-D3R_PNP_HD bool sample(uint64_t seed, uint32_t h, uint32_t n, int32_t idx[kSample]) {
+D3R_HD bool sample(uint64_t seed, uint32_t h, uint32_t n, int32_t idx[kSample]) {
   if (n == (uint32_t)kSample) {
-#pragma unroll
+D3R_UNROLL
     for (int j = 0; j < kSample; ++j) idx[j] = j;
     return true;
   }
@@ -90,10 +69,10 @@ D3R_PNP_HD bool sample(uint64_t seed, uint32_t h, uint32_t n, int32_t idx[kSampl
   for (uint32_t k = 0; k < (uint32_t)kMaxDraws && m < kSample; ++k) {
     const int32_t i = (int32_t)draw(seed, h, k, n);
     bool dup = false;
-#pragma unroll
+D3R_UNROLL
     for (int j = 0; j < kSample; ++j) dup |= (j < m) && idx[j] == i;
     if (!dup) {
-#pragma unroll
+D3R_UNROLL
       for (int j = 0; j < kSample; ++j)
         if (j == m) idx[j] = i;
       ++m;
@@ -107,7 +86,7 @@ D3R_PNP_HD bool sample(uint64_t seed, uint32_t h, uint32_t n, int32_t idx[kSampl
 struct Scratch {
   double* p;
   int stride;
-  D3R_PNP_HD double& operator()(int k) const { return p[(long long)k * stride]; }
+  D3R_HD double& operator()(int k) const { return p[(long long)k * stride]; }
 };
 
 enum : int {
@@ -132,10 +111,12 @@ enum : int {
   kScratch = kBest + 12
 };
 
+// The EPnP stages below are D3R_HD_NOINLINE: separate register allocations, no spills.
+
 // cyclic Jacobi on the n x n symmetric matrix at s(kA): eigenvalues on its diagonal, eigenvectors in the columns of s(kV).
 // Rotations as in Numerical Recipes' jacobi: after 4 sweeps an element negligible against both diagonal entries is set to
 // 0; the loop ends when every off-diagonal element is 0 (or a NaN appeared).
-D3R_PNP_SUB void jacobi(Scratch s, int n) {
+D3R_HD_NOINLINE void jacobi(Scratch s, int n) {
   for (int i = 0; i < n; ++i)
     for (int j = 0; j < n; ++j) s(kV + i * n + j) = i == j ? 1.0 : 0.0;
   for (int sweep = 0; sweep < kJacobiSweeps; ++sweep) {
@@ -181,7 +162,7 @@ D3R_PNP_SUB void jacobi(Scratch s, int n) {
 
 // least squares min |Q x - rhs| for the 6 x ncol matrix at s(kQ) (row stride 5) by Householder QR; x at s(kX).  False when a
 // column is (numerically) dependent on the previous ones.
-D3R_PNP_SUB bool lsq6(Scratch s, int ncol) {
+D3R_HD_NOINLINE bool lsq6(Scratch s, int ncol) {
   for (int k = 0; k < ncol; ++k) {
     double nrm = 0.0;
     for (int i = k; i < 6; ++i) nrm += s(kQ + i * 5 + k) * s(kQ + i * 5 + k);
@@ -213,13 +194,13 @@ D3R_PNP_SUB bool lsq6(Scratch s, int ncol) {
 }
 
 // the pairs of control points, in epnp.cpp's order
-D3R_PNP_HD void pair_of(int k, int& a, int& b) {
+D3R_HD void pair_of(int k, int& a, int& b) {
   a = k < 3 ? 0 : (k < 5 ? 1 : 2);
   b = k < 3 ? k + 1 : (k < 5 ? k - 1 : 3);
 }
 
 // Gauss-Newton on the 6 distance equations from the betas at s(kBeta) (epnp.cpp: compute_A_and_b_gauss_newton, qr_solve)
-D3R_PNP_SUB void gauss_newton(Scratch s) {
+D3R_HD_NOINLINE void gauss_newton(Scratch s) {
   for (int it = 0; it < kGaussNewton; ++it) {
     const double b0 = s(kBeta), b1 = s(kBeta + 1), b2 = s(kBeta + 2), b3 = s(kBeta + 3);
     for (int i = 0; i < 6; ++i) {
@@ -238,7 +219,7 @@ D3R_PNP_SUB void gauss_newton(Scratch s) {
 }
 
 // camera control points from the betas, camera points, sign, rotation and translation into s(kRt); mean reprojection error
-D3R_PNP_SUB double compute_r_and_t(Scratch s, double fu, double fv, double uc, double vc) {
+D3R_HD_NOINLINE double compute_r_and_t(Scratch s, double fu, double fv, double uc, double vc) {
   for (int c = 0; c < 12; ++c) {
     double v = 0.0;
     for (int k = 0; k < 4; ++k) v += s(kBeta + k) * s(kNull + 12 * k + c);
@@ -256,7 +237,7 @@ D3R_PNP_SUB double compute_r_and_t(Scratch s, double fu, double fv, double uc, d
   }
   double pc0[3] = {0, 0, 0}, pw0[3] = {0, 0, 0};
   for (int i = 0; i < kSample; ++i)
-#pragma unroll
+D3R_UNROLL
     for (int d = 0; d < 3; ++d) {
       pc0[d] += s(kPc + 3 * i + d) / kSample;
       pw0[d] += s(kPw + 3 * i + d) / kSample;
@@ -264,15 +245,15 @@ D3R_PNP_SUB double compute_r_and_t(Scratch s, double fu, double fv, double uc, d
   // S[a][b] = sum (pw - pw0)_a (pc - pc0)_b; Horn's 4x4 N, its top eigenvector is the quaternion of the rotation pw -> pc
   double S[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};
   for (int i = 0; i < kSample; ++i)
-#pragma unroll
+D3R_UNROLL
     for (int a = 0; a < 3; ++a)
-#pragma unroll
+D3R_UNROLL
       for (int b = 0; b < 3; ++b) S[a][b] += (s(kPw + 3 * i + a) - pw0[a]) * (s(kPc + 3 * i + b) - pc0[b]);
   const double N[16] = {S[0][0] + S[1][1] + S[2][2], S[1][2] - S[2][1], S[2][0] - S[0][2], S[0][1] - S[1][0],
                         S[1][2] - S[2][1], S[0][0] - S[1][1] - S[2][2], S[0][1] + S[1][0], S[2][0] + S[0][2],
                         S[2][0] - S[0][2], S[0][1] + S[1][0], -S[0][0] + S[1][1] - S[2][2], S[1][2] + S[2][1],
                         S[0][1] - S[1][0], S[2][0] + S[0][2], S[1][2] + S[2][1], -S[0][0] - S[1][1] + S[2][2]};
-#pragma unroll
+D3R_UNROLL
   for (int k = 0; k < 16; ++k) s(kA + k) = N[k];
   jacobi(s, 4);
   int top = 0;
@@ -284,9 +265,9 @@ D3R_PNP_SUB double compute_r_and_t(Scratch s, double fu, double fv, double uc, d
   const double R[9] = {w * w + x * x - y * y - z * z, 2 * (x * y - w * z), 2 * (x * z + w * y),
                        2 * (x * y + w * z), w * w - x * x + y * y - z * z, 2 * (y * z - w * x),
                        2 * (x * z - w * y), 2 * (y * z + w * x), w * w - x * x - y * y + z * z};
-#pragma unroll
+D3R_UNROLL
   for (int k = 0; k < 9; ++k) s(kRt + k) = R[k];
-#pragma unroll
+D3R_UNROLL
   for (int r = 0; r < 3; ++r) s(kRt + 9 + r) = pc0[r] - (R[3 * r] * pw0[0] + R[3 * r + 1] * pw0[1] + R[3 * r + 2] * pw0[2]);
   // epnp.cpp: reprojection_error
   double sum = 0.0;
@@ -303,17 +284,17 @@ D3R_PNP_SUB double compute_r_and_t(Scratch s, double fu, double fv, double uc, d
 
 // EPnP on the 5 points at s(kPw) / s(kUv); the pose of least reprojection error at s(kBest) = [R row-major | t].  False when
 // the sample is degenerate (no finite pose).
-D3R_PNP_SUB bool epnp(Scratch s, double fu, double fv, double uc, double vc) {
+D3R_HD_NOINLINE bool epnp(Scratch s, double fu, double fv, double uc, double vc) {
   // choose_control_points: centroid + PCA of the world points
   double c0[3] = {0, 0, 0};
   for (int i = 0; i < kSample; ++i)
-#pragma unroll
+D3R_UNROLL
     for (int d = 0; d < 3; ++d) c0[d] += s(kPw + 3 * i + d);
-#pragma unroll
+D3R_UNROLL
   for (int d = 0; d < 3; ++d) c0[d] /= kSample;
-#pragma unroll
+D3R_UNROLL
   for (int a = 0; a < 3; ++a)
-#pragma unroll
+D3R_UNROLL
     for (int b = 0; b < 3; ++b) {
       double v = 0.0;
       for (int i = 0; i < kSample; ++i) v += (s(kPw + 3 * i + a) - c0[a]) * (s(kPw + 3 * i + b) - c0[b]);
@@ -321,9 +302,9 @@ D3R_PNP_SUB bool epnp(Scratch s, double fu, double fv, double uc, double vc) {
     }
   jacobi(s, 3);
   int ord[3] = {0, 1, 2};   // eigenvalues in decreasing order
-#pragma unroll
+D3R_UNROLL
   for (int i = 0; i < 3; ++i)
-#pragma unroll
+D3R_UNROLL
     for (int j = i + 1; j < 3; ++j)
       if (s(kA + 4 * ord[j]) > s(kA + 4 * ord[i])) {
         const int t = ord[i];
@@ -333,34 +314,34 @@ D3R_PNP_SUB bool epnp(Scratch s, double fu, double fv, double uc, double vc) {
   const double lmax = s(kA + 4 * ord[0]);
   if (!(lmax > 0.0) || !isfinite(lmax)) return false;
   double e[3][3], sig[3];
-#pragma unroll
+D3R_UNROLL
   for (int k = 0; k < 3; ++k) {
     const double l = s(kA + 4 * ord[k]);
     sig[k] = l > kFlat * lmax ? sqrt(l / kSample) : 0.0;
-#pragma unroll
+D3R_UNROLL
     for (int d = 0; d < 3; ++d) e[k][d] = s(kV + 3 * d + ord[k]);
     // canonical sign: the component of largest magnitude (the first of equal ones) is positive
     int big = 0;
-#pragma unroll
+D3R_UNROLL
     for (int d = 1; d < 3; ++d)
       if (fabs(e[k][d]) > fabs(e[k][big])) big = d;
     const double sg = e[k][big] < 0.0 ? -1.0 : 1.0;
-#pragma unroll
+D3R_UNROLL
     for (int d = 0; d < 3; ++d) e[k][d] *= sg;
   }
-#pragma unroll
+D3R_UNROLL
   for (int d = 0; d < 3; ++d) s(kCw + d) = c0[d];
-#pragma unroll
+D3R_UNROLL
   for (int k = 0; k < 3; ++k)
-#pragma unroll
+D3R_UNROLL
     for (int d = 0; d < 3; ++d) s(kCw + 3 * (k + 1) + d) = c0[d] + sig[k] * e[k][d];
   // compute_barycentric_coordinates (CC is U diag(sig): its pseudo-inverse is diag(1/sig) U^T)
   for (int i = 0; i < kSample; ++i) {
     double a0 = 1.0;
-#pragma unroll
+D3R_UNROLL
     for (int k = 0; k < 3; ++k) {
       double p = 0.0;
-#pragma unroll
+D3R_UNROLL
       for (int d = 0; d < 3; ++d) p += e[k][d] * (s(kPw + 3 * i + d) - c0[d]);
       const double a = sig[k] > 0.0 ? p / sig[k] : 0.0;
       s(kAlpha + 4 * i + k + 1) = a;
@@ -380,10 +361,10 @@ D3R_PNP_SUB bool epnp(Scratch s, double fu, double fv, double uc, double vc) {
         s(m + 3 * j + 1) = r == 0 ? 0.0 : a * fv;
         s(m + 3 * j + 2) = a * (r == 0 ? du : dv);
       }
-#pragma unroll 1
+D3R_UNROLL_BY(1)
       for (int p = 0; p < 12; ++p) {
         const double mp = s(m + p);
-#pragma unroll 4
+D3R_UNROLL_BY(4)
         for (int q = 0; q < 12; ++q) s(kA + 12 * p + q) += mp * s(m + q);
       }
     }
@@ -421,9 +402,9 @@ D3R_PNP_SUB bool epnp(Scratch s, double fu, double fv, double uc, double vc) {
     int a, b;
     pair_of(k, a, b);
     double dv[4][3];
-#pragma unroll
+D3R_UNROLL
     for (int v = 0; v < 4; ++v)
-#pragma unroll
+D3R_UNROLL
       for (int d = 0; d < 3; ++d) dv[v][d] = s(kNull + 12 * v + 3 * a + d) - s(kNull + 12 * v + 3 * b + d);
     auto dot = [&](int p, int q) { return dv[p][0] * dv[q][0] + dv[p][1] * dv[q][1] + dv[p][2] * dv[q][2]; };
     const int r = kL + 10 * k;
@@ -491,7 +472,7 @@ struct Camera {
 };
 
 // squared reprojection error of one correspondence in fp32, as OpenCV's PnP RANSAC callback computes it
-D3R_PNP_HD float reproj_err2(const double Rt[12], const Camera& cam, float X, float Y, float Z, float u, float v) {
+D3R_HD float reproj_err2(const double Rt[12], const Camera& cam, float X, float Y, float Z, float u, float v) {
   const double x = dadd(dadd(dadd(dmul(Rt[0], X), dmul(Rt[1], Y)), dmul(Rt[2], Z)), Rt[9]);
   const double y = dadd(dadd(dadd(dmul(Rt[3], X), dmul(Rt[4], Y)), dmul(Rt[5], Z)), Rt[10]);
   double z = dadd(dadd(dadd(dmul(Rt[6], X), dmul(Rt[7], Y)), dmul(Rt[8], Z)), Rt[11]);
@@ -504,7 +485,7 @@ D3R_PNP_HD float reproj_err2(const double Rt[12], const Camera& cam, float X, fl
 
 // ---- stopping rule ----
 // calib3d/src/ptsetreg.cpp: RANSACUpdateNumIters
-D3R_PNP_HD int update_num_iters(double p, double ep, int model_points, int max_iters) {
+D3R_HD int update_num_iters(double p, double ep, int model_points, int max_iters) {
   p = p > 0.0 ? (p < 1.0 ? p : 1.0) : 0.0;
   ep = ep > 0.0 ? (ep < 1.0 ? ep : 1.0) : 0.0;
   double num = 1.0 - p;
@@ -527,7 +508,7 @@ struct State {
   double pose[12];     // the best hypothesis' [R | t]
 };
 
-D3R_PNP_HD void state_init(State& st, int max_iters) {
+D3R_HD void state_init(State& st, int max_iters) {
   st.best = -1;
   st.best_count = 0;
   st.niters = max_iters > 1 ? max_iters : 1;
@@ -539,7 +520,7 @@ D3R_PNP_HD void state_init(State& st, int max_iters) {
 
 // Runs the sequential loop over hypotheses h0 .. h0 + m - 1 with their counts (a count < 0 marks an invalid hypothesis) and
 // poses.  With n == kSample there is one hypothesis and no scoring: valid means all 5 points are inliers.
-D3R_PNP_HD void scan_round(State& st, int32_t h0, int32_t m, const int32_t* counts, const double* poses, int32_t n,
+D3R_HD void scan_round(State& st, int32_t h0, int32_t m, const int32_t* counts, const double* poses, int32_t n,
                            double confidence) {
   if (st.done) return;
   for (int32_t i = 0; i < m; ++i) {

@@ -13,11 +13,7 @@
 #pragma once
 #include <stdint.h>
 
-#if defined(__CUDACC__)
-#define D3R_IMG_HD __host__ __device__ __forceinline__
-#else
-#define D3R_IMG_HD inline
-#endif
+#include "hd.h"
 
 namespace d3r {
 namespace image {
@@ -25,7 +21,7 @@ namespace image {
 constexpr int kPrecisionBits = 22;   // Resample.c PRECISION_BITS = 32 - 8 - 2
 
 // Resample.c clip8: arithmetic shift, then clamp to [0, 255]
-D3R_IMG_HD uint8_t clip8(uint32_t acc) {
+D3R_HD uint8_t clip8(uint32_t acc) {
   const int32_t v = (int32_t)acc >> kPrecisionBits;
   return (uint8_t)(v < 0 ? 0 : (v > 255 ? 255 : v));
 }
@@ -43,7 +39,7 @@ struct HorizontalArgs {
 
 // thread t -> pixel (row yi, column xi) of tmp, all three channels (one coefficient load serves R, G and B); xi fastest, so a
 // warp reads one contiguous stretch of a source row per tap and writes 96 contiguous bytes
-D3R_IMG_HD void horizontal_body(long long t, const HorizontalArgs& a) {
+D3R_HD void horizontal_body(long long t, const HorizontalArgs& a) {
   const long long total = (long long)a.rows * a.cols;
   if (t >= total) return;
   const int xi = (int)(t % a.cols);
@@ -79,7 +75,7 @@ struct VerticalArgs {
 
 // The resampled bytes of output pixel (y2, x2), before ImgNorm: the vertical pass of every caller (vertical_body below and the
 // view stage of view_core.h, which stores them elsewhere).  `out` is not read.
-D3R_IMG_HD void vertical_pixel(const VerticalArgs& a, int y2, int x2, uint8_t rgb[3]) {
+D3R_HD void vertical_pixel(const VerticalArgs& a, int y2, int x2, uint8_t rgb[3]) {
   const int y1 = a.crop_y0 + y2;
   const int lo = a.bounds[2 * y1] - a.row0, cnt = a.bounds[2 * y1 + 1];
   const int32_t* k = a.coefs + y1;
@@ -101,7 +97,7 @@ D3R_IMG_HD void vertical_pixel(const VerticalArgs& a, int y2, int x2, uint8_t rg
 // thread t -> pixel (row y2, column x2) of out, all three channel planes; x2 fastest: a warp reads 96 contiguous bytes of an
 // intermediate row per tap (the coefficient is the same for the whole row: a broadcast load) and writes three coalesced
 // 128-byte lines
-D3R_IMG_HD void vertical_body(long long t, const VerticalArgs& a) {
+D3R_HD void vertical_body(long long t, const VerticalArgs& a) {
   const long long plane = (long long)a.H2 * a.W2;
   if (t >= plane) return;
   uint8_t rgb[3];

@@ -13,11 +13,7 @@
 #pragma once
 #include <stdint.h>
 
-#if defined(__CUDACC__)
-#define D3R_SKY_HD __host__ __device__ __forceinline__
-#else
-#define D3R_SKY_HD inline
-#endif
+#include "hd.h"
 
 namespace d3r {
 namespace sky {
@@ -29,7 +25,7 @@ struct Hsv {
 };
 
 // c0, c1, c2 = the three bytes of one pixel in memory order (R, G, B of the scene images)
-D3R_SKY_HD Hsv bgr_to_hsv(int32_t c0, int32_t c1, int32_t c2) {
+D3R_HD Hsv bgr_to_hsv(int32_t c0, int32_t c1, int32_t c2) {
   int32_t v = c0 > c1 ? c0 : c1;
   v = v > c2 ? v : c2;
   int32_t mn = c0 < c1 ? c0 : c1;
@@ -45,11 +41,11 @@ D3R_SKY_HD Hsv bgr_to_hsv(int32_t c0, int32_t c1, int32_t c2) {
 }
 
 // inRange(hsv, (0, 0, 100), (30, 255, 255)) plus the three "luminous gray" terms
-D3R_SKY_HD bool sky_candidate(const Hsv& p) {
+D3R_HD bool sky_candidate(const Hsv& p) {
   return (p.h <= 30 && p.v >= 100) || (p.s < 10 && p.v > 150) || (p.s < 30 && p.v > 180) || (p.s < 50 && p.v > 220);
 }
 
-D3R_SKY_HD bool sky_candidate(const uint8_t* px) { return sky_candidate(bgr_to_hsv(px[0], px[1], px[2])); }
+D3R_HD bool sky_candidate(const uint8_t* px) { return sky_candidate(bgr_to_hsv(px[0], px[1], px[2])); }
 
 }  // namespace sky
 }  // namespace d3r

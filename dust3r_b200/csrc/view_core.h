@@ -13,6 +13,7 @@
 #include <stdint.h>
 
 #include "../../include/dust3r_b200.h"
+#include "hd.h"
 #include "resample_core.h"
 
 namespace d3r {
@@ -21,19 +22,10 @@ namespace view {
 constexpr int kThreads = 256;
 enum Pass { kHorizontal = 0, kVertical = 1, kDepth = 2 };
 
-// fp32 / fp64 operations rounded one at a time: nvcc would contract a multiply and an add into an FMA, numpy does not
-#if defined(__CUDA_ARCH__)
-__device__ __forceinline__ float mul_rn(float a, float b) { return __fmul_rn(a, b); }
-__device__ __forceinline__ float add_rn(float a, float b) { return __fadd_rn(a, b); }
-#else
-inline float mul_rn(float a, float b) { return a * b; }
-inline float add_rn(float a, float b) { return a + b; }
-#endif
-
-D3R_IMG_HD bool finite(float v) { return v == v && v - v == 0.0f; }
+D3R_HD bool finite(float v) { return v == v && v - v == 0.0f; }
 
 // threads of view d in pass p
-D3R_IMG_HD long long pass_threads(const d3r_view_desc& d, int p) {
+D3R_HD long long pass_threads(const d3r_view_desc& d, int p) {
   return p == kHorizontal ? (long long)d.rows * d.W2 : (long long)d.H2 * d.W2;
 }
 
@@ -48,7 +40,7 @@ inline void assign_blocks(d3r_view_desc* desc, int n_views, long long totals[3])
 }
 
 // view owning `block` of pass p: the last v with desc[v].blocks[p] <= block
-D3R_IMG_HD int find_view(const d3r_view_desc* desc, int n_views, long long block, int p) {
+D3R_HD int find_view(const d3r_view_desc* desc, int n_views, long long block, int p) {
   int lo = 0, hi = n_views - 1;
   while (lo < hi) {
     const int mid = (lo + hi + 1) >> 1;
@@ -57,13 +49,13 @@ D3R_IMG_HD int find_view(const d3r_view_desc* desc, int n_views, long long block
   return lo;
 }
 
-D3R_IMG_HD void horizontal_thread(long long block, int thread, const d3r_view_desc* desc, int n_views) {
+D3R_HD void horizontal_thread(long long block, int thread, const d3r_view_desc* desc, int n_views) {
   const d3r_view_desc& d = desc[find_view(desc, n_views, block, kHorizontal)];
   const image::HorizontalArgs a{d.src, d.src_pitch, d.row0, d.rows, d.crop_x0, d.W2, d.W1, d.xbounds, d.xcoefs, d.tmp};
   image::horizontal_body((block - d.blocks[kHorizontal]) * kThreads + thread, a);
 }
 
-D3R_IMG_HD void vertical_thread(long long block, int thread, const d3r_view_desc* desc, int n_views, const float* lut) {
+D3R_HD void vertical_thread(long long block, int thread, const d3r_view_desc* desc, int n_views, const float* lut) {
   const d3r_view_desc& d = desc[find_view(desc, n_views, block, kVertical)];
   const long long t = (block - d.blocks[kVertical]) * kThreads + thread, plane = (long long)d.H2 * d.W2;
   if (t >= plane) return;
@@ -78,13 +70,13 @@ D3R_IMG_HD void vertical_thread(long long block, int thread, const d3r_view_desc
 }
 
 // cv2.resize(INTER_NEAREST) source index of destination index i when n_in samples become n_out
-D3R_IMG_HD int nearest_index(int i, int n_out, int n_in) {
+D3R_HD int nearest_index(int i, int n_out, int n_in) {
   const double s = (double)i * (1.0 / ((double)n_out / (double)n_in));
   const int k = (int)s;               // s >= 0: truncation is floor
   return k < n_in - 1 ? k : n_in - 1;
 }
 
-D3R_IMG_HD void depth_thread(long long block, int thread, const d3r_view_desc* desc, int n_views) {
+D3R_HD void depth_thread(long long block, int thread, const d3r_view_desc* desc, int n_views) {
   const d3r_view_desc& d = desc[find_view(desc, n_views, block, kDepth)];
   const long long t = (block - d.blocks[kDepth]) * kThreads + thread;
   if (t >= (long long)d.H2 * d.W2) return;
@@ -97,7 +89,7 @@ D3R_IMG_HD void depth_thread(long long block, int thread, const d3r_view_desc* d
   const float* P = d.pose;
   float w[3];
   for (int i = 0; i < 3; ++i)
-    w[i] = add_rn(add_rn(add_rn(mul_rn(P[4 * i], x), mul_rn(P[4 * i + 1], y)), mul_rn(P[4 * i + 2], z)), P[4 * i + 3]);
+    w[i] = fadd(fadd(fadd(fmul(P[4 * i], x), fmul(P[4 * i + 1], y)), fmul(P[4 * i + 2], z)), P[4 * i + 3]);
   const long long o = d.transpose ? (long long)x2 * d.H2 + y2 : t;
   d.depthmap[o] = z;
   d.pts3d[3 * o] = w[0];

@@ -86,74 +86,60 @@ def _pillow_rgb(data):
     return np.array(exif_transpose(PIL.Image.open(io.BytesIO(data))).convert('RGB'), dtype=np.uint8)
 
 
-def _jpeg_stage(data):
-    """Host half of decode_jpeg, safe to run on a worker thread: (descriptor, oriented (width, height), pinned bytes), or None
-    when the file is outside the device decoder's set (csrc/jpeg_ops.cu)."""
-    from . import jpeg
+class Unsupported(ValueError):
+    """The file is valid for Pillow perhaps, but not something the device decoders reproduce."""
+
+
+def oriented_size(header, orient):
+    """(width, height) after exif_transpose."""
+    w, h = header['width'], header['height']
+    return (h, w) if orient >= 5 else (w, h)
+
+
+def _stage(codec, data):
+    """Host half of a device decode by `codec` (the module utils.jpeg or utils.png), safe to run on a worker thread:
+    (descriptor, oriented (width, height), pinned payload), or None when the file is outside that decoder's set."""
     try:
-        head = jpeg.parse(data)
-    except jpeg.Unsupported:
+        desc, size, payload = codec.stage(data)
+    except Unsupported:
         return None
-    orient = jpeg.orientation(data)
-    pinned = torch.frombuffer(bytearray(data), dtype=torch.uint8)
+    pinned = torch.frombuffer(bytearray(payload), dtype=torch.uint8)
     if torch.cuda.is_available():
         pinned = pinned.pin_memory()
-    return jpeg.descriptor(head, orient), jpeg.oriented_size(head, orient), pinned
+    return desc, size, pinned
+
+
+def _launch(entry, staged, dev):
+    """Uploads the payload and enqueues the decode `entry` (d3r_jpeg_decode, d3r_png_decode) on `dev`'s current stream ->
+    (uint8 (H, W, 3) image, int32 status) on `dev`."""
+    import ctypes
+    from .. import _lib
+    desc, (w, h), pinned = staged
+    n = int(pinned.numel())
+    ws_bytes = int(getattr(_lib.get_lib(), entry + '_workspace_bytes')(ctypes.byref(desc), n))
+    if ws_bytes <= 0:
+        raise _lib.D3RError(f'{entry}_workspace_bytes rejected the descriptor')
+    src = pinned.to(dev, non_blocking=True)
+    out = torch.empty((h, w, 3), dtype=torch.uint8, device=dev)
+    status = torch.empty((1,), dtype=torch.int32, device=dev)
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+    _lib.launch(dev, entry, ctypes.byref(desc), src.data_ptr(), n, out.data_ptr(), status.data_ptr(), ws.data_ptr(), ws_bytes)
+    return out, status
+
+
+# the two device decoders: host half (csrc/jpeg_ops.cu / csrc/png_ops.cu take what it stages) and launch
+def _jpeg_stage(data):
+    from . import jpeg
+    return _stage(jpeg, data)
 
 
 def _png_stage(data):
-    """Host half of decode_png, safe to run on a worker thread: (descriptor, oriented (width, height), pinned zlib stream), or
-    None when the file is outside the device decoder's set (csrc/png_ops.cu)."""
     from . import png
-    try:
-        head = png.parse(data)
-        orient = png.orientation(head)
-    except png.Unsupported:
-        return None
-    pinned = torch.frombuffer(bytearray(head['idat']), dtype=torch.uint8)
-    if torch.cuda.is_available():
-        pinned = pinned.pin_memory()
-    return png.descriptor(head, orient), png.oriented_size(head, orient), pinned
+    return _stage(png, data)
 
 
-def _jpeg_launch(staged, dev):
-    """Uploads the bytes and enqueues the decode on `dev`'s current stream -> (uint8 (H, W, 3) image, int32 status) on `dev`."""
-    import ctypes
-    from .. import _lib
-    desc, (w, h), pinned = staged
-    lib = _lib.get_lib()
-    n = int(pinned.numel())
-    ws_bytes = int(lib.d3r_jpeg_decode_workspace_bytes(ctypes.byref(desc), n))
-    if ws_bytes <= 0:
-        raise _lib.D3RError('d3r_jpeg_decode_workspace_bytes rejected the descriptor')
-    src = pinned.to(dev, non_blocking=True)
-    out = torch.empty((h, w, 3), dtype=torch.uint8, device=dev)
-    status = torch.empty((1,), dtype=torch.int32, device=dev)
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-    _lib.launch(dev, 'd3r_jpeg_decode', ctypes.byref(desc), src.data_ptr(), n, out.data_ptr(), status.data_ptr(), ws.data_ptr(),
-                ws_bytes)
-    return out, status
-
-
-def _png_launch(staged, dev):
-    """Uploads the zlib stream and enqueues the decode on `dev`'s current stream -> (uint8 (H, W, 3) image, int32 status) on
-    `dev`."""
-    import ctypes
-    from .. import _lib
-    desc, (w, h), pinned = staged
-    lib = _lib.get_lib()
-    n = int(pinned.numel())
-    ws_bytes = int(lib.d3r_png_decode_workspace_bytes(ctypes.byref(desc), n))
-    if ws_bytes <= 0:
-        raise _lib.D3RError('d3r_png_decode_workspace_bytes rejected the descriptor')
-    src = pinned.to(dev, non_blocking=True)
-    out = torch.empty((h, w, 3), dtype=torch.uint8, device=dev)
-    status = torch.empty((1,), dtype=torch.int32, device=dev)
-    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
-    _lib.launch(dev, 'd3r_png_decode', ctypes.byref(desc), src.data_ptr(), n, out.data_ptr(), status.data_ptr(), ws.data_ptr(),
-                ws_bytes)
-    return out, status
-
+_jpeg_launch = functools.partial(_launch, 'd3r_jpeg_decode')
+_png_launch = functools.partial(_launch, 'd3r_png_decode')
 
 _PNG_SIGNATURE = b'\x89PNG\r\n\x1a\n'
 # load_images decodes a PNG on the GPU from this many pixels on.  Each GPU decode costs a fixed ~35 ms (one thread per DEFLATE
@@ -165,15 +151,27 @@ PNG_DEVICE_MIN_PIXELS = 8_000_000
 def _device_stage(data):
     """(launch, staged) of a file the GPU decoders take -- PNGs of at least PNG_DEVICE_MIN_PIXELS by their signature,
     everything else as a JPEG -- or None."""
+    stage, launch = _jpeg_stage, _jpeg_launch
     if data[:8] == _PNG_SIGNATURE:
         import struct
         width, height = struct.unpack('>II', data[16:24]) if len(data) >= 24 else (0, 0)
         if width * height < PNG_DEVICE_MIN_PIXELS:
             return None
-        staged = _png_stage(data)
-        return None if staged is None else (_png_launch, staged)
-    staged = _jpeg_stage(data)
-    return None if staged is None else (_jpeg_launch, staged)
+        stage, launch = _png_stage, _png_launch
+    staged = stage(data)
+    return None if staged is None else (launch, staged)
+
+
+def _decode(stage, launch, data, device):
+    from .. import _lib
+    dev = _lib.cuda_device(device)
+    data = bytes(data)
+    staged = stage(data)
+    if staged is not None:
+        img, status = launch(staged, dev)
+        if int(status.item()) == 0:
+            return img
+    return torch.from_numpy(_pillow_rgb(data)).to(dev)
 
 
 @torch.no_grad()
@@ -183,17 +181,7 @@ def decode_jpeg(data, device='cuda'):
     4:4:4, 4:2:2 or 4:2:0) are decoded by the GPU kernels of csrc/jpeg_ops.cu; any other file, and any stream those kernels
     report they cannot reproduce exactly, is decoded by Pillow and uploaded -- the choice is made from the file, so the result
     is Pillow's either way (including the exception Pillow raises for a broken file)."""
-    from .. import _lib
-    dev = _lib.require_cuda_device(device)
-    if dev.index is None:
-        dev = torch.device('cuda', torch.cuda.current_device())
-    data = bytes(data)
-    staged = _jpeg_stage(data)
-    if staged is not None:
-        img, status = _jpeg_launch(staged, dev)
-        if int(status.item()) == 0:
-            return img
-    return torch.from_numpy(_pillow_rgb(data)).to(dev)
+    return _decode(_jpeg_stage, _jpeg_launch, data, device)
 
 
 @torch.no_grad()
@@ -203,17 +191,7 @@ def decode_png(data, device='cuda'):
     alpha, RGBA) are inflated, unfiltered and converted by the GPU kernels of csrc/png_ops.cu; any other file, and any stream
     those kernels report they cannot reproduce exactly, is decoded by Pillow and uploaded -- the choice is made from the file,
     so the result is Pillow's either way (including the exception Pillow raises for a broken file)."""
-    from .. import _lib
-    dev = _lib.require_cuda_device(device)
-    if dev.index is None:
-        dev = torch.device('cuda', torch.cuda.current_device())
-    data = bytes(data)
-    staged = _png_stage(data)
-    if staged is not None:
-        img, status = _png_launch(staged, dev)
-        if int(status.item()) == 0:
-            return img
-    return torch.from_numpy(_pillow_rgb(data)).to(dev)
+    return _decode(_png_stage, _png_launch, data, device)
 
 
 def _host_view(pil, size, square_ok, patch_size):
@@ -289,9 +267,7 @@ def load_images(folder_or_list, size, square_ok=False, verbose=True, patch_size=
             img = preprocess_image_u8(item, size, square_ok, device, patch_size)
         else:
             from .. import _lib
-            dev = _lib.require_cuda_device(device)
-            if dev.index is None:
-                dev = torch.device('cuda', torch.cuda.current_device())
+            dev = _lib.cuda_device(device)
             data, (launch, dev_staged) = item
             pixels, status_dev = launch(dev_staged, dev)
             img = preprocess_image_u8(pixels, size, square_ok, dev, patch_size)
@@ -439,9 +415,7 @@ def preprocess_image_u8(pixels, size, square_ok=False, device='cuda', patch_size
     `device`, what load_images stores under 'img' for that picture: resize (long edge -> size; size 224: short edge -> 224),
     centre crop to multiples of 16 (224: square), x / 255 normalised to [-1, 1]."""
     from .. import _lib
-    dev = _lib.require_cuda_device(device)
-    if dev.index is None:
-        dev = torch.device('cuda', torch.cuda.current_device())
+    dev = _lib.cuda_device(device)
     src = torch.as_tensor(pixels)
     if src.dtype != torch.uint8 or src.ndim != 3 or src.shape[2] != 3:
         raise ValueError(f'preprocess_image_u8 expects uint8 (H, W, 3) RGB, got {src.dtype} {tuple(src.shape)}')

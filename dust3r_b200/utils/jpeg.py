@@ -14,14 +14,12 @@ import struct
 
 import numpy as np
 
+from .image import Unsupported, oriented_size
+
 # jutils.c jpeg_natural_order
 NATURAL = np.array([0, 1, 8, 16, 9, 2, 3, 10, 17, 24, 32, 25, 18, 11, 4, 5, 12, 19, 26, 33, 40, 48, 41, 34, 27, 20, 13, 6, 7, 14,
                     21, 28, 35, 42, 49, 56, 57, 50, 43, 36, 29, 22, 15, 23, 30, 37, 44, 51, 58, 59, 52, 45, 38, 31, 39, 46, 53,
                     60, 61, 54, 47, 55, 62, 63])
-
-
-class Unsupported(ValueError):
-    """The file is valid for Pillow perhaps, but not something the device decoder reproduces."""
 
 
 def _huff_table(counts, symbols, is_dc):
@@ -202,7 +200,9 @@ def descriptor(header, orient=1):
     return d
 
 
-def oriented_size(header, orient):
-    """(width, height) after exif_transpose."""
-    w, h = header['width'], header['height']
-    return (h, w) if orient >= 5 else (w, h)
+def stage(data):
+    """(descriptor, oriented (width, height), payload) of a file the device decoder takes; the payload is the whole file.
+    Raises Unsupported for the others."""
+    head = parse(data)
+    orient = orientation(data)
+    return descriptor(head, orient), oriented_size(head, orient), data

@@ -19,15 +19,13 @@ import zlib
 
 import numpy as np
 
+from .image import Unsupported, oriented_size
+
 SIGNATURE = b'\x89PNG\r\n\x1a\n'
 _BPP = {0: 1, 2: 3, 3: 1, 4: 2, 6: 4}
 # ancillary chunks of the PNG specification; they travel to the orientation stand-in unchanged
 _ANCILLARY = {b'cHRM', b'gAMA', b'iCCP', b'sBIT', b'sRGB', b'bKGD', b'hIST', b'pHYs', b'sPLT', b'tIME', b'iTXt', b'tEXt',
               b'zTXt', b'eXIf', b'cICP', b'mDCv', b'cLLi'}
-
-
-class Unsupported(ValueError):
-    """The file is valid for Pillow perhaps, but not something the device decoder reproduces."""
 
 
 def parse(data):
@@ -151,7 +149,9 @@ def descriptor(header, orient=1):
     return d
 
 
-def oriented_size(header, orient):
-    """(width, height) after exif_transpose."""
-    w, h = header['width'], header['height']
-    return (h, w) if orient >= 5 else (w, h)
+def stage(data):
+    """(descriptor, oriented (width, height), payload) of a file the device decoder takes; the payload is the concatenated
+    IDAT data.  Raises Unsupported for the others."""
+    head = parse(data)
+    orient = orientation(head)
+    return descriptor(head, orient), oriented_size(head, orient), head['idat']

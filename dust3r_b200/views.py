@@ -282,8 +282,7 @@ def _device(device):
     if dev.type == 'cpu':
         return dev
     from . import _lib
-    dev = _lib.require_cuda_device(dev)
-    return torch.device('cuda', torch.cuda.current_device()) if dev.index is None else dev
+    return _lib.cuda_device(dev)
 
 
 def _item_idx(idx):

@@ -10,15 +10,14 @@
 """
 import ctypes
 import os
-import shutil
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN, ROOT, reference_golden
+from conftest import GOLDEN, reference_golden
+import native_harness
 from dust3r_b200.utils import image as img_mod
 from dust3r_b200.utils.synth import synth_photo
 from oracle import image_oracle as io
@@ -115,14 +114,8 @@ def test_oracle_and_host_port_equal_live_reference_load_images(tmp_path):
 
 # ------------------------------------------------------------------------------------------------ the GPU code, on the host
 @pytest.fixture(scope='module')
-def host_kernels(tmp_path_factory):
-    gxx = shutil.which('g++')
-    if gxx is None:
-        pytest.skip('no g++')
-    out = os.path.join(str(tmp_path_factory.mktemp('native')), 'resample_host.so')
-    src = os.path.join(ROOT, 'tests', 'native', 'resample_host.cpp')
-    subprocess.run([gxx, '-O2', '-std=c++17', '-shared', '-fPIC', '-Wall', '-Wextra', '-Werror', '-o', out, src], check=True)
-    lib = ctypes.CDLL(out)
+def host_kernels():
+    lib = ctypes.CDLL(native_harness.build('resample_host'))
     vp, i32 = ctypes.c_void_p, ctypes.c_int32
     lib.resample_host.restype = ctypes.c_int
     lib.resample_host.argtypes = [vp, i32, i32, i32, i32, vp, vp, i32, vp, vp, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp]

@@ -7,13 +7,12 @@ Pillow by their header.  The `-m gpu` twin is tests/test_jpeg_gpu.py, on the sam
 import ctypes
 import io
 import os
-import shutil
 import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
+import native_harness
 
 
 def _pixels(h, w, seed, kind='photo'):
@@ -89,19 +88,9 @@ def pillow_rgb(data):
     return np.asarray(exif_transpose(PIL.Image.open(io.BytesIO(data))).convert('RGB'))
 
 
-def _compile(out, *flags):
-    gxx = shutil.which('g++')
-    if gxx is None:
-        pytest.skip('no g++')
-    src = os.path.join(ROOT, 'tests', 'native', 'jpeg_host.cpp')
-    subprocess.run([gxx, '-std=c++17', '-Wall', '-Wextra', '-Werror', *flags, '-o', out, src], check=True)
-    return out
-
-
 @pytest.fixture(scope='module')
-def host_jpeg(tmp_path_factory):
-    out = _compile(os.path.join(str(tmp_path_factory.mktemp('native')), 'jpeg_host.so'), '-O2', '-shared', '-fPIC')
-    lib = ctypes.CDLL(out)
+def host_jpeg():
+    lib = ctypes.CDLL(native_harness.build('jpeg_host'))
     lib.jpeg_host_workspace_bytes.restype = ctypes.c_longlong
     lib.jpeg_host_workspace_bytes.argtypes = [ctypes.c_void_p, ctypes.c_longlong]
     lib.jpeg_host_decode.restype = ctypes.c_int
@@ -245,8 +234,8 @@ def test_corrupt_streams_set_the_status_word(host_jpeg, corpus):
 def test_corrupt_streams_stay_in_bounds_under_asan(tmp_path, corpus):
     """The same corrupt streams through the stand-alone harness built with -fsanitize=address: every buffer has its exact size,
     so any read past the compressed bytes aborts the run."""
-    exe = _compile(str(tmp_path / 'jpeg_host_asan'), '-O1', '-g', '-fsanitize=address,undefined', '-fno-sanitize-recover=all',
-                   '-DJPEG_HOST_MAIN')
+    exe = native_harness.build('jpeg_host', '-O1', '-g', '-fsanitize=address,undefined', '-fno-sanitize-recover=all',
+                                '-DJPEG_HOST_MAIN', shared=False)
     rng = np.random.default_rng(1)
     args = []
     for name in ('q90_420_64x48', 'rst1_422_100x75', 'grey_rst3_33x17', 'size_420_1x1', 'noise_q100_444_96x80'):

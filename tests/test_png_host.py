@@ -8,7 +8,6 @@ The `-m gpu` twin is tests/test_png_gpu.py, on the same corpus."""
 import ctypes
 import io
 import os
-import shutil
 import struct
 import subprocess
 import zlib
@@ -16,7 +15,7 @@ import zlib
 import numpy as np
 import pytest
 
-from conftest import ROOT
+import native_harness
 
 SHORT, ADLER, FAR, FILTER, PALETTE = 4, 8, 2, 16, 32     # D3R_PNG_*
 
@@ -164,19 +163,9 @@ def pillow_rgb(data):
     return np.asarray(exif_transpose(PIL.Image.open(io.BytesIO(data))).convert('RGB'))
 
 
-def _compile(out, *flags):
-    gxx = shutil.which('g++')
-    if gxx is None:
-        pytest.skip('no g++')
-    src = os.path.join(ROOT, 'tests', 'native', 'png_host.cpp')
-    subprocess.run([gxx, '-std=c++17', '-Wall', '-Wextra', '-Werror', *flags, '-o', out, src], check=True)
-    return out
-
-
 @pytest.fixture(scope='module')
-def host_png(tmp_path_factory):
-    out = _compile(os.path.join(str(tmp_path_factory.mktemp('native')), 'png_host.so'), '-O2', '-shared', '-fPIC')
-    lib = ctypes.CDLL(out)
+def host_png():
+    lib = ctypes.CDLL(native_harness.build('png_host'))
     lib.png_host_workspace_bytes.restype = ctypes.c_longlong
     lib.png_host_workspace_bytes.argtypes = [ctypes.c_void_p, ctypes.c_longlong]
     lib.png_host_decode.restype = ctypes.c_int
@@ -421,8 +410,8 @@ def test_corrupt_streams_set_the_status_word(host_png, corpus):
 def test_corrupt_streams_stay_in_bounds_under_asan(tmp_path, corpus):
     """The same corrupt and crafted streams through the stand-alone harness built with -fsanitize=address: every buffer has
     its exact size, so any read past the stream aborts the run."""
-    exe = _compile(str(tmp_path / 'png_host_asan'), '-O1', '-g', '-fsanitize=address,undefined', '-fno-sanitize-recover=all',
-                   '-DPNG_HOST_MAIN')
+    exe = native_harness.build('png_host', '-O1', '-g', '-fsanitize=address,undefined', '-fno-sanitize-recover=all',
+                                '-DPNG_HOST_MAIN', shared=False)
     rng = np.random.default_rng(1)
     args = []
     cases = [(n, corpus[n]) for n in ('pil_RGB_53x37', 'zlib_fixed_RGB_200x150', 'pil_level0_RGB_53x37', 'size_1x1',

@@ -10,15 +10,12 @@
 The `-m gpu` twin is tests/test_pnp_gpu.py.
 """
 import ctypes as C
-import os
-import shutil
-import subprocess
 
 import cv2
 import numpy as np
 import pytest
 
-from conftest import ROOT
+import native_harness
 from oracle import pnp_float64 as O
 
 SEED = O.DEFAULT_SEED
@@ -26,14 +23,8 @@ P = lambda a: a.ctypes.data_as(C.c_void_p)
 
 
 @pytest.fixture(scope='module')
-def host(tmp_path_factory):
-    gxx = shutil.which('g++')
-    if gxx is None:
-        pytest.skip('no g++')
-    out = os.path.join(str(tmp_path_factory.mktemp('native')), 'pnp_host.so')
-    src = os.path.join(ROOT, 'tests', 'native', 'pnp_host.cpp')
-    subprocess.run([gxx, '-O2', '-std=c++17', '-ffp-contract=off', '-shared', '-fPIC', src, '-o', out], check=True)
-    lib = C.CDLL(out)
+def host():
+    lib = C.CDLL(native_harness.build('pnp_host'))
     d = C.c_double
     lib.pnp_hypotheses_host.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, d, d, d, d, d, C.c_uint64, C.c_int32, C.c_int32,
                                         C.c_void_p, C.c_void_p, C.c_void_p]

@@ -10,14 +10,13 @@ The `-m gpu` twin is tests/test_sky_gpu.py.  The image cases below are shared wi
 import copy
 import ctypes
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN, ROOT
+from conftest import GOLDEN
+import native_harness
 from dust3r_b200.utils.synth import synth_consistent_scene, synth_pair_predictions, synth_sky_image
 from oracle import sky_oracle
 
@@ -142,14 +141,8 @@ def golden_mask(gold, name):
 
 # ------------------------------------------------------------------------------------------------ the GPU colour test, on the host
 @pytest.fixture(scope='module')
-def host_colour(tmp_path_factory):
-    gxx = shutil.which('g++')
-    if gxx is None:
-        pytest.skip('no g++')
-    out = os.path.join(str(tmp_path_factory.mktemp('native')), 'sky_host.so')
-    src = os.path.join(ROOT, 'tests', 'native', 'sky_host.cpp')
-    subprocess.run([gxx, '-O2', '-std=c++17', '-shared', '-fPIC', '-Wall', '-Wextra', '-Werror', '-o', out, src], check=True)
-    lib = ctypes.CDLL(out)
+def host_colour():
+    lib = ctypes.CDLL(native_harness.build('sky_host'))
     lib.sky_classify_host.restype = ctypes.c_int
     lib.sky_classify_host.argtypes = [ctypes.c_void_p, ctypes.c_longlong, ctypes.c_void_p, ctypes.c_void_p]
     return lib

@@ -5,14 +5,13 @@ run over every block and thread of the three launches, bit-equal to the oracle; 
 import ctypes
 import json
 import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 import torch
 
 from conftest import GOLDEN, ROOT
+import native_harness
 
 from dust3r_b200.utils.synth import synth_rgbd_frame
 from dust3r_b200.views import final_crop_box, item_rng, prepare_batch, prepare_views, view_descriptors
@@ -108,16 +107,8 @@ def test_oracle_equals_live_reference():
 # csrc/view_core.h on the host
 # ------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope='module')
-def view_host(tmp_path_factory):
-    gxx = shutil.which('g++')
-    if gxx is None:
-        pytest.skip('no g++')
-    out = os.path.join(str(tmp_path_factory.mktemp('native')), 'view_host.so')
-    src = os.path.join(ROOT, 'tests', 'native', 'view_host.cpp')
-    # no contraction of a * b + c: the device code rounds every fp32 operation on its own, like numpy
-    subprocess.run([gxx, '-O2', '-std=c++17', '-shared', '-fPIC', '-Wall', '-Wextra', '-Werror', '-ffp-contract=off', '-o', out, src],
-                   check=True)
-    lib = ctypes.CDLL(out)
+def view_host():
+    lib = ctypes.CDLL(native_harness.build('view_host'))
     lib.view_host.restype = ctypes.c_int
     lib.view_host.argtypes = [ctypes.c_int32, ctypes.c_void_p, ctypes.c_void_p]
     return lib
