@@ -101,6 +101,8 @@ PROTOTYPES = {
     'd3r_align_pixel_pass': (i32, [_DESC, i32, vp]),
     'd3r_align_small_step': (i32, [_DESC, i32, vp]),
     'd3r_align_reduce_block': (i32, [i32, i32, C.POINTER(i64), C.POINTER(i64)]),
+    'd3r_align_grad_pixel_pass': (i32, [_DESC, vp, vp]),
+    'd3r_align_grad_small_step': (i32, [_DESC, vp, vp, vp]),
     'd3r_align_loss_grad': (i32, [_DESC, vp, vp, vp, vp]),
     'd3r_align_overflow_flag': (i32, [_DESC, C.POINTER(i32), vp]),
     'd3r_align_pts3d': (i32, [_DESC, vp, vp]),

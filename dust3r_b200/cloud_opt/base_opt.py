@@ -288,20 +288,24 @@ class BasePCOptimizer(nn.Module):
         raise NotImplementedError()
 
     def _engine_grads(self, eng, logd_grad, small_grad):
-        """Gradients of _engine_params() from the flat gradients of AlignEngine.loss_and_grad, each shaped like its
-        parameter."""
+        """Gradients of _engine_params() from the flat gradients of AlignEngine.loss_and_grad (or sharded_loss_and_grad),
+        each shaped like its parameter."""
         raise NotImplementedError()
 
     def forward(self, ret_details=False):
         """Objective at the current parameters (a CUDA scalar tensor).  With grad mode on and a parameter that requires
         grad, the loss carries an autograd graph: backward() hands the fused kernel's analytic gradients to the
-        parameters.  ret_details=True also returns the (n, n) CPU tensor of per-edge losses li + lj (-1 off the edges)."""
+        parameters.  ret_details=True also returns the (n, n) CPU tensor of per-edge losses li + lj (-1 off the edges).
+        On a scene of distributed.global_aligner_sharded this is a collective, like compute_global_alignment: every rank of
+        the group calls it, the objective is taken at rank 0's parameters, and every rank gets the same loss, details and
+        .grad (backward() itself runs no collective)."""
         eng = self._get_engine()
         self._engine_push(eng)
         params = self._engine_params()
         if not ret_details and not (torch.is_grad_enabled() and any(p.requires_grad for p in params)):
             return eng.evaluate_loss()
-        loss, logd_grad, small_grad, ent = eng.loss_and_grad(entry_loss=ret_details)
+        loss_and_grad = eng.sharded_loss_and_grad if eng.shards is not None else eng.loss_and_grad
+        loss, logd_grad, small_grad, ent = loss_and_grad(entry_loss=ret_details)
         loss = _FusedObjective.apply(loss, self._engine_grads(eng, logd_grad, small_grad), *params)
         if not ret_details:
             return loss

@@ -10,7 +10,9 @@ HBM layout (all fp32, owned by torch):
 
 Sharded over the ranks of a process group (`shards=`), each rank packs and streams only its own images' entries and runs
 every iteration as pixel pass -> one all-reduce of the fixed-point accumulator block -> small step (d3r_align_pixel_pass /
-d3r_align_small_step), so that every rank computes the same small parameters; `logd` keeps its global layout.
+d3r_align_small_step), so that every rank computes the same small parameters; `logd` keeps its global layout.  The
+objective's gradient is split the same way (sharded_loss_and_grad: d3r_align_grad_pixel_pass -> the all-reduce ->
+d3r_align_grad_small_step, then one broadcast per owner of its images' log-depth gradients).
 """
 from __future__ import annotations
 
@@ -98,9 +100,9 @@ class AlignEngine:
     packed by ONE launch (d3r_align_pack_entries).
 
     shards: optional list of contiguous image ranges [lo, hi), one per rank of `group` (distributed.shard_images); this
-    rank packs and streams only the entries of its own range, and run() / evaluate_loss() exchange the accumulators with
-    one all-reduce per iteration.  Streaming kernel only.  The inputs of entries outside the range are never read and may
-    be None (a scene of the rows inference_sharded(keep='owned') kept)."""
+    rank packs and streams only the entries of its own range, and run() / evaluate_loss() / sharded_loss_and_grad()
+    exchange the accumulators with one all-reduce per iteration.  Streaming kernel only.  The inputs of entries outside the
+    range are never read and may be None (a scene of the rows inference_sharded(keep='owned') kept)."""
 
     def __init__(self, edges: Sequence[Tuple[int, int]], imshapes: Sequence[Tuple[int, int]],
                  pred_i: Sequence[torch.Tensor], pred_j: Sequence[torch.Tensor],
@@ -481,11 +483,13 @@ class AlignEngine:
         tdist.all_reduce(self._reduce, op=tdist.ReduceOp.SUM, group=self.group)
         _lib.launch(self.device, 'd3r_align_small_step', C.byref(d), it)
 
-    def _sync_end(self):
-        """Every owner broadcasts its images' log-depths, so that every rank holds the whole scene."""
+    def _sync_end(self, flat=None):
+        """Every owner broadcasts its images' slice of `flat` (default: the log-depths), laid out like `logd`, so that every
+        rank holds the whole scene."""
+        flat = self.logd if flat is None else flat
         for r, (a, b) in enumerate(self.shards):
             if b > a:
-                tdist.broadcast(self.logd[int(self.pix_off[a]):int(self.pix_off[b])], src=self._src(r), group=self.group)
+                tdist.broadcast(flat[int(self.pix_off[a]):int(self.pix_off[b])], src=self._src(r), group=self.group)
 
     def check_overflow(self):
         """Raises if a fixed-point accumulator left its range (host sync)."""
@@ -518,8 +522,8 @@ class AlignEngine:
         for, the (E, 2) coefficient-weighted loss of every (edge, side), else None.  Every tensor is freshly allocated,
         so results of two calls never alias."""
         if self.shards is not None:
-            raise NotImplementedError('the differentiable objective (loss.backward(), ret_details=True) is not available on a '
-                                      'sharded alignment scene; use global_aligner for it')
+            raise NotImplementedError('loss_and_grad is the single-GPU launch; a sharded engine takes the objective and its '
+                                      'gradient with sharded_loss_and_grad, which every rank of the group calls')
         dev = self.device
         loss = torch.zeros((), dtype=torch.float32, device=dev)
         logd_grad = torch.zeros_like(self.logd)
@@ -530,6 +534,33 @@ class AlignEngine:
         d.loss_out = loss.data_ptr()
         _lib.launch(self.device, 'd3r_align_loss_grad', C.byref(d), logd_grad.data_ptr(), small_grad.data_ptr(),
                     ent.data_ptr() if ent is not None else None)
+        return loss, logd_grad, small_grad, ent
+
+    def sharded_loss_and_grad(self, entry_loss=False):
+        """loss_and_grad of a sharded engine, and like run() a collective: every rank of the group calls it.  The objective
+        is taken at rank 0's parameters (one broadcast, as evaluate_loss does).  This rank's gradient pixel pass
+        (d3r_align_grad_pixel_pass) writes the log-depth gradients of its own images, one all-reduce combines the accumulator
+        block, every rank's gradient small step (d3r_align_grad_small_step) forms the same loss, small-parameter gradients
+        and entry losses, and one broadcast per owner of its images' log-depth gradients gives every rank all of them.
+        Returns what loss_and_grad returns, bit-identical on every rank; on a one-rank group the bits of loss_and_grad."""
+        if self.shards is None:
+            raise ValueError('sharded_loss_and_grad needs a sharded engine (shards=); use loss_and_grad')
+        dev = self.device
+        loss = torch.zeros((), dtype=torch.float32, device=dev)
+        logd_grad = torch.zeros_like(self.logd)
+        small_grad = torch.empty((self.n_small,), dtype=torch.float32, device=dev)
+        ent = torch.empty((self.E, 2), dtype=torch.float32, device=dev) if entry_loss else None
+        with torch.cuda.device(dev):
+            self._sync_start()
+            self.prepare()
+            d = self._desc()
+            d.loss_out = loss.data_ptr()
+            if self.n_items:
+                _lib.launch(dev, 'd3r_align_grad_pixel_pass', C.byref(d), logd_grad.data_ptr())
+            tdist.all_reduce(self._reduce, op=tdist.ReduceOp.SUM, group=self.group)
+            _lib.launch(dev, 'd3r_align_grad_small_step', C.byref(d), small_grad.data_ptr(), ent.data_ptr() if ent is not None else None)
+            # owner ranges are broadcast, not summed: an all-reduce over zero-filled ranges would turn -0.0 into +0.0
+            self._sync_end(logd_grad)
         return loss, logd_grad, small_grad, ent
 
     def pts3d(self):

@@ -1,7 +1,7 @@
 """Scenes built from the rows of distributed.inference_sharded(keep='owned'): each rank of the group holds only the rows its
 images need -- the whole row of every pair whose first image it owns, the view-2 half of every pair whose second image it
-owns (distributed.PairOutputRoute).  The alignment loop needs nothing else (the engine packs its own images' entries); what
-needs more is assembled here with collectives on the scene's device:
+owns (distributed.PairOutputRoute).  The alignment loop and the differentiable objective need nothing else (the engine packs
+its own images' entries); what needs more is assembled here with collectives on the scene's device:
 
   share_im_conf      each owner forms its images' confidence maxima from its own entries; one broadcast per owner.
   edge_scores        the spanning tree's edge scores, each computed on the rank keeping the whole row; one all-reduce.

@@ -339,7 +339,7 @@ __global__ void __launch_bounds__(kThreads) pts3d_kernel(const __grid_constant__
 
 namespace d3r { namespace align {
 int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, const GradOut* go, cudaStream_t st);
-int launch_stream_split(const d3r_align_desc* desc, int it, bool pixel, cudaStream_t st);
+int launch_stream_split(const d3r_align_desc* desc, int it, bool pixel, const GradOut* go, cudaStream_t st);
 int stream_set_debug(unsigned long long* p);
 } }
 
@@ -414,7 +414,16 @@ extern "C" int d3r_align_pixel_pass(const d3r_align_desc* desc, int32_t it, void
   if (rc) return rc;
   D3R_CHECK_ARG(it >= 0, "d3r_align_pixel_pass: bad iteration %d", it);
   prof::Scope scope("align_pixel", (cudaStream_t)stream, 0.0, 0.0, 1);
-  return launch_stream_split(desc, it, true, (cudaStream_t)stream);
+  return launch_stream_split(desc, it, true, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_align_grad_pixel_pass(const d3r_align_desc* desc, float* logd_grad, void* stream) {
+  int rc = validate(desc, false);
+  if (rc) return rc;
+  D3R_CHECK_ARG(logd_grad, "d3r_align_grad_pixel_pass: null gradient buffer");
+  prof::Scope scope("align_grad_pixel", (cudaStream_t)stream, 0.0, 0.0, 1);
+  const GradOut go{logd_grad, nullptr, nullptr};
+  return launch_stream_split(desc, 0, true, &go, (cudaStream_t)stream);
 }
 
 extern "C" int d3r_align_small_step(const d3r_align_desc* desc, int32_t it, void* stream) {
@@ -426,7 +435,18 @@ extern "C" int d3r_align_small_step(const d3r_align_desc* desc, int32_t it, void
     D3R_CUDA(cudaMemsetAsync(ws0.flags, 0, sizeof(int), (cudaStream_t)stream));
   }
   prof::Scope scope("align_small", (cudaStream_t)stream, 0.0, 0.0, 1);
-  return launch_stream_split(desc, it, false, (cudaStream_t)stream);
+  return launch_stream_split(desc, it, false, nullptr, (cudaStream_t)stream);
+}
+
+extern "C" int d3r_align_grad_small_step(const d3r_align_desc* desc, float* small_grad, float* entry_loss, void* stream) {
+  int rc = validate(desc, false);
+  if (rc) return rc;
+  D3R_CHECK_ARG(small_grad, "d3r_align_grad_small_step: null gradient buffer");
+  const Workspace ws0 = carve(desc->workspace, desc->n_imgs, desc->n_edges);
+  D3R_CUDA(cudaMemsetAsync(ws0.flags, 0, sizeof(int), (cudaStream_t)stream));   // the overflow flag reports on this evaluation
+  prof::Scope scope("align_grad_small", (cudaStream_t)stream, 0.0, 0.0, 1);
+  const GradOut go{nullptr, small_grad, entry_loss};
+  return launch_stream_split(desc, 0, false, &go, (cudaStream_t)stream);
 }
 
 extern "C" int d3r_align_reduce_block(int32_t n_imgs, int32_t n_edges, int64_t* offset_floats, int64_t* n_words) {

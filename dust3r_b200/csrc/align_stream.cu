@@ -23,7 +23,8 @@
 //
 // The last CTA of the grid (ticket) runs the same small-parameter step as the general kernel (align_common.cuh).  A split
 // iteration (align_stream_pixel_kernel + align_small_step_kernel) runs the same two halves as two launches, so that a
-// multi-GPU caller can all-reduce the accumulators between them.
+// multi-GPU caller can all-reduce the accumulators between them; the gradient export splits the same way
+// (align_stream_grad_pixel_kernel + align_grad_small_step_kernel).
 #include "align_common.cuh"
 
 namespace d3r {
@@ -276,11 +277,12 @@ __device__ __forceinline__ void adam_slots(const d3r_align_desc& D, const uint8_
   for (int v = 0; v < kImgVals; ++v) { float lo, hi; unpack2(S[v], lo, hi); s12[v] = lo + hi; }
 }
 
-// Body of all three instantiation families: kGrad = false is the training iteration (align_stream_kernel), kGrad = true the
+// Body of all four instantiation families: kGrad = false is the training iteration (align_stream_kernel), kGrad = true the
 // gradient export (align_stream_grad_kernel): its MV stage brings only the image row, writes dL/dlog-depth to go.logd_grad
-// and still forms the image sums; the last CTA runs small_grad_step.  kSplit (align_stream_pixel_kernel) is the training
-// iteration's pixel pass alone: partial-range overflow goes to ws.ovf, which travels with the sums, and every CTA leaves
-// where the grid ticket would be taken -- align_small_step_kernel runs the small step.
+// and still forms the image sums; the last CTA runs small_grad_step.  kSplit is the pixel pass alone, of the training
+// iteration (align_stream_pixel_kernel) or of the gradient export (align_stream_grad_pixel_kernel): partial-range overflow
+// goes to ws.ovf, which travels with the sums, and every CTA leaves where the grid ticket would be taken --
+// align_small_step_kernel / align_grad_small_step_kernel runs the small step.
 template <bool kGrad, bool kL2, int PPT, int NST, bool kSplit>
 __device__ __forceinline__ void stream_body(const d3r_align_desc& D, int it, const GradOut& go) {
   static_assert(PPT == 3, "the per-slot specialisations below are written for 3 slots per item");
@@ -478,6 +480,29 @@ align_stream_grad_kernel(const __grid_constant__ d3r_align_desc D, GradOut go) {
   stream_body<true, kL2, PPT, NST, false>(D, 0, go);
 }
 
+// The gradient export as a split launch (d3r_align_grad_pixel_pass + d3r_align_grad_small_step), so that a multi-GPU caller
+// can all-reduce the accumulators between the halves.  The pixel pass is align_stream_grad_kernel's body up to the grid ticket:
+// dL/dlog-depth of its items' pixels to go.logd_grad, the sums, partial-range overflow to ws.ovf.
+template <bool kL2, int PPT, int NST>
+__global__ void __launch_bounds__(kSThreads, 2)
+align_stream_grad_pixel_kernel(const __grid_constant__ d3r_align_desc D, GradOut go) {
+  stream_body<true, kL2, PPT, NST, true>(D, 0, go);
+}
+
+// Its second half: one CTA of a streaming CTA's blockDim, so that small_grad_step sums in the order of the fused launch's last
+// CTA, runs on the (all-reduced) accumulators; the overflow word joins the flag before any total is read and is then cleared.
+__global__ void __launch_bounds__(kSThreads, 2)
+align_grad_small_step_kernel(const __grid_constant__ d3r_align_desc D, GradOut go) {
+  __shared__ float s_red[40];
+  const Workspace ws = carve(D.workspace, D.n_imgs, D.n_edges);
+  // everything below reads what the pixel pass and the reduction wrote
+  pdl::sync_with_predecessor();
+  if (threadIdx.x == 0 && __ldcg(ws.ovf) != 0) *ws.flags = 1;
+  __syncthreads();
+  small_grad_step(D, ws, go, s_red);
+  if (threadIdx.x == 0) *ws.ovf = 0;
+}
+
 // ---- one launch packs every entry (device-resident forward output -> observation layout) ----------------------
 __device__ __forceinline__ float conf_trf(float c, int mode) {
   switch (mode) {
@@ -558,10 +583,11 @@ int launch_stream(const d3r_align_desc* desc, int it_begin, int it_end, const Gr
   return launch_iterations(kernel, desc, desc->stream_grid, kSThreads, smem, it_begin, it_end, st);
 }
 
-// One half of split iteration `it`: the pixel pass over this descriptor's items (none: nothing to launch), or the
-// one-CTA small step.
-int launch_stream_split(const d3r_align_desc* desc, int it, bool pixel, cudaStream_t st) {
-  const char* op = pixel ? "d3r_align_pixel_pass" : "d3r_align_small_step";
+// One half of split iteration `it` (go == nullptr) or of the split gradient launch: the pixel pass over this descriptor's
+// items (none: nothing to launch), or the one-CTA small step.
+int launch_stream_split(const d3r_align_desc* desc, int it, bool pixel, const GradOut* go, cudaStream_t st) {
+  const char* op = go ? (pixel ? "d3r_align_grad_pixel_pass" : "d3r_align_grad_small_step")
+                      : (pixel ? "d3r_align_pixel_pass" : "d3r_align_small_step");
   D3R_CHECK_ARG(desc->stream_kernel, "%s: the split iteration runs on the streaming kernel only", op);
   D3R_CHECK_ARG(desc->stream_ppt == 3, "%s: stream_ppt=%d is not built (3)", op, desc->stream_ppt);
   D3R_CHECK_ARG(desc->stream_window >= 1, "%s: stream_window must be >= 1", op);
@@ -570,11 +596,18 @@ int launch_stream_split(const d3r_align_desc* desc, int it, bool pixel, cudaStre
   const bool deep = depth == 4;
   const size_t smem = stream_smem_bytes(3, depth, desc->stream_window);
   if (!pixel) {
+    if (go) return launch_gradient(align_grad_small_step_kernel, desc, 1, kSThreads, smem, *go, st);
     void (*kernel)(d3r_align_desc, int) = deep ? align_small_step_kernel<3, 4> : align_small_step_kernel<3, 3>;
     return launch_iterations(kernel, desc, 1, kSThreads, smem, it, it + 1, st);
   }
   if (desc->n_items == 0) return D3R_OK;
   D3R_CHECK_ARG(desc->items && desc->warp_item_ptr && desc->stream_grid > 0, "%s: no work-item table", op);
+  if (go) {
+    void (*kernel)(d3r_align_desc, GradOut) =
+        desc->dist_l2 ? (deep ? align_stream_grad_pixel_kernel<true, 3, 4> : align_stream_grad_pixel_kernel<true, 3, 3>)
+                      : (deep ? align_stream_grad_pixel_kernel<false, 3, 4> : align_stream_grad_pixel_kernel<false, 3, 3>);
+    return launch_gradient(kernel, desc, desc->stream_grid, kSThreads, smem, *go, st);
+  }
   void (*kernel)(d3r_align_desc, int) = desc->dist_l2 ? (deep ? align_stream_pixel_kernel<true, 3, 4> : align_stream_pixel_kernel<true, 3, 3>)
                                                       : (deep ? align_stream_pixel_kernel<false, 3, 4> : align_stream_pixel_kernel<false, 3, 3>);
   return launch_iterations(kernel, desc, desc->stream_grid, kSThreads, smem, it, it + 1, st);

@@ -106,11 +106,14 @@ def global_aligner_sharded(dust3r_output, device, mode=None, group=None, **optim
     (cloud_opt/owned.py).  PairViewer needs every pair and is refused for such an output.
 
     Without an initialised process group, or in a group of one rank, this is global_aligner().  PairViewer has no loop
-    and is returned as global_aligner builds it.  On the returned scene compute_global_alignment (every init=), scene()
-    under no_grad, the getters, clean_pointcloud and mask_sky behave as on one GPU; the differentiable objective
-    (loss.backward(), ret_details=True) raises NotImplementedError.  With the full result every rank holds all the
-    predictions and only the packed observations and the per-pixel Adam state are divided; with the owned rows the
-    predictions are divided too."""
+    and is returned as global_aligner builds it.  On the returned scene compute_global_alignment (every init=), scene(),
+    the getters, clean_pointcloud and mask_sky behave as on one GPU, and so does the differentiable objective:
+    `loss = scene(); loss.backward()` fills every trainable parameter's .grad and ModularPointCloudOptimizer's
+    scene(ret_details=True) returns the per-edge losses.  scene() is a collective, as compute_global_alignment is: every
+    rank of the group calls it, it evaluates at rank 0's parameters, and every rank gets the same loss, details and .grad
+    (each rank's pixel pass covers its own images; one all-reduce of the sums, then one broadcast per owner of its images'
+    log-depth gradients).  With the full result every rank holds all the predictions and only the packed observations and
+    the per-pixel Adam state are divided; with the owned rows the predictions are divided too."""
     from .cloud_opt import GlobalAlignerMode, global_aligner
     mode = GlobalAlignerMode.PointCloudOptimizer if mode is None else mode
     owned = dust3r_output.get('owned') if isinstance(dust3r_output, dict) else None

@@ -181,6 +181,22 @@ int d3r_align_pixel_pass(const d3r_align_desc* desc, int32_t it, void* stream);
 int d3r_align_small_step(const d3r_align_desc* desc, int32_t it, void* stream);
 /* *offset_floats: where the all-reduce block starts in `workspace` (in floats, 16-byte aligned); *n_words: its length in int64. */
 int d3r_align_reduce_block(int32_t n_imgs, int32_t n_edges, int64_t* offset_floats, int64_t* n_words);
+/* d3r_align_loss_grad (below) as two launches around the same all-reduce of the d3r_align_reduce_block block:
+ *   d3r_align_grad_pixel_pass(desc, logd_grad)   the gradient launch's per-pixel work over desc's items: dL/dlog-depth of
+ *                                                their pixels to logd_grad (other pixels are not written: pass a zeroed
+ *                                                buffer), the sums, and the overflow word -- nothing is launched when
+ *                                                n_items == 0;
+ *   all-reduce(SUM) of the block (optional: one GPU needs none);
+ *   d3r_align_grad_small_step(desc, small_grad, entry_loss)   the gradient launch's last-CTA step on the (reduced) sums:
+ *                                                loss -> desc->loss_out[0], small_grad, entry_loss (may be NULL).
+ * Streaming kernel only (stream_kernel = 1).  The contract is d3r_align_loss_grad's: no parameter or Adam moment is touched
+ * (logd_m, logd_v, small_m, small_v, small_trainable and sched may be NULL), the accumulators and the overflow word are left
+ * cleared, the small step sets the overflow flag, and when it is set loss_out[0], every element of small_grad and of
+ * entry_loss are NaN.  On one GPU the pair gives the bits of d3r_align_loss_grad; on several, each GPU's pixel pass writes
+ * the log-depth gradients of its own items' images, and every GPU's small step computes the same loss and small_grad.
+ * Asynchronous. */
+int d3r_align_grad_pixel_pass(const d3r_align_desc* desc, float* logd_grad, void* stream);
+int d3r_align_grad_small_step(const d3r_align_desc* desc, float* small_grad, float* entry_loss, void* stream);
 /* Objective and its gradient at the current parameters (net.forward() + loss.backward()): one launch of the pixel kernel
  * the descriptor selects + the last-CTA small step.  Updates no parameter or Adam moment; reads neither sched nor the moments
  * (logd_m, logd_v, small_m, small_v, small_trainable and sched may be NULL).  Call d3r_align_prepare first when `small` changed.
@@ -194,7 +210,8 @@ int d3r_align_reduce_block(int32_t n_imgs, int32_t n_edges, int64_t* offset_floa
 int d3r_align_loss_grad(const d3r_align_desc* desc, float* logd_grad, float* small_grad, float* entry_loss, void* stream);
 /* Cross-CTA sums use order-independent 2^40 fixed-point integer atomics (bit-reproducible).  *host_out = 1 when a
  * partial sum (|x| >= 2^18) or a total (|x| >= 2^22) left the supported range (unreasonably scaled scene, NaN / Inf input)
- * since iteration 0 of the current d3r_align_run batch (or of the split iterations), or during the last d3r_align_loss_grad.  Every iteration from the one
+ * since iteration 0 of the current d3r_align_run batch (or of the split iterations), or during the last d3r_align_loss_grad
+ * (or d3r_align_grad_pixel_pass + d3r_align_grad_small_step).  Every iteration from the one
  * that set it writes NaN to loss_out (eval_only runs included). */
 int d3r_align_overflow_flag(const d3r_align_desc* desc, int32_t* host_out, void* stream);
 /* World-frame pointmaps X[i] = R_i * unproject(depth_i) + T_i for every image

@@ -9,7 +9,12 @@ Prints one JSON line per config from rank 0: iterations/s of the fused loop on r
 at world N; the per-iteration split of the sharded loop into pixel pass, all-reduce and small step (CUDA events, in a run
 of its own); the packed observation bytes of every rank and the max / mean ratio; and, for config 5, the end to end time of
 inference_sharded + sharded alignment.  At N = 1 the sharded loop is the split iteration with a one-rank all-reduce: what
-the split costs against the fused launch.  The card, its power limit and clocks are read in the same run."""
+the split costs against the fused launch.
+
+The gradient leg (--grad-iters, 0 skips it): host-synchronised wall ms per `loss = scene(); loss.backward()` on the fused
+scene on rank 0's GPU alone (one d3r_align_loss_grad launch) and on the sharded scene at world N (sharded_loss_and_grad), and,
+in a run of its own, the CUDA-event split of the sharded call into gradient pixel pass, all-reduce, gradient small step and
+the log-depth-gradient broadcasts.  The card, its power limit and clocks are read in the same run."""
 import argparse
 import ctypes
 import json
@@ -22,7 +27,7 @@ import torch
 import torch.distributed as dist
 
 from bench import build_model
-from common import barrier_sync, card
+from common import barrier_sync, card, wall_ms
 from dust3r_b200 import _lib
 from dust3r_b200.cloud_opt import GlobalAlignerMode, global_aligner
 from dust3r_b200.distributed import _AlignShard, global_aligner_sharded, inference_sharded, shard_images
@@ -78,11 +83,58 @@ def split_breakdown(eng, niter):
     return dict(pixel_pass_ms=round(parts[0], 4), all_reduce_ms=round(parts[1], 4), small_step_ms=round(parts[2], 4))
 
 
+def fwd_bwd(scene):
+    scene.zero_grad(set_to_none=True)
+    scene().backward()
+
+
+def timed_ms(fn, iters):
+    """Wall ms per call of the collective `fn` on every rank: host clock between two barriers after device synchronises."""
+    fn()
+    barrier_sync()
+    t0 = time.perf_counter()
+    for _ in range(iters):
+        fn()
+    barrier_sync()
+    return 1e3 * (time.perf_counter() - t0) / iters
+
+
+def grad_breakdown(eng, iters):
+    """Mean ms of the gradient pixel pass, the all-reduce, the gradient small step and the log-depth-gradient broadcasts of
+    one sharded_loss_and_grad (CUDA events around each, the same launches and collectives in the same order)."""
+    with torch.cuda.device(eng.device):
+        eng._sync_start()
+        eng.prepare()
+    d = eng._desc()
+    loss = torch.zeros((), dtype=torch.float32, device=eng.device)
+    d.loss_out = loss.data_ptr()
+    logd_grad = torch.zeros_like(eng.logd)
+    small_grad = torch.empty((eng.n_small,), dtype=torch.float32, device=eng.device)
+    ev = [[torch.cuda.Event(enable_timing=True) for _ in range(5)] for _ in range(iters)]
+    barrier_sync()
+    for it in range(iters):
+        ev[it][0].record()
+        if eng.n_items:
+            _lib.launch(eng.device, 'd3r_align_grad_pixel_pass', ctypes.byref(d), logd_grad.data_ptr())
+        ev[it][1].record()
+        dist.all_reduce(eng._reduce, op=dist.ReduceOp.SUM)
+        ev[it][2].record()
+        _lib.launch(eng.device, 'd3r_align_grad_small_step', ctypes.byref(d), small_grad.data_ptr(), None)
+        ev[it][3].record()
+        eng._sync_end(logd_grad)
+        ev[it][4].record()
+    barrier_sync()
+    parts = [sum(ev[it][k].elapsed_time(ev[it][k + 1]) for it in range(iters)) / iters for k in range(4)]
+    return dict(grad_pixel_pass_ms=round(parts[0], 4), grad_all_reduce_ms=round(parts[1], 4),
+                grad_small_step_ms=round(parts[2], 4), grad_broadcasts_ms=round(parts[3], 4))
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument('--niter', type=int, default=300)
     ap.add_argument('--no-e2e', action='store_true')
     ap.add_argument('--configs', default='5,3')
+    ap.add_argument('--grad-iters', type=int, default=20, help='calls per timing of the gradient leg (0: no gradient leg)')
     ap.add_argument('--out', default=None, help='also write the results of every config to this JSON file')
     args = ap.parse_args()
 
@@ -110,6 +162,8 @@ def main():
             torch.cuda.synchronize()
             dt = time.perf_counter() - t0
             res.update(fused_1gpu_s=round(dt, 4), fused_1gpu_it_per_s=round(args.niter / dt, 1), fused_final_loss=loss)
+            if args.grad_iters:
+                res.update(grad_fused_1gpu_ms=round(wall_ms(lambda: fwd_bwd(scene), args.grad_iters, 2), 4))
             del scene
             torch.cuda.empty_cache()
         barrier_sync()
@@ -122,6 +176,10 @@ def main():
                    shards=[o[0] for o in obs], obs_bytes_per_rank=[o[1] for o in obs],
                    obs_bytes_max_over_mean=round(max(o[1] for o in obs) / (sum(o[1] for o in obs) / world), 4))
         res.update(split_breakdown(eng, args.niter))
+        if args.grad_iters:
+            fwd_bwd(scene)
+            res.update(grad_sharded_ms=round(timed_ms(lambda: fwd_bwd(scene), args.grad_iters), 4))
+            res.update(grad_breakdown(eng, args.grad_iters))
         del scene, eng
         torch.cuda.empty_cache()
         if key == '5' and not args.no_e2e:
